@@ -1,4 +1,4 @@
-"""ezaudio_b200 -- B200-native (sm_100a) implementation of EzAudio's DiT-denoise + VAE-decode hot path.
+"""ezaudio_b200 -- H100-native (sm_90a) implementation of EzAudio's DiT-denoise + VAE-decode hot path.
 
 Python host code mirrors the reference's call surface (api/ezaudio.py, api/controlnet.py,
 src/models/conditioners.py::MaskDiT, src/modules/autoencoder_wrapper.py::Autoencoder) and calls

@@ -1,4 +1,4 @@
-"""Builds libezb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libezb200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libezb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
          "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -28,7 +28,7 @@ def needs_build() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return LIB
-    dbg = ["-DEZB_GEMM_DEBUG"] if os.environ.get("EZB_DEBUG") else []  # cycle counters in the GEMM / attention kernels
+    dbg = ["-DEZB_GEMM_DEBUG"] if os.environ.get("EZB_DEBUG") else []  # cycle counters in the GEMM kernel (ezb_debug_read)
     cmd = [NVCC] + FLAGS + dbg + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB] + sources() + ["-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or r.returncode != 0:

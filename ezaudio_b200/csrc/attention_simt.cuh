@@ -1,6 +1,6 @@
 // fp32 CUDA-core attention: softmax(q k^T * scale [+ bias] [+ key mask]) v   (attention.py:107-110, mask attention.py:30-37;
 // with scale 1 and a relative-position bias: T5Attention).
-// Used by the bf16x3 parity mode (fp32-grade numerics) and as the on-device comparator of the tcgen05 kernel.
+// Used by the bf16x3 parity mode (fp32-grade numerics) and as the on-device comparator of the tensor-core kernel.
 // q,k,v fp32 [B,H,L,dh]; out bf16 [B, Lq, H*dh] token-major (A operand of the output projection).
 #pragma once
 #include "elementwise.cuh"

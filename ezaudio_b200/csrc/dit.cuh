@@ -7,9 +7,7 @@
 #include <vector>
 
 #include "attention_simt.cuh"
-#include "attention_tc4.cuh"
-#include "attention_tc6.cuh"
-#include "attention_tc7.cuh"
+#include "attention_mma.cuh"
 #include "host.cuh"
 #include "gemm_ln.cuh"
 
@@ -83,7 +81,7 @@ struct Dit {
   float2* rope_cs = nullptr;
   float h_inv_freq[48] = {};
   bool fused_heads = false;
-  bool pair = true;       // CTA-pair (cta_group::2) GEMMs
+  bool pair = true;       // 2-CTA cluster GEMMs sharing the weight tile (host.cuh gemm2)
   bool swap_ab = true;    // swap-AB tiles for the fp32-output N = D layers
   // LayerNorm folded into the neighbouring GEMMs (fast mode, uniform timestep): see gemm.cuh
   bool fold_cfg = false;  // handle built with the fold tables / buffers
@@ -615,7 +613,7 @@ struct Dit {
       return gemm2<224, EpiHeads<72, 3, false, false, true>>(*dev, st, A, D, W, D, M, H * 224, D, e);
     }
     if (qkv3_bn > 0 && N == 3 * D) {  // packed self-attention QKV: three heads per tile
-      if (dh == 72 && (opt_ksub2() & 2) && !fo) return gemm2<224, EpiHeads<72, 3, true, false>, 2>(*dev, st, A, D, W, D, M, H * 224, D, e);   // 128-deep stages (needs the staging-free epilogue)
+      if (dh == 72 && (opt_ksub2() & 2) && !fo) return gemm2<224, EpiHeads<72, 3, true, false>, 2>(*dev, st, A, D, W, D, M, H * 224, D, e);   // 128-deep slots (needs the staging-free epilogue)
       if (dh == 72) return EZB_HEADS(224, 72, 3, H * 224);
       return EZB_HEADS(192, 64, 3, H * 192);
     }
@@ -651,9 +649,7 @@ struct Dit {
       EZB_CUDA(cudaGetLastError());
       return EZB_OK;
     }
-    if (opt_attn7()) return attention_tc7(*dev, st, q16_, k16_, vt16_, mask, attn_out, B, H, Lq, Lk, Lkpad, dh, DHP, DVP, scale);
-    if (opt_attn6() & 1) return attention_tc6(*dev, st, q16_, k16_, vt16_, mask, attn_out, B, H, Lq, Lk, Lkpad, dh, DHP, DVP, scale);
-    return attention_tc4(*dev, st, q16_, k16_, vt16_, mask, attn_out, B, H, Lq, Lk, Lkpad, dh, DHP, DVP, scale);
+    return attention_mma(*dev, st, q16_, k16_, vt16_, mask, attn_out, B, H, Lq, Lk, Lkpad, dh, DHP, DVP, scale);
   }
 
   // ---------------------------------------------------------------- step-invariant precompute
@@ -855,11 +851,11 @@ struct Dit {
       }
       if (opt_skip() & 16) {}
       else if (geglu_bn == 256 && fc.on) EZB_TRY((gemm2<256, EpiGeglu<256, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
-      else if (geglu_bn == 256 && (opt_ksub2() & 1) && kmul == 1) EZB_TRY((gemm2<256, EpiGeglu<256>, 2>(*dev, st, act, D, w.mlp1, D, M, 2 * inner, D, g)));   // 128-deep stages
+      else if (geglu_bn == 256 && (opt_ksub2() & 1) && kmul == 1) EZB_TRY((gemm2<256, EpiGeglu<256>, 2>(*dev, st, act, D, w.mlp1, D, M, 2 * inner, D, g)));   // 128-deep slots
       else if (geglu_bn == 256) EZB_TRY((gemm2<256, EpiGeglu<256>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       else if (fc.on) EZB_TRY((gemm<128, EpiGeglu<128, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       else EZB_TRY((gemm<128, EpiGeglu<128>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
-      if (opt_mlp2_pair() && pair && kmul == 1 && !fc.on)   // MLP-out on CTA-pair tiles (256 tokens x 128 features, thread = token row) instead of swap-AB
+      if (opt_mlp2_pair() && pair && kmul == 1 && !fc.on)   // MLP-out on 2-CTA cluster tiles (128 tokens x 128 features, thread = token row) instead of swap-AB
         EZB_TRY((gemm2<128, EpiLinear<128>>(*dev, st, mid, inner, w.mlp2, inner, M, D, inner, e)));
       else
       EZB_TRY(lin(st, mid, inner, w.mlp2, M, D, e, fc.on ? nullptr : next_ln, next_done));

@@ -397,8 +397,8 @@ __global__ void patch_pack_kernel(const float* __restrict__ x, const float* __re
 // FinalBlock tail (blocks.py:207-211): y [B*L, C] token-major -> unpatchify (transpose) -> Conv1d(C, C, k=3, pad=1).
 // w packed [3][Cin][Cout].  CTA = 32 positions x all C = 128 output channels, 512 threads = 4 input-channel groups x 128; within a group
 // thread = 4 output channels x 8 positions, so one input channel costs 10 broadcast LDS + 3 coalesced float4 weight loads for 96 FMAs; the four
-// groups' partial sums meet in shared memory.  (Round 1: one dependent global weight load per (tap, channel), 211 us; round 2a: 128 threads
-// walking all 128 input channels, 62.5 us per step -- four warps per SM cannot hide the L2 latency of the weight loads; this one: 16 warps.)
+// groups' partial sums meet in shared memory.  (Four warps per SM walking all 128 input channels cannot hide the L2 latency of the weight
+// loads; this one: 16 warps.)
 constexpr int FC_GROUPS = 4;
 __global__ void __launch_bounds__(128 * FC_GROUPS) final_conv_kernel(const float* __restrict__ y, const float* __restrict__ wp, const float* __restrict__ bias,
                                                                      float* __restrict__ out, int B, int C, int L) {
@@ -503,7 +503,7 @@ __global__ void __launch_bounds__(256) small_linear_kernel(const float* __restri
 }
 
 // RoPE table (rotary.py:48-70): cs[l][i] = (cos, sin)(l * inv_freq[i]), fp32, i < dh/2 (token-major: a thread reads its
-// token's dh/2 pairs as 9 full 32-byte sectors; the frequency-major alternative measured slower, profiles/r1)
+// token's dh/2 pairs as 9 full 32-byte sectors; the frequency-major alternative is strided)
 __global__ void rope_table_kernel(const float* __restrict__ inv_freq, float2* __restrict__ cs, int L, int half) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L * half) return;
@@ -580,7 +580,7 @@ __global__ void permute3_kernel(const float* __restrict__ src, float* __restrict
 // ---------------------------------------------------------------------------------------------------------------
 // Classifier-free guidance + rescale (src/inference.py:12-23,88-93) fused with the DDIM v-prediction update
 // (diffusers DDIMScheduler.step, SURVEY Appendix B).  coef = {sqrt(a), sqrt(1-a), sqrt(a_prev), sqrt(1-a_prev-sigma^2), sigma}.
-// One CLUSTER of CFG_CLUSTER CTAs per sample (the first version ran one CTA per sample: 4 of 148 SMs busy, 77 us per step):
+// One CLUSTER of CFG_CLUSTER CTAs per sample (one CTA per sample would leave all but a handful of SMs idle):
 // every CTA reduces the four sums of its slice (double accumulation, fixed order -> deterministic), the partials are exchanged
 // through distributed shared memory, every CTA forms the same ratio and updates its slice.
 constexpr int CFG_CLUSTER = 8;

@@ -13,7 +13,8 @@ namespace {
 Device& device_ctx(int device) {
   static Device devs[16];
   Device& d = devs[device & 15];
-  if (d.num_sms == 148 && d.id == 0 && device >= 0) {
+  if (!d.queried && device >= 0) {
+    d.queried = true;
     int sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && sms > 0) d.num_sms = sms;
     d.id = device;
@@ -54,8 +55,8 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
     if (opt_swap_mc()) return gemm_swapped_mc<EpiLinearT<256>, 3>(dev, st, a, lda, w, ldw, M, N, K, p);
     return gemm_swapped<EpiLinearT<256>>(dev, st, a, lda, w, ldw, M, N, K, p);
   }
-  if (epi_kind == 10 || epi_kind == 11) {  // CTA-pair kernel (bn is the pair tile's N)
-    if (cp) return fail(EZB_ERR_UNSUPPORTED, "pair GEMM has no conv addressing");
+  if (epi_kind == 10 || epi_kind == 11) {  // 2-CTA cluster kernel with the W tile multicast (bn is the tile's N)
+    if (cp) return fail(EZB_ERR_UNSUPPORTED, "cluster GEMM has no conv addressing");
     if (epi_kind == 10) {
       EpiLinearParams p = to_epi(e);
       if (bn == 128) return gemm2<128, EpiLinear<128>>(dev, st, a, lda, w, ldw, M, N, K, p);
@@ -233,7 +234,7 @@ EZB_API int ezb_vae_decode(ezb_vae* h, const float* z, float* wav, int B, int L,
   if (!h || !z || !wav) return fail(EZB_ERR_ARG, "ezb_vae_decode: null argument");
   return reinterpret_cast<Vae*>(h)->decode(z, wav, B, L, ST(stream));
 }
-// impl 0: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]); impl 1: tcgen05 kernel (q,k bf16 [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad])
+// impl 0: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]); impl 1/4/6/7 (+100): tensor-core kernel (q,k bf16 [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad])
 EZB_API int ezb_test_attention(int device, const void* q, const void* k, const void* v, const uint8_t* key_mask, void* out, int B, int H, int Lq,
                                int Lk, int dh, int impl, void* stream) {
   if (!q || !k || !v || !out) return fail(EZB_ERR_ARG, "ezb_test_attention: null pointer");
@@ -250,18 +251,14 @@ EZB_API int ezb_test_attention(int device, const void* q, const void* k, const v
     EZB_CUDA(cudaGetLastError());
     return EZB_OK;
   }
-  // impl 1 / 5: q, k rows of `dhp` elements: 64-multiple (round-1 layout) or, with impl >= 100 (impl - 100 = kernel), 80 for dh = 72
-  int dhp = (dh + 63) / 64 * 64;
-  if (impl >= 100) { impl -= 100; if (dh == 72) dhp = 80; }
+  // impl 1: the variant the options select; 4 / 6 / 7: that generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's
+  // layout) instead of a 64-multiple
+  const int variant = impl % 100, row80 = impl >= 100;
+  if (variant != 1 && variant != 4 && variant != 6 && variant != 7) return fail(EZB_ERR_ARG, "ezb_test_attention: impl %d", impl);
+  const int dhp = (row80 && dh == 72) ? 80 : (dh + 63) / 64 * 64;
   const int dvp = (dh + 15) / 16 * 16, lkpad = (Lk + 7) / 8 * 8;
-  if (impl == 7 || (impl == 1 && opt_attn7()))
-    return attention_tc7(device_ctx(device), ST(stream), reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                         reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale);
-  if (impl == 6 || (impl == 1 && (opt_attn6() & 1)))
-    return attention_tc6(device_ctx(device), ST(stream), reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                         reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale);
-  return attention_tc4(device_ctx(device), ST(stream), reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                       reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale);
+  return attention_mma(device_ctx(device), ST(stream), reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
+                       reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale, variant == 1 ? 0 : variant);
 }
 
 
@@ -278,12 +275,18 @@ EZB_API int ezb_set_option(const char* name, int value) {
   if (name && !strcmp(name, "mlp2_pair")) { opt_mlp2_pair() = value; return EZB_OK; }
   if (name && !strcmp(name, "cq_single")) { opt_cq_single() = value; return EZB_OK; }
   if (name && !strcmp(name, "ksub2")) { opt_ksub2() = value; return EZB_OK; }
-  if (name && !strcmp(name, "attn_res")) { opt_attn_res() = value; return EZB_OK; }
-  if (name && !strcmp(name, "attn_pp")) { opt_attn_pp() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn6")) { opt_attn6() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn7")) { opt_attn7() = value; return EZB_OK; }
-  if (name && !strcmp(name, "w_prefetch")) { opt_w_prefetch() = value; return EZB_OK; }
+  if (name && !strcmp(name, "attn_res")) { opt_attn_res() = value; return EZB_OK; }
+  if (name && !strcmp(name, "attn_pp")) { opt_attn_pp() = value; return EZB_OK; }
+  if (name && !strcmp(name, "gemm_debug")) {  // cycle counters of CTA 0 of every 2-CTA cluster GEMM launch (accumulated; needs -DEZB_GEMM_DEBUG)
+    if (value && !gemm_dbg_buf()) { EZB_CUDA(cudaMalloc(&gemm_dbg_buf(), 64)); EZB_CUDA(cudaMemset(gemm_dbg_buf(), 0, 64)); }
+    if (!value && gemm_dbg_buf()) { cudaFree(gemm_dbg_buf()); gemm_dbg_buf() = nullptr; }
+    return EZB_OK;
+  }
+  if (name && !strcmp(name, "attn_poly")) { opt_attn_poly() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn_dbg")) { opt_attn_dbg() = value; return EZB_OK; }
+  if (name && !strcmp(name, "w_prefetch")) { opt_w_prefetch() = value; return EZB_OK; }
   if (name && !strcmp(name, "ln_variant")) { opt_ln_variant() = value; return EZB_OK; }
   if (name && !strcmp(name, "mlp_fused")) { opt_mlp_fused() = value; return EZB_OK; }
   if (name && !strcmp(name, "heads_direct")) { opt_heads_direct() = value; return EZB_OK; }
@@ -291,13 +294,7 @@ EZB_API int ezb_set_option(const char* name, int value) {
   if (name && !strcmp(name, "ln_fold")) { opt_fold() = value; return EZB_OK; }
   if (name && !strcmp(name, "skip")) { opt_skip() = value; return EZB_OK; }
   if (name && !strcmp(name, "swap_mc")) { opt_swap_mc() = value; return EZB_OK; }
-  if (name && !strcmp(name, "attn_poly")) { opt_attn_poly() = value; return EZB_OK; }
   if (name && !strcmp(name, "rope_mufu")) { opt_rope_mufu() = value; return EZB_OK; }
-  if (name && !strcmp(name, "gemm_debug")) {  // cycle counters of CTA 0 of every pair-GEMM launch (accumulated)
-    if (value && !gemm_dbg_buf()) { EZB_CUDA(cudaMalloc(&gemm_dbg_buf(), 64)); EZB_CUDA(cudaMemset(gemm_dbg_buf(), 0, 64)); }
-    if (!value && gemm_dbg_buf()) { cudaFree(gemm_dbg_buf()); gemm_dbg_buf() = nullptr; }
-    return EZB_OK;
-  }
   return fail(EZB_ERR_ARG, "unknown option");
 }
 EZB_API int ezb_debug_read(unsigned long long* out8) {

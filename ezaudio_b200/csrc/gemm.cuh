@@ -1,10 +1,11 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a:  C[M,N] = A[M,K] * W[N,K]^T  (bf16 in, fp32 accumulate in TMEM)
+// Persistent warp-specialised wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * W[N,K]^T  (bf16 in, fp32 accumulate)
 //
-//   warp 0      TMA producer   : cp.async.bulk.tensor tiles of A (128 x 64) and W (BN x 64) into a STAGES-deep smem ring
-//   warp 1      MMA issuer     : one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16) x4 per stage,
-//                                tcgen05.commit releases the smem slot / publishes the accumulator
-//   warps 2..5  epilogue       : tcgen05.ld the 128 x BN fp32 accumulator (thread == output row), fused epilogue, global stores
-//   TMEM holds two accumulator stages (2 x BN columns) so the epilogue of tile i overlaps the mainloop of tile i+1.
+//   last warp           TMA producer : cp.async.bulk.tensor tiles of A (128 x 64) and W (BN x 64) into a STAGES-deep smem ring
+//   warpgroups 0..      consumers    : the first one or two warpgroups issue wgmma.mma_async m64nBNk16 (accumulator in registers,
+//                                      64 rows per warpgroup; a single MMA warpgroup takes both 64-row halves), release each ring
+//                                      slot once its MMAs have completed, then park the finished 128 x BN fp32 tile in shared memory
+//                                      (over the ring, which is idle then); every consumer warp runs the fused epilogue on 32 rows
+//                                      (thread == row) of it.  The producer refills the ring for the next tile once the epilogue is done.
 //
 // A can also be addressed as an implicit-GEMM operand of a 1-D convolution over channels-last activations
 // [B, T, C]: k-block kb -> tap = kb / cin_blocks, rows shifted by (tap - center) * dilation with TMA zero fill at
@@ -34,10 +35,10 @@ struct GemmShape {
   // implicit-conv addressing of A (taps == 0 -> plain 2-D A[M,K])
   int taps, center, dilation, cin_blocks, T, tiles_per_batch;
   int stride, pad;     // stride > 1: strided conv (VAE encoder): A is a 4-D map [B, T/stride, stride, C], tap k reads row q*stride + k - pad
-  unsigned long long* dbg;  // optional cycle counters (CTA 0): [0] mma wait full, [1] mma wait tempty, [2] producer wait empty,
-                            // [3] epilogue warp 2 wait tfull, [4] epilogue warp 2 busy, [5] total
+  unsigned long long* dbg;  // optional cycle counters of CTA 0 (builds with -DEZB_GEMM_DEBUG): [0] warpgroup 0 mainloop incl. its full-slot waits,
+                            // [1] consumer wait for the accumulator tile, [2] producer wait for empty slots, [3] unused, [4] warp 0 epilogue, [5] total
   // L2 prefetch of the weights the NEXT GEMM of the step will stream (host.cuh WeightSeq): every layer's weights are read once per step,
-  // i.e. from HBM, and a kernel's first k-blocks pay that latency on top of its ramp (GEGLU: 58 us with L2-resident weights, 68.6 us in situ).
+  // i.e. from HBM, and a kernel's first k-blocks pay that latency on top of its ramp.
   const char* pf;
   unsigned int pf_bytes;    // multiple of 16
 };
@@ -126,7 +127,24 @@ struct EpiLinearParams {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// Epilogue staging: a warp reads its 32 accumulator rows from TMEM (thread == row), transposes 64-column chunks through
+// The finished accumulator tile in shared memory, as an epilogue warp sees it: its 32 rows (row = lane), fp32, `pitch` floats apart.
+// pitch = BN + 4 keeps the 16-byte row reads of 8 consecutive lanes on distinct banks.
+struct AccRows {
+  const float* base;
+  int pitch;
+};
+template <int N>
+__device__ __forceinline__ void acc_ld(const AccRows& a, int col, int lane, uint32_t* r) {
+  const float4* p = reinterpret_cast<const float4*>(a.base + lane * a.pitch + col);
+#pragma unroll
+  for (int i = 0; i < N / 4; ++i) {
+    const float4 v = p[i];
+    r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y); r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Epilogue staging: a warp reads its 32 accumulator rows (thread == row), transposes 64-column chunks through
 // a private 8 KB smem tile (XOR-swizzled 8-byte granules: conflict-free both ways) and then works with lane == column
 // pair, so every global access is a fully coalesced 128/256-byte row segment.
 constexpr int EPI_STAGE_FLOATS = 32 * 64;
@@ -226,12 +244,12 @@ __device__ __forceinline__ void rows_generic(const EpiLinearParams& ep, const Ro
 template <int BN>
 struct EpiLinear {
   using Params = EpiLinearParams;
-  static constexpr int EPI_WARPS = BN >= 128 ? 8 : 4;       // two warps per TMEM lane group split the tile's columns
+  static constexpr int EPI_WARPS = BN >= 128 ? 8 : 4;       // two warps per 32-row group split the tile's columns
   static constexpr int STAGE_FLOATS = EPI_STAGE_FLOATS;
   // row0: global row of this warp's first accumulator row; nvalid: rows of the 32 that exist (<= 0: none);
   // [c_begin, c_end): this warp's column range inside the tile; wait(): blocks until the accumulator is complete.
   template <class Wait>
-  static __device__ __forceinline__ void run(const Params& ep, float* st, uint32_t taddr_row, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
                                              int c_end, Wait wait) {
     const int nv = nvalid < 32 ? nvalid : 32;
     bool waited = false;
@@ -268,8 +286,7 @@ struct EpiLinear {
 #pragma unroll
       for (int hc = 0; hc < 2; ++hc) {  // two 32-column halves: 32 accumulator registers live next to the 64 prefetched residual values (one 64-wide
         uint32_t r[32];                 // load spilled 780 bytes per thread under the 168-register cap of this 320-thread CTA)
-        tmem_ld_32x32(taddr_row + c + 32 * hc, r);
-        tmem_ld_wait();
+        acc_ld<32>(ar, c + 32 * hc, lane, r);
 #pragma unroll
         for (int g = 0; g < 16; ++g) stage_put(st, lane, 16 * hc + g, __uint_as_float(r[2 * g]), __uint_as_float(r[2 * g + 1]));
       }
@@ -340,7 +357,7 @@ struct EpiGeglu {
   static constexpr int EPI_WARPS = BN == 256 ? 8 : 4;   // 8 warps: each takes 64 of the tile's 128 output features
   static constexpr int STAGE_FLOATS = 32 * 32;          // 64 packed bf16 per row
   template <class Wait>
-  static __device__ __forceinline__ void run(const Params& ep, float* st, uint32_t taddr_row, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
                                              int c_end, Wait wait) {
     constexpr bool fold = FOLD;
     float rstd = 1.f, nmr = 0.f;
@@ -356,9 +373,8 @@ struct EpiGeglu {
 #pragma unroll 1
         for (int q4 = 0; q4 < 2; ++q4) {
           __syncwarp();
-          tmem_ld_32x32(taddr_row + c + q4 * 32, h);
-          tmem_ld_32x32(taddr_row + HALF + c + q4 * 32, g);
-          tmem_ld_wait();
+          acc_ld<32>(ar, c + q4 * 32, lane, h);
+          acc_ld<32>(ar, HALF + c + q4 * 32, lane, g);
           if (lane < nvalid) {
             __nv_bfloat16* o = ep.out_bf16 + (size_t)(row0 + lane) * ep.ld16 + (n0 / 2 + c + q4 * 32);
 #pragma unroll
@@ -376,9 +392,8 @@ struct EpiGeglu {
       for (int q4 = 0; q4 < 2; ++q4) {
         uint32_t h[32], g[32];
         __syncwarp();
-        tmem_ld_32x32(taddr_row + c + q4 * 32, h);
-        tmem_ld_32x32(taddr_row + HALF + c + q4 * 32, g);
-        tmem_ld_wait();
+        acc_ld<32>(ar, c + q4 * 32, lane, h);
+        acc_ld<32>(ar, HALF + c + q4 * 32, lane, g);
         if (fold) {   // warp-uniform: h = rstd * acc - rstd * mu * u + (v + bias)
           const float* bh = ep.fin.v + n0 + c + q4 * 32;
           const float* bg = ep.fin.v + n0 + HALF + c + q4 * 32;
@@ -420,10 +435,9 @@ struct EpiGeglu {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// Transposed ("swap-AB") linear epilogue.  For N_out = 1152-wide layers the natural 128/144-column tiles leave the tensor
-// pipe ~55 % efficient (operand bytes per flop) and a 256-column tile does not divide 1152.  Computing C^T = W A^T instead
-// puts the 1152 output features on the accumulator ROWS (9 tiles of 128) and 256 tokens on the columns: 144 tiles of
-// 128 x 256 = one full wave on 148 SMs.  A thread now owns one output feature; for a given token the 32 lanes of a warp hold
+// Transposed ("swap-AB") linear epilogue.  For N_out = 1152-wide layers the natural 128/144-column tiles spend more operand
+// bytes per flop and a 256-column tile does not divide 1152.  Computing C^T = W A^T instead puts the 1152 output features on the
+// accumulator ROWS (9 tiles of 128) and 256 tokens on the columns (the widest wgmma tile).  A thread now owns one output feature; for a given token the 32 lanes of a warp hold
 // 32 consecutive features, so residual loads and stores are 128-byte coalesced without any staging.
 template <int BN>
 struct EpiLinearT {
@@ -437,7 +451,7 @@ struct EpiLinearT {
     for (int j = 0; j < 32; ++j) x[j] = (f_ok && j < nt) ? ep.resid[(size_t)(t0 + j) * ep.ldr + f] : 0.f;
   }
   template <class Wait>
-  static __device__ __forceinline__ void run(const Params& ep, float* st, uint32_t taddr_row, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
                                              int c_end, Wait wait) {
     const int f = row0 + lane;                 // output feature of this thread
     const bool f_ok = lane < nvalid;
@@ -466,8 +480,7 @@ struct EpiLinearT {
       if (!waited) { wait(); waited = true; }
       uint32_t r[32];
       __syncwarp();
-      tmem_ld_32x32(taddr_row + c, r);
-      tmem_ld_wait();
+      acc_ld<32>(ar, c, lane, r);
       if (f_ok) {
         float* o = ep.out_f32 + (size_t)t0 * ep.ld32 + f;
 #pragma unroll
@@ -488,14 +501,14 @@ struct EpiLinearT {
 };
 
 // Fold-capable variant (LayerNorm folded in / out, see FoldIn / FoldOut).  Kept apart from EpiLinearT on purpose: the extra outputs and the
-// warp transposes cost this one-wave kernel ~19 us per launch (measured, profiles/r2), more than the LayerNorm pass they replace.
+// warp transposes lengthen this epilogue, which matters when the LayerNorm is not folded.
 template <int BN>
 struct EpiLinearTF {
   using Params = EpiLinearParams;   // bias/gate indexed by feature, resid/out_f32 [token, feature]; bf16/act/split unsupported
   static constexpr int EPI_WARPS = 8;
   static constexpr int STAGE_FLOATS = 0;
   template <class Wait>
-  static __device__ __forceinline__ void run(const Params& ep, float* st, uint32_t taddr_row, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
                                              int c_end, Wait wait) {
     const int f = row0 + lane;                 // output feature of this thread
     const bool f_ok = lane < nvalid;
@@ -531,8 +544,7 @@ struct EpiLinearTF {
       if (!waited) { wait(); waited = true; }
       uint32_t r[32];
       __syncwarp();
-      tmem_ld_32x32(taddr_row + c, r);
-      tmem_ld_wait();
+      acc_ld<32>(ar, c, lane, r);
       float val[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -582,150 +594,205 @@ struct EpiLinearTF {
   }
 };
 
-// KSUB: 64-wide K sub-tiles per pipeline stage.  The single MMA thread pays ~250 cycles of fixed cost per stage (mbarrier
-// wait, fence, two commits); with N <= 144 a 64-deep stage is only 4 x 64..72 cycles of tensor work, so narrow tiles use
-// 128-deep stages (KSUB = 2) to keep the issue loop off the critical path.
-template <int BN, class Epi, bool PAIR, int KSUB = 1>
+// Shared-memory plan of one CTA: the STAGES-deep operand ring (which also holds the finished fp32 accumulator tile between the
+// mainloop and the epilogue of a tile), the epilogues' per-warp transpose tiles, the barriers.
+// KSUB: 64-wide k-blocks per ring slot.  KSUB = 2 gives 128-deep slots: half as many full / empty barrier round trips (and wgmma
+// commit / wait pairs) per k, with the same bytes in flight.
+template <int BN, class Epi, int KSUB = 1>
 struct GemmCfg {
   static constexpr int A_SUB = GEMM_BM * GEMM_BK * 2;
-  static constexpr int B_SUB = (PAIR ? BN / 2 : BN) * GEMM_BK * 2;
+  static constexpr int B_SUB = BN * GEMM_BK * 2;
   static constexpr int A_BYTES = KSUB * A_SUB;
   static constexpr int B_BYTES = KSUB * B_SUB;
   static constexpr int EPI_WARPS = Epi::EPI_WARPS;
-  static constexpr int THREADS = 64 + 32 * EPI_WARPS;
+  // Every consumer warpgroup issues wgmma.  One warpgroup: both 64-row halves of the tile.  Two: one half each.  Three (EpiHeads, three
+  // heads per tile): all 128 rows of one head's columns each -- 72 / 72 / 80 (the last head plus the 8 zero columns) or 3 x 64 -- which
+  // keeps the accumulator at 80 registers under the 128-register cap of a 416-thread CTA.
+  static constexpr int MMA_WG = EPI_WARPS / 4;
+  static constexpr int NSUB = MMA_WG == 2 ? 1 : 2;                // 64-row halves per warpgroup
+  static constexpr int WN0 = MMA_WG == 3 ? (BN == 224 ? 72 : BN / 3) : BN;   // columns of warpgroups 0 .. MMA_WG - 2
+  static constexpr int WNL = MMA_WG == 3 ? BN - 2 * WN0 : BN;                 // columns of the last one
+  static constexpr int THREADS = 32 * EPI_WARPS + 32;             // consumer warpgroups + the producer warp
+  static constexpr int ACC_PITCH = BN + 4;
+  static constexpr int ACC_BYTES = GEMM_BM * ACC_PITCH * 4;
   static constexpr int STAGE_BYTES = EPI_WARPS * Epi::STAGE_FLOATS * 4;   // one transpose tile per epilogue warp
   static constexpr int FIT = (GEMM_SMEM_BUDGET - STAGE_BYTES) / (A_BYTES + B_BYTES);
   static constexpr int STAGES = FIT > 8 ? 8 : FIT;
-  static constexpr int BYTES = 1024 /*align slack*/ + STAGES * (A_BYTES + B_BYTES) + STAGE_BYTES + (2 * STAGES + 4) * 8 + 16;
-  static_assert(STAGES >= 3, "smem budget");
+  static constexpr int RING = STAGES * (A_BYTES + B_BYTES) > ACC_BYTES ? STAGES * (A_BYTES + B_BYTES) : ACC_BYTES;
+  static constexpr int BYTES = 1024 /*align slack*/ + RING + STAGE_BYTES + (2 * STAGES + 1) * 8;
+  static_assert(STAGES >= 2, "smem budget");
+  static_assert(BYTES <= 227 * 1024, "smem budget");
 };
 
+// One consumer warpgroup's share of a tile: WN accumulator columns from col0 over NSUB 64-row halves from 64-row block row64.  Runs the
+// k-loop (slot s is released once wgmma.wait_group shows its MMAs complete, while slot s + 1's are in flight), then, after every warpgroup's
+// MMAs have completed, writes its fragments into the accumulator tile in shared memory.
+template <int BN, class Epi, int MC, int WN, int KSUB>
+__device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
+                                              int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane) {
+  using SM = GemmCfg<BN, Epi, KSUB>;
+  constexpr int NSUB = SM::NSUB;
+  auto release = [&](uint32_t s) {   // one thread per warpgroup, on the slot's barrier in every CTA of the cluster
+    if ((threadIdx.x & 127) == 0) {
+      if (MC == 1) mbar_arrive(&empty[s]);
+      else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
+    }
+  };
+  float d[NSUB][WN / 2];
+  uint32_t prev = 0;
+  for (int kb = 0; kb < num_k_blocks; kb += KSUB) {
+    mbar_wait(&full[stage], phase);
+    wgmma_fence();
+    const int nsub = num_k_blocks - kb < KSUB ? num_k_blocks - kb : KSUB;
+#pragma unroll
+    for (int sub = 0; sub < KSUB; ++sub) {
+      if (sub >= nsub) break;
+      const uint32_t a0 = smem_u32(sA + stage * SM::A_BYTES + sub * SM::A_SUB + row64 * 8192);
+      const uint32_t b0 = smem_u32(sB + stage * SM::B_BYTES + sub * SM::B_SUB + col0 * 128);
+#pragma unroll
+      for (int k = 0; k < GEMM_BK / 16; ++k) {
+#pragma unroll
+        for (int s = 0; s < NSUB; ++s)
+          Wgmma<WN>::mma(d[s], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0) + 2 * k, (kb | sub | k) != 0);
+      }
+    }
+    wgmma_commit();
+    if (kb > 0) { wgmma_wait<1>(); release(prev); }
+    prev = stage;
+    if (++stage == SM::STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  release(prev);
+#pragma unroll
+  for (int s = 0; s < NSUB; ++s) wgmma_fence_regs(d[s]);
+  named_bar_sync(1, 32 * SM::EPI_WARPS);   // every MMA of the tile has completed: the ring may now hold the accumulator
+  // m64nN fragment: register 4i + {0,1} -> row 16 * (warp % 4) + lane / 4, columns 8i + 2 (lane % 4) + {0,1}; 4i + {2,3} -> row + 8
+#pragma unroll
+  for (int s = 0; s < NSUB; ++s) {
+    float* r0 = sAcc + (size_t)((row64 + s) * 64 + 16 * lg + (lane >> 2)) * SM::ACC_PITCH + col0 + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < WN / 8; ++i) {
+      *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(d[s][4 * i], d[s][4 * i + 1]);
+      *reinterpret_cast<float2*>(r0 + 8 * SM::ACC_PITCH + 8 * i) = make_float2(d[s][4 * i + 2], d[s][4 * i + 3]);
+    }
+  }
+}
+
 // MC > 1: launched as clusters of MC CTAs with consecutive blockIdx.x = consecutive M tiles of the SAME N tile (host guarantees
-// num_m_tiles % MC == 0, gridDim.x % MC == 0 and num_tiles % MC == 0, so the CTAs of a cluster walk the same number of tiles in step).
-// The N-side operand tile (BN rows x 64 columns) is then fetched ONCE per cluster: tmB is a map with 32-row boxes, CTA rank r issues the
-// sub-boxes j = r, r + MC, ... with .multicast::cluster, every CTA still expects the full A + B bytes on its own `full` barrier, and a
-// stage is free again only when all MC consumers have released it (`empty` counts MC multicast commits).
-template <int BN, class Epi, int MC = 1>
+// num_m_tiles % MC == 0 and gridDim.x % MC == 0, so the CTAs of a cluster walk the same number of tiles in step).
+// The N-side operand tile (BN rows x 64 columns) is then fetched ONCE per cluster: tmB is a map with SUBROWS-row boxes, CTA rank r issues
+// the sub-boxes j = r, r + MC, ... with .multicast::cluster, every CTA still expects the full A + B bytes on its own `full` barrier, a
+// stage is free again only when the MMA warpgroups of all MC CTAs have released it (`empty` counts their arrivals), and the ring is
+// refilled for the next tile only when every CTA of the cluster has finished reading its accumulator out of it (`acc_free`).
+// FIRST_PHASE: another GEMM phase follows in the same kernel (mlp_fused_kernel): the barriers are invalidated at the end so that the next
+// phase may lay out its own in the same shared memory.
+template <int BN>
+struct McSub { static constexpr int ROWS = BN % 32 == 0 ? 32 : 16; };
+template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, int KSUB = 1>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw) {
   static_assert(BN % 16 == 0 && BN >= 64 && BN <= 256, "BN");
-  static_assert(MC >= 1 && MC <= 8 && (MC == 1 || BN % 32 == 0), "MC");
+  static_assert(MC >= 1 && MC <= 8 && BN % McSub<BN>::ROWS == 0, "MC");
+  using SM = GemmCfg<BN, Epi, KSUB>;
+  constexpr int STAGES = SM::STAGES, EPI_WARPS = SM::EPI_WARPS, NSUB = SM::NSUB;
   constexpr uint16_t MC_MASK = static_cast<uint16_t>((1u << MC) - 1u);
-  using SM = GemmCfg<BN, Epi, false>;
-  constexpr int STAGES = SM::STAGES;
-  constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  // 1024-byte alignment by pointer arithmetic on the __shared__ array (a round trip through uintptr_t loses the address space and
-  // turns every staging access into a generic LD.E / ST.E)
+  // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array (a round trip through uintptr_t loses the
+  // address space and turns every staging access into a generic LD.E / ST.E)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * SM::A_BYTES;
-  float* sStage = reinterpret_cast<float*>(sB + STAGES * SM::B_BYTES);
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * SM::B_BYTES + SM::STAGE_BYTES);
+  float* sAcc = reinterpret_cast<float*>(smem);
+  float* sStage = reinterpret_cast<float*>(smem + SM::RING);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + SM::RING + SM::STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* acc_free = empty + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = g.num_m_tiles * g.num_n_tiles;
+  constexpr int PRODUCER = EPI_WARPS;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], MC);
+      mbar_init(&empty[i], SM::MMA_WG * MC);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 32 * SM::EPI_WARPS);
-    }
+    mbar_init(acc_free, EPI_WARPS * MC);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
   if (MC > 1) cluster_sync_all();  // peers multicast into our stages and arrive on our barriers: they must exist first
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch();
-  if (warp == 0 && g.pf_bytes != 0) {   // constant data: no need to wait for the previous kernel
+  if (warp == PRODUCER && g.pf_bytes != 0) {   // constant data: no need to wait for the previous kernel
     if (elect_one()) prefetch_weights_l2(g.pf, g.pf_bytes, blockIdx.x, gridDim.x);
     __syncwarp();
   }
   pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
+  EZB_DBG(const bool dbg = g.dbg != nullptr && blockIdx.x == 0; const long long t_start = clock64(); long long w0 = 0, w1 = 0, w4 = 0;)
 
-  if (warp == 0) {
-    // ------------------------------------------------ TMA producer.  The loop is warp-uniform and the copies are issued under elect.sync:
-    // inside an `if (lane == 0)` region ptxas wraps every UTMALDG / UTCHMMA / UTCBAR (uniform-datapath instructions) in an
-    // ELECT ... BRA.U.ANY serialisation loop with R2UR broadcasts (~40-60 cycles per instruction); under elect.sync it knows a
-    // single lane is active and issues them back to back.
-    {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
-        const int n0 = nt * BN;
-        for (int kb = 0; kb < g.num_k_blocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          if (elect_one()) {
-          mbar_expect_tx(&full[stage], SM::A_BYTES + SM::B_BYTES);
+  if (warp == PRODUCER) {
+    // ------------------------------------------------ TMA producer (warp-uniform loop, copies issued under elect.sync)
+    uint32_t stage = 0, phase = 0, af_phase = 0;
+    bool first = true;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
+      const int n0 = nt * BN;
+      if (!first) { mbar_wait(acc_free, af_phase); af_phase ^= 1; }   // the ring held the previous tile's accumulator
+      first = false;
+      for (int kb0 = 0; kb0 < g.num_k_blocks; kb0 += KSUB) {
+        EZB_DBG(const long long tq = clock64();)
+        mbar_wait(&empty[stage], phase ^ 1);
+        EZB_DBG(w0 += clock64() - tq;)
+        const int nsub = g.num_k_blocks - kb0 < KSUB ? g.num_k_blocks - kb0 : KSUB;
+        if (elect_one()) {
+          mbar_expect_tx(&full[stage], nsub * (SM::A_SUB + SM::B_SUB));
+          for (int sub = 0; sub < nsub; ++sub) {
+          const int kb = kb0 + sub;
+          uint8_t* dA = sA + stage * SM::A_BYTES + sub * SM::A_SUB;
+          uint8_t* dB = sB + stage * SM::B_BYTES + sub * SM::B_SUB;
           if (g.taps == 0) {
-            tma_load_2d(sA + stage * SM::A_BYTES, &tmA, &full[stage], kb * GEMM_BK, mt * GEMM_BM);
+            tma_load_2d(dA, &tmA, &full[stage], kb * GEMM_BK, mt * GEMM_BM);
           } else {
             const int tap = kb / g.cin_blocks, cb = kb - tap * g.cin_blocks;
             const int bidx = mt / g.tiles_per_batch, t0 = (mt - bidx * g.tiles_per_batch) * GEMM_BM;
             if (g.stride > 1) {
               const int off = tap - g.pad;                                   // input row = q * stride + off
               const int r = ((off % g.stride) + g.stride) % g.stride, dq = (off - r) / g.stride;
-              tma_load_4d(sA + stage * SM::A_BYTES, &tmA, &full[stage], cb * GEMM_BK, r, t0 + dq, bidx);
+              tma_load_4d(dA, &tmA, &full[stage], cb * GEMM_BK, r, t0 + dq, bidx);
             } else {
-              tma_load_3d(sA + stage * SM::A_BYTES, &tmA, &full[stage], cb * GEMM_BK, t0 + (tap - g.center) * g.dilation, bidx);
+              tma_load_3d(dA, &tmA, &full[stage], cb * GEMM_BK, t0 + (tap - g.center) * g.dilation, bidx);
             }
           }
           if (MC == 1) {
-            tma_load_2d(sB + stage * SM::B_BYTES, &tmB, &full[stage], kb * GEMM_BK, n0);
+            tma_load_2d(dB, &tmB, &full[stage], kb * GEMM_BK, n0);
           } else {
-            for (int j = (int)cluster_ctarank(); j < BN / 32; j += MC)
-              tma_load_2d_mc(sB + stage * SM::B_BYTES + j * 4096, &tmB, &full[stage], kb * GEMM_BK, n0 + j * 32, MC_MASK);
+            constexpr int SR = McSub<BN>::ROWS;
+            for (int j = (int)cluster_ctarank(); j < BN / SR; j += MC)
+              tma_load_2d_mc(dB + j * SR * 128, &tmB, &full[stage], kb * GEMM_BK, n0 + j * SR, MC_MASK);
           }
           }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer (warp-uniform loop, one elected lane issues: see the producer's note)
-    constexpr uint32_t idesc = umma_idesc_bf16(GEMM_BM, BN);
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < g.num_k_blocks; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t ad = umma_desc_sw128(smem_u32(sA + stage * SM::A_BYTES));
-          const uint64_t bd = umma_desc_sw128(smem_u32(sB + stage * SM::B_BYTES));
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc, (kb | k) != 0);
-          if (MC == 1) umma_commit(&empty[stage]);
-          else umma_commit_mc(&empty[stage], MC_MASK);
-          if (kb == g.num_k_blocks - 1) umma_commit(&tfull[acc]);
         }
         __syncwarp();
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
   } else {
-    // ------------------------------------------------ epilogue (warps 2..5; TMEM lane group = warp % 4)
-    const int lg = warp & 3;
-    uint32_t acc = 0, acc_phase = 0;
+    // ------------------------------------------------ consumers: wgmma mainloop (MMA warpgroups), accumulator -> smem, epilogue (all)
+    const int wg = warp >> 2, lg = warp & 3;
+    uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
+      EZB_DBG(const long long tm = clock64();)
+      if constexpr (SM::MMA_WG == 3) {
+        if (wg == 2) gemm_mma_part<BN, Epi, MC, SM::WNL, KSUB>(2 * SM::WN0, 0, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
+        else gemm_mma_part<BN, Epi, MC, SM::WN0, KSUB>(wg * SM::WN0, 0, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
+      } else {
+        gemm_mma_part<BN, Epi, MC, BN, KSUB>(0, wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
+      }
+      EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
+      named_bar_sync(1, 32 * EPI_WARPS);     // accumulator tile complete in shared memory
+      EZB_DBG(const long long te = clock64(); w1 += te - ta;)
       int row0, nvalid;
       if (g.taps == 0) {
         row0 = mt * GEMM_BM + lg * 32;
@@ -735,32 +802,41 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
         row0 = bidx * g.T + t0;
         nvalid = g.T - t0;
       }
-      const uint32_t taddr_row = tmem_base + acc * BN + (static_cast<uint32_t>(lg * 32) << 16);
-      constexpr int CW = BN / (SM::EPI_WARPS / 4);  // columns per warp
-      const int ch = (warp - 2) >> 2;
-      uint64_t* tf = &tfull[acc];
-      const uint32_t ph = acc_phase;
-      Epi::run(ep, sStage + (warp - 2) * Epi::STAGE_FLOATS, taddr_row, row0, nvalid, nt * BN, g.N, lane, ch * CW, (ch + 1) * CW, [tf, ph]() {
-        mbar_wait(tf, ph);
-        tc_fence_after();
-      });
-      tc_fence_before();
-      mbar_arrive(&tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
+      constexpr int CW = BN / (EPI_WARPS / 4);  // columns per warp
+      const AccRows ar{sAcc + lg * 32 * SM::ACC_PITCH, SM::ACC_PITCH};
+      Epi::run(ep, sStage + warp * Epi::STAGE_FLOATS, ar, row0, nvalid, nt * BN, g.N, lane, wg * CW, (wg + 1) * CW, []() {});
+      EZB_DBG(w4 += clock64() - te;)
+      fence_proxy_async_smem();   // this warp's generic accesses to the ring are ordered before the producer's next TMA writes into it
+      __syncwarp();
+      if (lane == 0) {
+        if (MC == 1) mbar_arrive(acc_free);
+        else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(acc_free), r));
+      }
     }
   }
-  tc_fence_before();
+  EZB_DBG(if (dbg && lane == 0) {
+    if (warp == PRODUCER) atomicAdd(&g.dbg[2], (unsigned long long)w0);
+    if (warp == 0) {
+      atomicAdd(&g.dbg[0], (unsigned long long)w0); atomicAdd(&g.dbg[1], (unsigned long long)w1); atomicAdd(&g.dbg[4], (unsigned long long)w4);
+      atomicAdd(&g.dbg[5], (unsigned long long)(clock64() - t_start));
+    }
+  })
   __syncthreads();
   if (MC > 1) cluster_sync_all();  // nobody leaves while a peer may still multicast into this CTA or arrive on its barriers
-  if (warp == 1) tmem_dealloc<TMEM_COLS>(tmem_base);
+  if (FIRST_PHASE) {
+    if (warp == PRODUCER && lane == 0) {
+      for (int i = 0; i < STAGES; ++i) { mbar_inval(&full[i]); mbar_inval(&empty[i]); }
+      mbar_inval(acc_free);
+    }
+    __syncthreads();
+  }
 }
-template <int BN, class Epi, int MC = 1>
-__global__ void __launch_bounds__((GemmCfg<BN, Epi, false>::THREADS), 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g,
-                    const typename Epi::Params ep) {
+template <int BN, class Epi, int MC = 1, int KSUB = 1>
+__global__ void __launch_bounds__((GemmCfg<BN, Epi, KSUB>::THREADS), 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g,
+                  const typename Epi::Params ep) {
   extern __shared__ uint8_t smem_dyn[];
-  gemm_body<BN, Epi, MC>(tmA, tmB, g, ep, smem_dyn);
+  gemm_body<BN, Epi, MC, false, KSUB>(tmA, tmB, g, ep, smem_dyn);
 }
 
 }  // namespace ezb
@@ -792,16 +868,16 @@ struct EpiHeadsParams {
 // 3H heads of [q | k | v] are regrouped three per tile (N-tile 224 for dh = 72: 3 x 72 + 8 zero columns; 192 for dh = 64), which
 // makes the tile wide enough for the tensor pipe (narrow tiles are operand-bandwidth bound) and keeps one head per warp.
 // DIRECT: every thread stores its own q / k row (dh bf16 = 128 or 144 contiguous bytes) with 16-byte stores instead of transposing it through a
-// per-warp 8 KB shared-memory tile.  The staging tiles of 12 epilogue warps take 96 KB, which leaves the 256 x 224 QKV tile only FOUR 30 KB
-// pipeline stages (the GEGLU kernel runs six); without them it gets seven.
+// per-warp 8 KB shared-memory tile.  The staging tiles of 12 epilogue warps take 96 KB, which leaves the 128 x 224 QKV tile only two 44 KB
+// pipeline stages; without them it gets four.
 template <int DH, int HPT = 2, bool DIRECT = false, bool FOLD = false, bool DBG = false>
 struct EpiHeads {
   using Params = EpiHeadsParams;
   static constexpr int BN = HPT == 3 ? (DH == 72 ? 224 : 3 * DH) : 2 * DH;
-  static constexpr int EPI_WARPS = 4 * HPT;   // the HPT warps of a TMEM lane group take one head each
+  static constexpr int EPI_WARPS = 4 * HPT;   // the HPT warps of a 32-row group take one head each
   static constexpr int STAGE_FLOATS = DIRECT ? 0 : EPI_STAGE_FLOATS;
   template <class Wait>
-  static __device__ __forceinline__ void run(const Params& ep, float* st, uint32_t taddr_row, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
                                              int c_end, Wait wait) {
     const int row = row0 + lane;
     const bool row_ok = lane < nvalid;
@@ -826,9 +902,8 @@ struct EpiHeads {
       const int kind = ep.kind[sec];
       uint32_t r[DH];
       __syncwarp();
-      tmem_ld_32x64(taddr_row + hh * DH, r);
-      if constexpr (DH == 72) tmem_ld_32x8(taddr_row + hh * DH + 64, r + 64);
-      tmem_ld_wait();
+      acc_ld<64>(ar, hh * DH, lane, r);
+      if constexpr (DH == 72) acc_ld<8>(ar, hh * DH + 64, lane, r + 64);
       float v[DH];
 #pragma unroll
       for (int i = 0; i < DH; ++i) v[i] = __uint_as_float(r[i]);
@@ -915,174 +990,7 @@ struct EpiHeads {
 
 namespace ezb {
 // ---------------------------------------------------------------------------------------------------------------
-// CTA-pair GEMM (tcgen05 cta_group::2): a cluster of two CTAs on one TPC computes a 256 x BN tile.  CTA r stages its own
-// 128 rows of A and rows [r*BN/2, (r+1)*BN/2) of the W tile; the leader's single MMA thread issues M=256 instructions that
-// read both CTAs' shared memory, so each SM pulls half the operand bytes per flop through L2 (the 128x128 single-CTA tile
-// is L2->smem bound at ~64 flop/B).  Accumulator rows 128r..128r+127 live in CTA r's TMEM; both CTAs run the epilogue.
-// FIRST_PHASE: the body is followed by another GEMM phase in the same kernel (mlp_fused_kernel): keep the TMEM allocation permit and
-// invalidate the mbarriers so that the next phase may lay out its own in the same shared memory.
-template <int BN, class Epi, int KSUB, bool FIRST_PHASE = false>
-__device__ __forceinline__ void gemm2_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw) {
-  static_assert(BN % 16 == 0 && BN >= 64 && BN <= 256, "BN");
-  using SM = GemmCfg<BN, Epi, true, KSUB>;
-  constexpr int STAGES = SM::STAGES;
-  constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  // 1024-byte alignment by pointer arithmetic on the __shared__ array (a round trip through uintptr_t loses the address space and
-  // turns every staging access into a generic LD.E / ST.E)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * SM::A_BYTES;
-  float* sStage = reinterpret_cast<float*>(sB + STAGES * SM::B_BYTES);
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * SM::B_BYTES + SM::STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-  const int num_tiles = g.num_m_tiles * g.num_n_tiles;  // num_m_tiles counts 256-row tiles here
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 2 * 32 * SM::EPI_WARPS);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc_pair<TMEM_COLS, !FIRST_PHASE>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_launch();
-  if (warp == 0 && g.pf_bytes != 0) {   // constant data: no need to wait for the previous kernel
-    if (elect_one()) prefetch_weights_l2(g.pf, g.pf_bytes, blockIdx.x, gridDim.x);
-    __syncwarp();
-  }
-  pdl_wait();
-  EZB_DBG(const bool dbg = g.dbg != nullptr && blockIdx.x == 0; const long long t_start = clock64(); long long w0 = 0, w1 = 0;)
-
-  if (warp == 0) {
-    // ------------------------------------------------ TMA producer (both CTAs; bytes are credited to the leader's barrier)
-    {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
-        const int m0 = mt * 2 * GEMM_BM + (int)rank * GEMM_BM, n0 = nt * BN + (int)rank * (BN / 2);
-        for (int kb = 0; kb < g.num_k_blocks; kb += KSUB) {
-          EZB_DBG(const long long tq = clock64();)
-          mbar_wait(&empty[stage], phase ^ 1);
-          EZB_DBG(w0 += clock64() - tq;)
-          const uint32_t bar = mapa_u32(smem_u32(&full[stage]), 0);
-          const int nsub = (g.num_k_blocks - kb) < KSUB ? (g.num_k_blocks - kb) : KSUB;
-          if (elect_one()) {
-            if (leader) mbar_expect_tx(&full[stage], 2 * nsub * (SM::A_SUB + SM::B_SUB));
-            for (int sub = 0; sub < nsub; ++sub) {
-              tma_load_2d_pair(sA + stage * SM::A_BYTES + sub * SM::A_SUB, &tmA, bar, (kb + sub) * GEMM_BK, m0);
-              tma_load_2d_pair(sB + stage * SM::B_BYTES + sub * SM::B_SUB, &tmB, bar, (kb + sub) * GEMM_BK, n0);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer (leader CTA only)
-    if (leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(2 * GEMM_BM, BN);
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        EZB_DBG(long long tq = clock64();)
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        EZB_DBG(w1 += clock64() - tq;)
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < g.num_k_blocks; kb += KSUB) {
-          EZB_DBG(tq = clock64();)
-          mbar_wait(&full[stage], phase);
-          EZB_DBG(w0 += clock64() - tq;)
-          tc_fence_after();
-          if (elect_one()) {
-            const int nsub = (g.num_k_blocks - kb) < KSUB ? (g.num_k_blocks - kb) : KSUB;
-            for (int sub = 0; sub < nsub; ++sub) {
-              const uint64_t ad = umma_desc_sw128(smem_u32(sA + stage * SM::A_BYTES + sub * SM::A_SUB));
-              const uint64_t bd = umma_desc_sw128(smem_u32(sB + stage * SM::B_BYTES + sub * SM::B_SUB));
-#pragma unroll
-              for (int k = 0; k < GEMM_BK / 16; ++k) umma_bf16_pair(d_tmem, ad + 2 * k, bd + 2 * k, idesc, (kb | sub | k) != 0);
-            }
-            umma_commit_pair(&empty[stage]);
-            if (kb + KSUB >= g.num_k_blocks) umma_commit_pair(&tfull[acc]);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else {
-    // ------------------------------------------------ epilogue (both CTAs, own 128 accumulator rows)
-    const int lg = warp & 3;
-    uint32_t acc = 0, acc_phase = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
-      const int row0 = mt * 2 * GEMM_BM + (int)rank * GEMM_BM + lg * 32;
-      const uint32_t taddr_row = tmem_base + acc * BN + (static_cast<uint32_t>(lg * 32) << 16);
-      constexpr int CW = BN / (SM::EPI_WARPS / 4);
-      const int ch = (warp - 2) >> 2;
-      uint64_t* tf = &tfull[acc];
-      const uint32_t ph = acc_phase;
-      EZB_DBG(const long long te = clock64(); long long tw = 0;)
-      Epi::run(ep, sStage + (warp - 2) * Epi::STAGE_FLOATS, taddr_row, row0, g.M - row0, nt * BN, g.N, lane, ch * CW, (ch + 1) * CW, [&]() {
-        EZB_DBG(const long long tq = clock64();)
-        mbar_wait(tf, ph);
-        EZB_DBG(tw = clock64() - tq;)
-        tc_fence_after();
-      });
-      EZB_DBG(w0 += tw; w1 += clock64() - te - tw;)
-      tc_fence_before();
-      mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[acc]), 0));
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-  EZB_DBG(if (dbg && lane == 0) {
-    if (warp == 0) atomicAdd(&g.dbg[2], (unsigned long long)w0);
-    if (warp == 1) { atomicAdd(&g.dbg[0], (unsigned long long)w0); atomicAdd(&g.dbg[1], (unsigned long long)w1); }
-    if (warp == 2) { atomicAdd(&g.dbg[3], (unsigned long long)w0); atomicAdd(&g.dbg[4], (unsigned long long)w1); atomicAdd(&g.dbg[5], (unsigned long long)(clock64() - t_start)); }
-  })
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) tmem_dealloc_pair<TMEM_COLS>(tmem_base);
-  if (FIRST_PHASE) {
-    if (warp == 0 && lane == 0) {
-      for (int i = 0; i < STAGES; ++i) { mbar_inval(&full[i]); mbar_inval(&empty[i]); }
-      for (int i = 0; i < 2; ++i) { mbar_inval(&tfull[i]); mbar_inval(&tempty[i]); }
-    }
-    __syncthreads();
-  }
-}
-template <int BN, class Epi, int KSUB>
-__global__ void __launch_bounds__((GemmCfg<BN, Epi, true, KSUB>::THREADS), 1)
-gemm2_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g, const typename Epi::Params ep) {
-  extern __shared__ uint8_t smem_dyn[];
-  gemm2_body<BN, Epi, KSUB>(tmA, tmB, g, ep, smem_dyn);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// The MLP of a DiT block (modules.py:263-277,366) as ONE persistent launch: phase 1 = the GEGLU projection (CTA-pair tiles, EpiGeglu), a
+// The MLP of a DiT block (modules.py:263-277,366) as ONE persistent launch: phase 1 = the GEGLU projection (2-CTA cluster tiles, EpiGeglu), a
 // grid-wide barrier, phase 2 = the output projection with its gated-residual epilogue (swap-AB tiles, EpiLinearT, incl. the LayerNorm fold
 // outputs for the next block).  The grid is one CTA per SM (all co-resident), launched as clusters of two for phase 1.  Phase 2 reads the
 // bf16 intermediate that phase 1 wrote with ordinary stores through TMA, hence the generic->async proxy fence after the barrier.
@@ -1108,13 +1016,13 @@ __device__ __forceinline__ void grid_barrier(GridBarrier* b) {
   asm volatile("fence.proxy.async;" ::: "memory");
 }
 template <int BN1, class Epi1, class Epi2>
-__global__ void __launch_bounds__((GemmCfg<BN1, Epi1, true, 1>::THREADS), 1)
+__global__ void __launch_bounds__((GemmCfg<BN1, Epi1>::THREADS), 1)
 mlp_fused_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1, const GemmShape g1, const typename Epi1::Params ep1,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2, const GemmShape g2, const typename Epi2::Params ep2,
                  GridBarrier* bar) {
-  static_assert(GemmCfg<BN1, Epi1, true, 1>::THREADS == GemmCfg<256, Epi2, false>::THREADS, "both phases use the same warp roles");
+  static_assert(GemmCfg<BN1, Epi1>::THREADS == GemmCfg<256, Epi2>::THREADS, "both phases use the same warp roles");
   extern __shared__ uint8_t smem_dyn[];
-  gemm2_body<BN1, Epi1, 1, true>(tmA1, tmB1, g1, ep1, smem_dyn);
+  gemm_body<BN1, Epi1, 2, true>(tmA1, tmB1, g1, ep1, smem_dyn);
   grid_barrier(bar);
   gemm_body<256, Epi2, 1>(tmA2, tmB2, g2, ep2, smem_dyn);
 }

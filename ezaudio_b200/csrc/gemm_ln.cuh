@@ -1,10 +1,9 @@
 // A residual-stream GEMM and the LayerNorm that follows it as ONE launch.
 //
-// In situ (CUDA-graph replay + programmatic dependent launch, profiles/r2) the 88 + 14 LayerNorm launches of a DiT step cost 1.2 ms = 12 us each,
-// for a pass that moves 27.6 MB of L2-resident data: launch ramp, one thin wave, drain.  Their producers (out-proj, cross-proj, MLP-out, skip and
-// patch-embed linears: blocks.py:128,141,151,156) are one-wave swap-AB GEMMs whose 144 CTAs are all resident, so the LayerNorm can run as a tail
-// phase of the same grid behind a grid-wide barrier: no second launch, no ramp, the rows are still hot in L2.  (Folding the LayerNorm algebraically
-// into both neighbouring GEMMs was tried first -- gemm.cuh FoldIn / FoldOut -- and lost: the extra epilogue work cost more than the pass.)
+// The LayerNorm launches of a DiT step each move a few MB of L2-resident data, so they are dominated by launch ramp, one thin wave and drain.  Their
+// producers (out-proj, cross-proj, MLP-out, skip and patch-embed linears: blocks.py:128,141,151,156) are swap-AB GEMMs that fit one resident wave
+// at the usual sizes, so the LayerNorm can run as a tail phase of the same grid behind a grid-wide barrier: no second launch, no ramp, the rows
+// are still hot in L2.  The alternative is folding the LayerNorm algebraically into both neighbouring GEMMs (gemm.cuh FoldIn / FoldOut).
 #pragma once
 #include "elementwise.cuh"
 #include "host.cuh"
@@ -12,7 +11,7 @@
 namespace ezb {
 
 template <int BN, class Epi>
-__global__ void __launch_bounds__((GemmCfg<BN, Epi, false>::THREADS), 1)
+__global__ void __launch_bounds__((GemmCfg<BN, Epi>::THREADS), 1)
 gemm_ln_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g, const typename Epi::Params ep,
                const LnParams lp, GridBarrier* bar) {
   extern __shared__ uint8_t smem_dyn[];
@@ -43,8 +42,8 @@ int gemm_swapped_ln(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int ld
   EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N_features, (uint64_t)ldw, GEMM_BM, &tA));
   EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M_tokens, (uint64_t)lda, BN, &tB));
   auto kern = gemm_ln_kernel<BN, Epi>;
-  constexpr int smem = GemmCfg<BN, Epi, false>::BYTES;
-  constexpr int THREADS = GemmCfg<BN, Epi, false>::THREADS;
+  constexpr int smem = GemmCfg<BN, Epi>::BYTES;
+  constexpr int THREADS = GemmCfg<BN, Epi>::THREADS;
   static bool attr_set[16] = {};
   if (!attr_set[dev.id & 15]) {
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

@@ -86,7 +86,7 @@ inline PFN_encodeTiled get_encode() {
 
 // bf16 tensor, innermost dim first; 128-byte swizzle, zero fill out of bounds.
 inline int make_tmap(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes /*rank-1*/,
-                     const uint32_t* box, int swizzle = 0 /* 0: SWIZZLE_128B, 1: SWIZZLE_32B, 2: none (dense box rows in shared memory) */) {
+                     const uint32_t* box) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return fail(EZB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
   cuuint64_t gd[5], gs[5];
@@ -101,7 +101,7 @@ inline int make_tmap(CUtensorMap* out, const void* ptr, int rank, const uint64_t
   for (int i = 0; i + 1 < rank; ++i)
     if (gs[i] % 16) return fail(EZB_ERR_ARG, "TMA stride %llu not a multiple of 16 B", (unsigned long long)gs[i]);
   CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_32B : swizzle == 2 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(EZB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): rank %d dims %llu,%llu box %u,%u", (int)r, rank,
                                      (unsigned long long)gd[0], (unsigned long long)gd[1], bx[0], bx[1]);
@@ -148,38 +148,6 @@ struct TmapCache {
   }
 };
 
-// 3-D [batch, rows, inner] bf16 map with a 16-element (32-byte, SWIZZLE_32B) inner box: the dh = 72 tail columns 64..79 of Q / K
-inline int get3d_sw32(TmapCache& c, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld_row, uint64_t ld_batch, uint32_t box_rows,
-                      const CUtensorMap** out) {
-  TmapCache::Key k(ptr, inner, rows, batch, ld_row * 1000003ull + ld_batch, box_rows, 32);
-  auto it = c.maps.find(k);
-  if (it == c.maps.end()) {
-    CUtensorMap m;
-    uint64_t dims[3] = {inner, rows, batch}, str[2] = {ld_row * 2, ld_batch * 2};
-    uint32_t box[3] = {16, box_rows, 1};
-    EZB_TRY(make_tmap(&m, ptr, 3, dims, str, box, true));
-    it = c.maps.emplace(k, m).first;
-  }
-  *out = &it->second;
-  return EZB_OK;
-}
-
-// 3-D [batch, rows, inner] bf16 map with an un-swizzled {box_inner, box_rows, 1} box (dense rows in shared memory): TMA stores of attention output tiles
-inline int get3d_plain(TmapCache& c, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld_row, uint64_t ld_batch, uint32_t box_inner,
-                       uint32_t box_rows, const CUtensorMap** out) {
-  TmapCache::Key k(ptr, inner, rows, batch, ld_row * 1000003ull + ld_batch, box_rows, 1000 + box_inner);
-  auto it = c.maps.find(k);
-  if (it == c.maps.end()) {
-    CUtensorMap m;
-    uint64_t dims[3] = {inner, rows, batch}, str[2] = {ld_row * 2, ld_batch * 2};
-    uint32_t box[3] = {box_inner, box_rows, 1};
-    EZB_TRY(make_tmap(&m, ptr, 3, dims, str, box, 2));
-    it = c.maps.emplace(k, m).first;
-  }
-  *out = &it->second;
-  return EZB_OK;
-}
-
 inline int make_tmap4_strided(CUtensorMap* out, const void* ptr, uint64_t C, uint64_t stride, uint64_t Tq, uint64_t B, uint64_t ldc) {
   // activations [B, Tq*stride, ldc] viewed as [B, Tq, stride, C]: box {64 channels, 1 phase, 128 rows, 1 clip}
   uint64_t dims[4] = {C, stride, Tq, B}, str[3] = {ldc * 2, stride * ldc * 2, Tq * stride * ldc * 2};
@@ -187,8 +155,7 @@ inline int make_tmap4_strided(CUtensorMap* out, const void* ptr, uint64_t C, uin
   return make_tmap(out, ptr, 4, dims, str, box);
 }
 
-inline int& opt_w_prefetch() {   // L2 prefetch of the next GEMM's weights (gemm.cuh GemmShape::pf).  Measured (call 21, three A/B pairs of one XL step under graph
-                                 // replay): 7.13 / 7.36 / 7.16 ms with, 7.18 / 7.12 / 7.25 ms without -- no effect beyond noise, so off by default.
+inline int& opt_w_prefetch() {   // L2 prefetch of the next GEMM's weights (gemm.cuh GemmShape::pf); off by default
   static int v = [] { const char* e = getenv("EZB_W_PREFETCH"); return e ? atoi(e) : 0; }();
   return v;
 }
@@ -201,7 +168,8 @@ struct WeightSeq {
 };
 struct Device {
   int id = 0;
-  int num_sms = 148;
+  int num_sms = 132;   // replaced by the device's count when the context is created
+  bool queried = false;
   TmapCache tmaps;
   std::map<std::tuple<const void*, int, long long>, WeightSeq> wseqs;
   WeightSeq* wcur = nullptr;
@@ -244,10 +212,6 @@ struct WeightSeqScope {   // RAII: entry points open a pass, error returns close
   ~WeightSeqScope() { dev->wseq_end(ok); }
 };
 
-inline int& opt_attn_poly() {
-  static int v = 0;  // measured: 27.3 us vs 25.9 us (self, XL) with one exp2 in four on the FMA pipe -- the softmax warps are issue-bound, not MUFU-bound
-  return v;
-}
 // profiling only: bit mask of kernel classes NOT launched (results are garbage, timing shows each class's in-situ cost under graph replay + PDL):
 // 1 LayerNorm passes, 2 attention, 4 QKV / cross-Q heads GEMMs, 8 fp32-output linears (proj, cross-proj, MLP-out, skip), 16 GEGLU GEMM
 inline int& opt_skip() {
@@ -262,37 +226,26 @@ inline int& opt_heads_dbg() {
   static int v = 0;
   return v;
 }
-inline int& opt_mlp2_pair() {   // MLP output projection (K = 4608) on the CTA-pair kernel instead of the one-wave swap-AB kernel
+inline int& opt_mlp2_pair() {   // MLP output projection (K = 4608) on the 2-CTA cluster kernel instead of the swap-AB kernel
   static int v = [] { const char* e = getenv("EZB_MLP2_PAIR"); return e ? atoi(e) : 0; }();
   return v;
 }
-inline int& opt_cq_single() {   // cross-attention Q projection on the single-CTA kernel (smaller tiles, better wave balance) instead of CTA pairs
+// 128-deep ring slots (gemm.cuh GemmCfg KSUB = 2): bit 0 GEGLU GEMM, bit 1 packed QKV GEMM (with the staging-free epilogue).  Off by default:
+// ptxas serialises the wgmma of the KSUB = 2 GEGLU instantiation (register pressure of the two-k-block slot at BN = 256).
+inline int& opt_ksub2() {
+  static int v = [] { const char* e = getenv("EZB_KSUB2"); return e ? atoi(e) : 0; }();
+  return v;
+}
+inline int& opt_cq_single() {   // cross-attention Q projection on the single-CTA kernel (no cluster pairing) instead of 2-CTA clusters
   static int v = [] { const char* e = getenv("EZB_CQ_SINGLE"); return e ? atoi(e) : 0; }();
   return v;
 }
-inline int& opt_ksub2() {   // 128-deep pipeline stages (half as many per-stage waits / commits for the single MMA thread): bit 0 GEGLU GEMM (76 -> 68 us, default),
-                            // bit 1 packed QKV GEMM with the staging-free epilogue (no gain, off)
-  static int v = [] { const char* e = getenv("EZB_KSUB2"); return e ? atoi(e) : 1; }();
-  return v;
-}
-inline int& opt_attn_res() {   // attention with K / V^T resident per (b, h) (attention_tc4.cuh, RES = 1)
-  static int v = [] { const char* e = getenv("EZB_ATTN_RES"); return e ? atoi(e) : 0; }();
-  return v;
-}
-inline int& opt_attn_pp() {   // attention: the two softmax groups alternate their exponent phases (MUFU token, attention_tc4.cuh)
-  static int v = [] { const char* e = getenv("EZB_ATTN_PP"); return e ? atoi(e) : 0; }();
-  return v;
-}
-inline int& opt_attn_dbg() {
-  static int v = 0;
-  return v;
-}
 inline int& opt_ln_variant() {
-  static int v = [] { const char* e = getenv("EZB_LN_VARIANT"); return e ? atoi(e) : 2; }();   // 2: precombined affine in registers + register-resident skip_norm (8.9 -> 6.2 us per launch)
+  static int v = [] { const char* e = getenv("EZB_LN_VARIANT"); return e ? atoi(e) : 2; }();   // 2: precombined affine in registers + register-resident skip_norm
   return v;
 }
 inline int& opt_dhp80() {
-  static int v = [] { const char* e = getenv("EZB_DHP80"); return e ? atoi(e) : 1; }();   // default on: -0.5 % step time, -0.9 us per self-attention launch (profiles/r2)
+  static int v = [] { const char* e = getenv("EZB_DHP80"); return e ? atoi(e) : 1; }();   // 80-element q / k rows for dh = 72 (128 otherwise)
   return v;
 }
 // LayerNorm folded into the neighbouring GEMMs (gemm.cuh FoldIn / FoldOut); read when a handle is created
@@ -345,9 +298,9 @@ struct ConvAddr {  // implicit-GEMM addressing of A, see gemm.cuh
 template <int BN, class Epi>
 int launch_gemm_t(Device& dev, cudaStream_t st, const CUtensorMap* tA, const CUtensorMap* tB, const GemmShape& g,
                   const typename Epi::Params& ep) {
-  auto kern = gemm_tcgen05_kernel<BN, Epi>;
-  constexpr int smem = GemmCfg<BN, Epi, false>::BYTES;
-  constexpr int GEMM_THREADS = GemmCfg<BN, Epi, false>::THREADS;
+  auto kern = gemm_wgmma_kernel<BN, Epi>;
+  constexpr int smem = GemmCfg<BN, Epi>::BYTES;
+  constexpr int GEMM_THREADS = GemmCfg<BN, Epi>::THREADS;
   static bool attr_set[16] = {};
   if (!attr_set[dev.id & 15]) {
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -393,11 +346,11 @@ int gemm_swapped(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, 
   return launch_gemm_t<BN, Epi>(dev, st, tA, tB, g, ep);
 }
 
-// Swap-AB launch with the activation tile multicast across clusters of MC feature tiles (gemm_tcgen05_kernel<.., MC>): the one-wave
+// Swap-AB launch with the activation tile multicast across clusters of MC feature tiles (gemm_wgmma_kernel<.., MC>): the one-wave
 // swap-AB GEMMs are L2-feed bound (48 KB per CTA per k-block); sharing the 32 KB token tile between MC = 3 CTAs leaves 26.7 KB.
 // Falls back to the plain launch whenever the shape does not split into whole clusters or the device cannot host them in one wave.
 inline int& opt_swap_mc() {
-  static int v = 0;   // NOT validated on hardware yet (written at the end of round 1 without GPU time): off by default
+  static int v = 0;   // off by default
   return v;
 }
 template <class Epi, int MC>
@@ -405,9 +358,9 @@ int gemm_swapped_mc(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int ld
                     const typename Epi::Params& ep) {
   constexpr int BN = 256;
   const int mt = (N_features + GEMM_BM - 1) / GEMM_BM, nt = (M_tokens + BN - 1) / BN, tiles = mt * nt;
-  auto kern = gemm_tcgen05_kernel<BN, Epi, MC>;
-  constexpr int smem = GemmCfg<BN, Epi, false>::BYTES;
-  constexpr int GEMM_THREADS = GemmCfg<BN, Epi, false>::THREADS;
+  auto kern = gemm_wgmma_kernel<BN, Epi, MC>;
+  constexpr int smem = GemmCfg<BN, Epi>::BYTES;
+  constexpr int GEMM_THREADS = GemmCfg<BN, Epi>::THREADS;
   static int max_clusters[16] = {};   // 0 = not queried yet, -1 = unusable
   int& mc = max_clusters[dev.id & 15];
   if (mc == 0) {
@@ -450,8 +403,22 @@ int gemm_swapped_mc(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int ld
   return EZB_OK;
 }
 
-// CTA-pair GEMM launch: 256 x BN tiles, cluster (2,1,1), one pair per TPC.
-template <int BN, class Epi, int KSUB = (BN <= 144 ? 2 : 1)>
+// Cluster launch (2,1,1): the two CTAs of a cluster take consecutive 128-row M tiles of the same N tile, and the W tile is fetched once per
+// cluster and multicast into both (gemm.cuh, MC = 2), so each SM pulls half the weight bytes through L2.  The grid is sized to the clusters
+// that can be resident at once (1 CTA per SM; a GPC with an odd number of free SMs leaves one idle).
+template <class Kern>
+int resident_clusters2(Device& dev, Kern kern, int smem, int threads, int* n) {
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof cfg);
+  cfg.gridDim = dim3(dev.num_sms & ~1); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute at;
+  at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+  cfg.attrs = &at; cfg.numAttrs = 1;
+  EZB_CUDA(cudaOccupancyMaxActiveClusters(n, kern, &cfg));
+  if (*n <= 0) return fail(EZB_ERR_CUDA, "no 2-CTA cluster of this GEMM fits on the device");
+  return EZB_OK;
+}
+template <int BN, class Epi, int KSUB = 1>
 int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
           const typename Epi::Params& ep) {
   if (M <= 0 || N <= 0 || K <= 0) return fail(EZB_ERR_SHAPE, "gemm2: empty problem %d %d %d", M, N, K);
@@ -459,24 +426,24 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
   GemmShape g;
   memset(&g, 0, sizeof g);
   g.M = M; g.N = N;
-  g.dbg = gemm_dbg_buf();
   g.num_n_tiles = (N + BN - 1) / BN;
-  g.num_m_tiles = (M + 2 * GEMM_BM - 1) / (2 * GEMM_BM);
+  g.dbg = gemm_dbg_buf();
+  g.num_m_tiles = ((M + GEMM_BM - 1) / GEMM_BM + 1) & ~1;   // whole clusters: an odd count gets one empty tile (zero-filled, nothing stored)
   g.num_k_blocks = (K + GEMM_BK - 1) / GEMM_BK;
   dev.next_weights(W, (size_t)N * ldw * 2, &g.pf, &g.pf_bytes);
   const CUtensorMap *tA, *tB;
   EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, GEMM_BM, &tA));
-  EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, BN / 2, &tB));
-  auto kern = gemm2_tcgen05_kernel<BN, Epi, KSUB>;
-  constexpr int smem = GemmCfg<BN, Epi, true, KSUB>::BYTES;
-  constexpr int GEMM_THREADS = GemmCfg<BN, Epi, true, KSUB>::THREADS;
-  static bool attr_set[16] = {};
-  if (!attr_set[dev.id & 15]) {
+  EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, McSub<BN>::ROWS, &tB));
+  auto kern = gemm_wgmma_kernel<BN, Epi, 2, KSUB>;
+  constexpr int smem = GemmCfg<BN, Epi, KSUB>::BYTES;
+  constexpr int GEMM_THREADS = GemmCfg<BN, Epi, KSUB>::THREADS;
+  static int clusters[16] = {};
+  if (!clusters[dev.id & 15]) {
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set[dev.id & 15] = true;
+    EZB_TRY(resident_clusters2(dev, kern, smem, GEMM_THREADS, &clusters[dev.id & 15]));
   }
-  const int tiles = g.num_m_tiles * g.num_n_tiles, max_pairs = dev.num_sms / 2;
-  const int pairs = tiles < max_pairs ? tiles : max_pairs;
+  const int tiles = g.num_m_tiles * g.num_n_tiles, max_ctas = 2 * clusters[dev.id & 15];
+  const int ctas = tiles < max_ctas ? tiles : max_ctas;
   GemmProf& gp = gemm_prof();
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (gp.on) {
@@ -488,7 +455,7 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
     gp.flops.push_back(2.0 * (double)M * (double)N * (double)g.num_k_blocks * GEMM_BK);
     EZB_CUDA(cudaEventRecord(e0, st));
   }
-  EZB_TRY(launch_k(kern, dim3(2 * pairs), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, g, ep));
+  EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, g, ep));
   if (gp.on) EZB_CUDA(cudaEventRecord(e1, st));
   return EZB_OK;
 }
@@ -497,8 +464,8 @@ inline int& opt_mlp_fused() {
   static int v = [] { const char* e = getenv("EZB_MLP_FUSED"); return e ? atoi(e) : 0; }();
   return v;
 }
-// One persistent launch for the MLP of a DiT block (gemm.cuh mlp_fused_kernel): GEGLU projection A1[M,K1] W1[N1,K1]^T (packed, BN1 = 256 pair
-// tiles) -> bf16 `mid` -> grid barrier -> output projection mid[M,K2] W2[N2,K2]^T as swap-AB tiles with the EpiLinearT epilogue.
+// One persistent launch for the MLP of a DiT block (gemm.cuh mlp_fused_kernel): GEGLU projection A1[M,K1] W1[N1,K1]^T (packed, BN1 = 256,
+// 2-CTA clusters) -> bf16 `mid` -> grid barrier -> output projection mid[M,K2] W2[N2,K2]^T as swap-AB tiles with the EpiLinearT epilogue.
 template <class Epi1, class Epi2>
 int mlp_fused(Device& dev, cudaStream_t st, const __nv_bfloat16* A1, const __nv_bfloat16* W1, int M, int N1, int K1, const typename Epi1::Params& ep1,
               const __nv_bfloat16* mid, const __nv_bfloat16* W2, int N2, int K2, const typename Epi2::Params& ep2, GridBarrier* bar) {
@@ -508,23 +475,23 @@ int mlp_fused(Device& dev, cudaStream_t st, const __nv_bfloat16* A1, const __nv_
   memset(&g1, 0, sizeof g1);
   memset(&g2, 0, sizeof g2);
   g1.M = M; g1.N = N1;
-  g1.num_n_tiles = (N1 + BN1 - 1) / BN1; g1.num_m_tiles = (M + 2 * GEMM_BM - 1) / (2 * GEMM_BM); g1.num_k_blocks = (K1 + GEMM_BK - 1) / GEMM_BK;
+  g1.num_n_tiles = (N1 + BN1 - 1) / BN1; g1.num_m_tiles = ((M + GEMM_BM - 1) / GEMM_BM + 1) & ~1; g1.num_k_blocks = (K1 + GEMM_BK - 1) / GEMM_BK;
   g2.M = N2; g2.N = M;   // swap-AB: features on the accumulator rows
   g2.num_m_tiles = (N2 + GEMM_BM - 1) / GEMM_BM; g2.num_n_tiles = (M + BN2 - 1) / BN2; g2.num_k_blocks = (K2 + GEMM_BK - 1) / GEMM_BK;
   const CUtensorMap *tA1, *tB1, *tA2, *tB2;
   EZB_TRY(dev.tmaps.get2d(A1, (uint64_t)K1, (uint64_t)M, (uint64_t)K1, GEMM_BM, &tA1));
-  EZB_TRY(dev.tmaps.get2d(W1, (uint64_t)K1, (uint64_t)N1, (uint64_t)K1, BN1 / 2, &tB1));
+  EZB_TRY(dev.tmaps.get2d(W1, (uint64_t)K1, (uint64_t)N1, (uint64_t)K1, McSub<BN1>::ROWS, &tB1));
   EZB_TRY(dev.tmaps.get2d(W2, (uint64_t)K2, (uint64_t)N2, (uint64_t)K2, GEMM_BM, &tA2));
   EZB_TRY(dev.tmaps.get2d(mid, (uint64_t)K2, (uint64_t)M, (uint64_t)K2, BN2, &tB2));
   auto kern = mlp_fused_kernel<BN1, Epi1, Epi2>;
-  constexpr int s1 = GemmCfg<BN1, Epi1, true, 1>::BYTES, s2 = GemmCfg<BN2, Epi2, false>::BYTES, smem = s1 > s2 ? s1 : s2;
-  constexpr int THREADS = GemmCfg<BN1, Epi1, true, 1>::THREADS;
-  static bool attr_set[16] = {};
-  if (!attr_set[dev.id & 15]) {
+  constexpr int s1 = GemmCfg<BN1, Epi1>::BYTES, s2 = GemmCfg<BN2, Epi2>::BYTES, smem = s1 > s2 ? s1 : s2;
+  constexpr int THREADS = GemmCfg<BN1, Epi1>::THREADS;
+  static int clusters[16] = {};
+  if (!clusters[dev.id & 15]) {
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set[dev.id & 15] = true;
+    EZB_TRY(resident_clusters2(dev, kern, smem, THREADS, &clusters[dev.id & 15]));
   }
-  const int grid = dev.num_sms & ~1;   // one CTA per SM, whole pairs: every CTA is resident, so the grid barrier cannot dead-lock
+  const int grid = 2 * clusters[dev.id & 15];   // every CTA is resident, so the grid barrier cannot dead-lock
   return launch_k(kern, dim3(grid), dim3(THREADS), smem, st, 2, *tA1, *tB1, g1, ep1, *tA2, *tB2, g2, ep2, bar);
 }
 

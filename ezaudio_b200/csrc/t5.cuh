@@ -1,7 +1,7 @@
 // T5 (v1.1 / flan-T5, gated-GELU) text encoder: the step BEFORE the denoiser path (SURVEY 8(f) row 3).
 // Reference call site: src/inference.py:38-50 (`text_encoder(input_ids=, attention_mask=).last_hidden_state`), model class
 // transformers.T5EncoderModel (api/ezaudio.py:78-79).  Runs once per generate call on <= 100 tokens per prompt, so it is weight-bandwidth
-// bound (2.4 GB of bf16 weights for flan-T5-XL); the linears reuse the tcgen05 CTA-pair GEMM of the DiT, everything else is small fp32 kernels:
+// bound (2.4 GB of bf16 weights for flan-T5-XL); the linears reuse the wgmma 2-CTA cluster GEMM of the DiT, everything else is small fp32 kernels:
 //   ids -> embedding gather -> 24 x [ RMSNorm+cast -> QKV GEMM -> head permute -> fp32 attention (unscaled, + relative-position bias,
 //   + key mask) -> O GEMM (+ residual) -> RMSNorm+cast -> [wi_1 | wi_0] GEMM -> gelu_new(g) * h -> wo GEMM (+ residual) ] -> RMSNorm.
 #pragma once

@@ -1,7 +1,7 @@
 // Oobleck VAE decoder (stable_vae/models/autoencoders.py:149-190; DecoderBlock :82-113; ResidualUnit :38-61;
 // SnakeBeta stable_vae/models/blocks.py:317-359; weight_norm stable_vae/models/nn/layers.py:9-14).
 // Activations live channels-last ([B, T, C], bf16 tensor-core operands + an fp32 residual stream); every Conv1d /
-// ConvTranspose1d is an implicit GEMM on the tcgen05 kernel (gemm.cuh, conv addressing) with bias, residual add and the
+// ConvTranspose1d is an implicit GEMM on the wgmma kernel (gemm.cuh, conv addressing) with bias, residual add and the
 // NEXT layer's SnakeBeta fused into the epilogue.  Weight-norm is folded once at load time.
 #pragma once
 #include <map>
@@ -81,7 +81,7 @@ __global__ void latent_pack_kernel(const float* __restrict__ z, __nv_bfloat16* _
 // registers), and the 32 per-lane partial sums are reduced with a 31-shuffle transpose-reduction so that lane i ends up with output i.
 // Round 2: the rows are fetched in two batches of 19 unconditional loads (row index clamped, contribution zeroed by a select) -- the
 // round-1 loop tested `0 <= t < T` around every load, which kept ptxas from hoisting any of them: each warp had ONE 256-byte request in
-// flight (488 us = 0.5 TB/s for the 4 x 10 s decode).  Same accumulation order, bit-identical output.
+// flight.  Same accumulation order, bit-identical output.
 template <int KMUL>
 __global__ void __launch_bounds__(128, 3) wave_out_kernel(const __nv_bfloat16* __restrict__ act, const float* __restrict__ w, float* __restrict__ wav, int C, int T) {
   const int lane = threadIdx.x & 31;

@@ -128,7 +128,7 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
     # ---- the loop.  Every step is the same launch sequence on static buffers, so the WHOLE schedule (all steps: ~365 kernels each) is captured
     # once into one CUDA graph per shape / schedule and replayed with a single launch; the per-step Gaussian draws of DDIM (eta > 0) stay in
     # PyTorch -- same generators, same order, same per-step tensor shapes as the step-by-step loop -- and are simply made up front into one
-    # [steps, B, C, L] buffer (round 1 replayed one graph per step: 50 launches and 200 RNG kernels interleaved cost ~0.3 ms of gaps per step).
+    # [steps, B, C, L] buffer (one graph per step would interleave 50 launches and 200 RNG kernels).
     # Everything a captured launch sequence bakes in is in the key: shapes (incl. the context length, which fixes the cross-attention K/V layout and
     # tensor maps), the schedule, the guidance constants, which ControlNet handle (its serial, not id(): ids are recycled) and the
     # library's option epoch (ezb_set_option changes kernel selection).

@@ -1,4 +1,4 @@
-/* libezb200 -- C ABI of the B200-native EzAudio hot path (DiT denoiser step + Oobleck VAE decode).
+/* libezb200 -- C ABI of the H100-native (sm_90a) EzAudio hot path (DiT denoiser step + Oobleck VAE decode).
  *
  * The reference (haidog-yaqub/EzAudio) is pure Python/PyTorch and has no FFI of its own; its drop-in boundary is the
  * Python call surface (SURVEY.md section 8b).  Each entry point below names the reference interface it replaces
@@ -153,22 +153,23 @@ typedef struct {
   void* out_bf16; int32_t ld16; int32_t split_stride;
   int32_t act; const float* act_a; const float* act_b;
 } ezb_test_epilogue;
-/* C = A[M,K] W[N,K]^T through the tcgen05 GEMM; epi_kind 0 = linear epilogue, 1 = GEGLU (packed W). conv_* = 0 for plain. */
+/* C = A[M,K] W[N,K]^T through the wgmma GEMM; epi_kind 0 = linear epilogue, 1 = GEGLU (packed W); 10 / 11 = the same on 2-CTA
+   clusters; 20 = swap-AB. conv_* = 0 for plain. */
 int ezb_test_gemm(int device, const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K, int bn, int epi_kind,
                   const ezb_test_epilogue* e, int conv_taps, int conv_center, int conv_dil, int conv_cin_pad, int conv_T,
                   int conv_B, void* stream);
-/* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tcgen05 kernel the product uses (generation 6 unless the option "attn6" says
-   otherwise); 4 / 6: generation 4 / 6 forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of 128 */
+/* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7: that
+   generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
                        int B, int H, int Lq, int Lk, int dh, int impl, void* stream);
 
-/* runtime switches for A/B measurements and profiling (csrc/host.cuh, csrc/ezb.cu list them with their measured verdicts): e.g. "pair_gemm" (1 =
-   cta_group::2 256-row tiles, default), "attn6" (attention kernel generation / mode, default 5), "ksub2", "ln_variant", "skip" (profiling: kernel
-   classes not launched).  Defaults are the measured-best settings; products never need to call this. */
+/* runtime switches for A/B measurements and profiling (csrc/host.cuh, csrc/ezb.cu list them): e.g. "pair_gemm" (1 = 2-CTA cluster tiles
+   sharing the weight tile, default), "attn6" / "attn7" / "attn_res" (attention variant), "ksub2", "ln_variant", "skip" (profiling: kernel classes not launched).  Products never need to call this. */
 int ezb_set_option(const char* name, int value);
 /* incremented by every ezb_set_option call: hosts that cache captured CUDA graphs key them on it (options change kernel selection) */
 unsigned long long ezb_option_epoch(void);
-/* debugging aid: with option "gemm_debug"=1, CTA 0 of each pair-GEMM accumulates cycle counters; this reads and resets them */
+/* debugging aid: with option "gemm_debug"=1 (library built with EZB_DEBUG=1), CTA 0 of each 2-CTA cluster GEMM accumulates cycle
+   counters (gemm.cuh GemmShape::dbg); this reads and resets them */
 int ezb_debug_read(unsigned long long* out8);
 /* accounting: kernels launched by this library so far (process-wide); per-GEMM CUDA-event timing for bench.py's roofline leg */
 unsigned long long ezb_launch_count(void);

@@ -20,7 +20,7 @@ def checksum(sd):
 
 
 @torch.no_grad()
-def dit_case(ref, name, cfg, B, L, Lc, seed, inpaint, tscalar=None, tvec=None):
+def dit_case(ref, name, cfg, B, L, Lc, seed, inpaint, tscalar=None, tvec=None, out_stride=1):
     sd = weights.synthetic_state_dict(weights.dit_param_shapes(cfg), seed)
     m = refimport.build(ref.MaskDiT, sd, **cfg)
     x = synth.synth_latents(B, L)
@@ -31,14 +31,15 @@ def dit_case(ref, name, cfg, B, L, Lc, seed, inpaint, tscalar=None, tvec=None):
     t = torch.tensor(tscalar) if tvec is None else torch.tensor(tvec, dtype=torch.long)
     gt, gm = (synth.synth_gt(B, L) if inpaint else (None, None))
     out, mae = m(x, t, ctx, context_mask=mask, gt=None if gt is None else gt.clone(), mae_mask_infer=gm)
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), out=out.numpy(), sd_checksum=checksum(sd),
+    # configuration-scale cases keep every `out_stride`-th element of the last axis (files stay below 1 MB; tests compare the same view)
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), out=out[..., ::out_stride].contiguous().numpy(), sd_checksum=checksum(sd),
                         x_checksum=float(x.double().abs().sum()), seed=seed, B=B, L=L, Lc=Lc,
-                        inpaint=inpaint, t=t.numpy())
+                        inpaint=inpaint, t=t.numpy(), out_stride=out_stride)
     print(name, tuple(out.shape), float(out.std()), float(out.abs().max()))
 
 
 @torch.no_grad()
-def controlnet_case(ref, name, cfg, B, L, Lc, seed, skip_stride=1):
+def controlnet_case(ref, name, cfg, B, L, Lc, seed, skip_stride=1, out_stride=1):
     cn = synth.CONTROLNET
     sd = weights.synthetic_state_dict(weights.dit_param_shapes(cfg), seed)
     sd_cn = weights.synthetic_state_dict(weights.controlnet_param_shapes(cfg, cn), seed + 1)
@@ -52,19 +53,20 @@ def controlnet_case(ref, name, cfg, B, L, Lc, seed, skip_stride=1):
     skips = c(x257, t, ctx, context_mask=mask, condition=cond, conditioning_scale=0.8)
     out = m.model(x257, t, ctx, context_mask=mask, controlnet_skips=list(skips))
     # config-scale cases keep every `skip_stride`-th token row of the two stored skips (a full XL skip is 4.6 MB)
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), out=out.numpy(), skip0=skips[0][:, ::skip_stride].numpy(),
-                        skip_last=skips[-1][:, ::skip_stride].numpy(), sd_checksum=checksum(sd) + checksum(sd_cn), seed=seed,
-                        B=B, L=L, Lc=Lc, skip_stride=skip_stride)
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), out=out[..., ::out_stride].contiguous().numpy(),
+                        skip0=skips[0][:, ::skip_stride].contiguous().numpy(), skip_last=skips[-1][:, ::skip_stride].contiguous().numpy(),
+                        sd_checksum=checksum(sd) + checksum(sd_cn), seed=seed, B=B, L=L, Lc=Lc, skip_stride=skip_stride, out_stride=out_stride)
     print(name, tuple(out.shape), float(out.std()), float(skips[-1].std()))
 
 
 @torch.no_grad()
-def vae_case(ref, name, dcfg, B, L, seed):
+def vae_case(ref, name, dcfg, B, L, seed, out_stride=1):
     sd = weights.synthetic_state_dict(weights.vae_decoder_param_shapes(dcfg), seed)
     m = refimport.build(ref.OobleckDecoder, {k[len("decoder."):]: v for k, v in sd.items()}, **dcfg)
     z = synth.synth_latents(B, L, dcfg["latent_dim"], seed=31)
     wav = m(z)
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), out=wav.numpy(), sd_checksum=checksum(sd), seed=seed, B=B, L=L)
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), out=wav[..., ::out_stride].contiguous().numpy(), sd_checksum=checksum(sd), seed=seed,
+                        B=B, L=L, out_stride=out_stride)
     print(name, tuple(wav.shape), float(wav.std()), float(wav.abs().max()))
 
 
@@ -135,10 +137,30 @@ def main():
     dit_case(ref, "dit_L_c1", synth.model_cfg("l"), B=1, L=256, Lc=100, seed=1, inpaint=False, tscalar=999)  # BASELINE config 1
     dit_case(ref, "dit_XL", synth.model_cfg("xl"), B=2, L=500, Lc=100, seed=2, inpaint=False, tscalar=479)
     # ---- configuration-scale cases (BASELINE configs C4 / C5 and the 10-s codec the benchmark times)
-    controlnet_case(ref, "controlnet_XL", synth.model_cfg("xl"), B=2, L=500, Lc=100, seed=2, skip_stride=10)      # C4 shapes (B_eff = 2)
-    dit_case(ref, "dit_XL_inpaint_30s", synth.model_cfg("xl"), B=2, L=1500, Lc=100, seed=2, inpaint=True, tvec=[989, 9])  # C5 shapes
-    vae_case(ref, "vae_full_10s", synth.VAE_DECODER, B=2, L=500, seed=6)
+    controlnet_case(ref, "controlnet_XL", synth.model_cfg("xl"), B=2, L=500, Lc=100, seed=2, skip_stride=20, out_stride=2)      # C4 shapes (B_eff = 2)
+    dit_case(ref, "dit_XL_inpaint_30s", synth.model_cfg("xl"), B=2, L=1500, Lc=100, seed=2, inpaint=True, tvec=[989, 9], out_stride=2)  # C5 shapes
+    vae_case(ref, "vae_full_10s", synth.VAE_DECODER, B=2, L=500, seed=6, out_stride=3)
     vae_enc_case(ref, "vae_enc_full_10s", synth.VAE_ENCODER, B=1, T=480 * 500, seed=8)
+    param_shapes_case(ref, "reference_param_shapes")
+
+
+def param_shapes_case(ref, name):
+    """State-dict key -> shape of the reference MaskDiT (XL, L) and DiTControlNet (L), as gzipped JSON: the weight wire format the loaders accept."""
+    import contextlib
+    import copy
+    import gzip
+    import io
+    import json
+    out = {}
+    for size in ("xl", "l"):
+        with torch.device("meta"), contextlib.redirect_stdout(io.StringIO()):
+            m = ref.MaskDiT(**copy.deepcopy(synth.model_cfg(size)))
+        out[f"dit_{size}"] = {k: list(v.shape) for k, v in m.state_dict().items()}
+    with torch.device("meta"), contextlib.redirect_stdout(io.StringIO()):
+        c = ref.DiTControlNet(**copy.deepcopy(synth.model_cfg("l")), **copy.deepcopy(synth.CONTROLNET))
+    out["controlnet_l"] = {k: list(v.shape) for k, v in c.state_dict().items()}
+    with gzip.open(os.path.join(OUT, name + ".json.gz"), "wt") as f:
+        json.dump(out, f, separators=(",", ":"), sort_keys=True)
 
 
 if __name__ == "__main__":

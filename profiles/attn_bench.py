@@ -1,5 +1,6 @@
-"""Attention micro-benchmark through the C-ABI test hook: kernel v4 (one thread per query row) vs v5 (two threads per row), q / k row pitch 128 vs 80
-elements (dh = 72).  CUDA events over 20 back-to-back launches; the inputs of one call (Q, K, V^T: 20-60 MB) stay in the 126 MB L2 like in the step."""
+"""Attention micro-benchmark through the C-ABI test hook (attention_mma.cuh variants, q / k row pitch 128 vs 80 elements for dh = 72).  CUDA events
+over 20 back-to-back launches; the algorithmic FLOPs (4 Lq Lk dh per head) are also given as a share of the dense bf16 tensor peak.
+  python profiles/attn_bench.py [res_poly_pp_bits] [attn6] [attn7]        # no arguments: the product's default variant"""
 import os
 import sys
 
@@ -9,6 +10,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ezaudio_b200 import _lib  # noqa: E402
 
 L = _lib.lib()
+PEAK = float(os.environ.get("PEAK_TFLOPS", 989.0))   # H100 SXM data sheet, dense bf16
+print(torch.cuda.get_device_name(0))
 
 
 def run(B, H, Lq, Lk, dh, masked, label, impl, reps=20):
@@ -37,16 +40,17 @@ def run(B, H, Lq, Lk, dh, masked, label, impl, reps=20):
     torch.cuda.synchronize()
     ms = t0.elapsed_time(t1) / reps
     fl = 4.0 * B * H * Lq * Lk * dh
-    print(f"{label:14s} impl {impl:3d} B{B} H{H} Lq{Lq} Lk{Lk} dh{dh}: {ms * 1e3:7.1f} us  {fl / ms / 1e9:6.1f} TFLOP/s")
+    print(f"{label:14s} impl {impl:3d} B{B} H{H} Lq{Lq} Lk{Lk} dh{dh}: {ms * 1e3:7.1f} us  {fl / ms / 1e9:6.1f} TFLOP/s "
+          f"({fl / ms / 1e9 / PEAK:.3f} of {PEAK:.0f})")
 
 
 MMA2 = int(sys.argv[1]) if len(sys.argv) > 1 else 0
 L.ezb_set_option(b"attn_res", (MMA2 >> 1) & 1)
 L.ezb_set_option(b"attn_poly", (MMA2 >> 2) & 1)
 L.ezb_set_option(b"attn_pp", (MMA2 >> 3) & 1)
-A6 = int(sys.argv[2]) if len(sys.argv) > 2 else 0   # attention_tc6.cuh: 1 on, +2 MUFU token, +4 P in two halves
+A6 = int(sys.argv[2]) if len(sys.argv) > 2 else 5   # bit 0 generation 6 (else 4), +2 FMA-pipe exp2 on odd warps, +4 P V after each half block
 L.ezb_set_option(b"attn6", A6)
-A7 = int(sys.argv[3]) if len(sys.argv) > 3 else 0   # attention_tc7.cuh
+A7 = int(sys.argv[3]) if len(sys.argv) > 3 else 0   # generation 7: 128-key blocks
 L.ezb_set_option(b"attn7", A7)
 print("attn6 =", A6, "attn7 =", A7)
 print("attn_res =", (MMA2 >> 1) & 1, "attn_poly =", (MMA2 >> 2) & 1, "attn_pp =", (MMA2 >> 3) & 1)

@@ -1,5 +1,5 @@
-"""GEMM micro-benchmark through the C-ABI test hook: TFLOP/s per kernel variant on the DiT shapes, plus the cycle
-counters of CTA 0 (MMA wait on full / tempty, producer wait on empty, epilogue wait / busy)."""
+"""GEMM micro-benchmark through the C-ABI test hook: TFLOP/s per kernel variant on the DiT shapes, plus the cycle counters of CTA 0 of the
+2-CTA cluster launches (gemm.cuh GemmShape::dbg; build with EZB_DEBUG=1 for them to count)."""
 import ctypes as C
 import math
 import os
@@ -48,8 +48,8 @@ def run(M, N, K, bn, kind, label, resid=False, reps=20):
     L.ezb_debug_read(dbg)
     d = [v / reps for v in dbg[:6]]
     tf = 2.0 * M * N * K / ms / 1e9
-    print(f"{label:34s} M{M} N{N} K{K} bn{bn}: {ms * 1e3:7.1f} us  {tf:7.1f} TF/s | cta0 cycles: total {d[5]:.0f} mma_wait_full {d[0]:.0f} "
-          f"mma_wait_tempty {d[1]:.0f} prod_wait_empty {d[2]:.0f} epi_wait {d[3]:.0f} epi_busy {d[4]:.0f}")
+    print(f"{label:34s} M{M} N{N} K{K} bn{bn}: {ms * 1e3:7.1f} us  {tf:7.1f} TF/s | cta0 cycles: total {d[5]:.0f} mainloop {d[0]:.0f} "
+          f"acc_wait {d[1]:.0f} prod_wait_empty {d[2]:.0f} epi_busy {d[4]:.0f}")
 
 
 M = 4000

@@ -27,6 +27,13 @@ def load_golden(name):
     return np.load(os.path.join(GOLDEN, name + ".npz"))
 
 
+def golden_view(g, x):
+    """The part of an output `x` that golden `g` stores: configuration-scale goldens keep every `out_stride`-th element of the last axis
+    of `out` (the files stay below 1 MB)."""
+    s = int(g["out_stride"]) if "out_stride" in g.files else 1
+    return x[..., ::s]
+
+
 def dit_case_inputs(name):
     """-> cfg, sd, dict(x, t, ctx, mask, gt, gt_mask), golden npz."""
     mk, kw = DIT_CASES[name]

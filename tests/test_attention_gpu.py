@@ -1,12 +1,12 @@
 """Attention kernels vs a plain PyTorch fp32 reference of the same op (softmax(q k^T/sqrt(dh) + key mask) v).
 impl 0 = fp32 CUDA-core kernel (parity mode): tolerance 2e-2 is the bf16 rounding of the OUTPUT only (values O(1));
-impl 1 = tcgen05 kernel: q, k, v and P are bf16 operands -> tolerance 3e-2 abs on O(1) outputs."""
+impl 1 = tensor-core kernel: q, k, v and P are bf16 operands -> tolerance 3e-2 abs on O(1) outputs."""
 import math
 
 import pytest
 import torch
 
-ATTN6_DEFAULT = 5   # csrc/attention_tc6.cuh opt_attn6(): generation-6 kernel with P handed over in two halves
+ATTN6_DEFAULT = 5   # csrc/attention_mma.cuh opt_attn6(): generation 6 (bits 1 / 2 have no effect on sm_90a)
 
 pytestmark = pytest.mark.gpu
 
@@ -19,8 +19,8 @@ def _ref(q, k, v, mask):
     return o.permute(0, 2, 1, 3).reshape(q.shape[0], q.shape[2], -1)
 
 
-# 0 = fp32 CUDA-core kernel (parity mode); 1 = the tcgen05 kernel the product uses (generation 6, attention_tc6.cuh, unless the option attn6 says
-# otherwise); 4 = generation 4 (attention_tc4.cuh); +100 = q / k rows of 80 elements for dh = 72 (160-byte pitch) instead of 128
+# 0 = fp32 CUDA-core kernel (parity mode); 1 = the tensor-core kernel the product uses (generation 6 of attention_mma.cuh unless the options say
+# otherwise); 4 = generation 4 (128 query rows per CTA); +100 = q / k rows of 80 elements for dh = 72 (160-byte pitch) instead of 128
 @pytest.mark.parametrize("impl", [0, 1, 4, 101, 104])
 @pytest.mark.parametrize("B,H,Lq,Lk,dh,masked", [(2, 4, 500, 500, 72, False), (2, 3, 256, 256, 64, False), (3, 2, 500, 100, 72, True),
                                                  (2, 2, 40, 12, 72, True), (1, 2, 130, 130, 64, False), (1, 16, 1500, 1500, 72, False),
@@ -73,8 +73,8 @@ def _run(L, _lib, args, mask, out, B, H, Lq, Lk, dh, impl):
                                                  (2, 3, 256, 256, 64, False), (8, 16, 500, 500, 72, False), (2, 5, 400, 512, 72, "grow"), (5, 3, 300, 100, 64, True),
                                                  (16, 16, 500, 500, 72, False), (2, 2, 130, 385, 72, True)])
 def test_attention_kv_resident(B, H, Lq, Lk, dh, masked):
-    """attn4 with the K / V^T key blocks of a head resident in shared memory (option attn_res; falls back above 512 keys): odd and even numbers
-    of query tiles per head, one to four key blocks, more heads than SMs (two waves of CTAs), masks, growth."""
+    """Generation 4 with the K / V^T key blocks of a head resident in shared memory (option attn_res; falls back above 512 keys): odd and even
+    numbers of query tiles per head, one to eight key blocks, more heads than SMs (two waves of CTAs), masks, growth."""
     from ezaudio_b200 import _lib
     L = _lib.lib()
     _lib.check(L.ezb_set_option(b"attn6", 0))   # generation-4 kernel (the default is generation 6)
@@ -93,8 +93,8 @@ def test_attention_kv_resident(B, H, Lq, Lk, dh, masked):
                                                  (16, 16, 500, 500, 72, False), (2, 2, 130, 385, 72, True), (1, 1, 100, 300, 72, False), (1, 3, 128, 128, 72, True)])
 @pytest.mark.parametrize("res", [0, 1])
 def test_attention_mufu_token(B, H, Lq, Lk, dh, masked, res):
-    """attn4 with the exponent phases of the two softmax groups strictly alternating (option attn_pp): CTAs with an odd and an even number of
-    items (the group without a last item keeps passing the token), a single item, one to twelve key blocks, with and without resident K / V^T."""
+    """Generation 4 with the option attn_pp set (it scheduled the softmax groups of the sm_100a kernel and leaves the sm_90a kernel unchanged):
+    a single query tile, one to twelve key blocks, with and without resident K / V^T."""
     from ezaudio_b200 import _lib
     L = _lib.lib()
     _lib.check(L.ezb_set_option(b"attn6", 0))   # generation-4 kernel (the default is generation 6)
@@ -115,9 +115,9 @@ def test_attention_mufu_token(B, H, Lq, Lk, dh, masked, res):
                                                  (16, 16, 500, 500, 72, False), (2, 2, 130, 385, 72, True), (1, 1, 100, 300, 72, False), (1, 3, 128, 128, 72, True)])
 @pytest.mark.parametrize("mode", [0, 1, 3, 5, 7])
 def test_attention_gen6(B, H, Lq, Lk, dh, masked, mode):
-    """attn6 (attention_tc6.cuh: chunked two-pass softmax, packed f32x2 arithmetic; bit 1 of the option = MUFU token between the two softmax
-    groups, bit 2 = P handed to the MMA warp in two halves): every mode on odd / even item counts per CTA, a single item, one to twelve key
-    blocks, key masks, score growth (in-place O rescale before the exponent phase), dh = 64 and 72, both q / k row pitches."""
+    """Every value of the option attn6 (bit 0: generation 6, 64 query rows per CTA, else generation 4; bits 1 and 2 are accepted and change
+    nothing on sm_90a): a single query tile, one to twelve key blocks, key masks, score growth (O rescale), dh = 64 and 72, both q / k row
+    pitches."""
     from ezaudio_b200 import _lib
     L = _lib.lib()
     _lib.check(L.ezb_set_option(b"attn6", mode))
@@ -134,9 +134,7 @@ def test_attention_gen6(B, H, Lq, Lk, dh, masked, mode):
                                                  (16, 16, 500, 500, 72, False), (2, 2, 130, 385, 72, True), (1, 1, 100, 300, 72, False), (1, 3, 128, 128, 72, True),
                                                  (3, 5, 200, 65, 72, True), (1, 2, 640, 192, 64, False), (37, 4, 512, 512, 72, False)])
 def test_attention_gen7(B, H, Lq, Lk, dh, masked):
-    """attn7 (attention_tc7.cuh: 64-key score blocks, two S buffers per group, scores issued two blocks ahead, output stores issued by the Q producer
-    warp): odd / even item counts per CTA, a single item, an odd number of 64-key blocks per item (385, 65, 192 keys), a lone key in the last block,
-    up to 24 blocks, key masks, score growth (in-place O rescale), dh = 64 and 72, both q / k row pitches, Lk <= 64 (falls back to generation 6),
-    exactly four items on every CTA."""
+    """Generation 7 (128-key blocks): partial last blocks (385, 65, 192 keys), a lone key in the last block, up to 12 blocks, key masks, score
+    growth (O rescale), dh = 64 and 72, both q / k row pitches, Lk below one block, many CTAs."""
     test_attention(7, B, H, Lq, Lk, dh, masked)
     test_attention(107, B, H, Lq, Lk, dh, masked)

@@ -29,7 +29,7 @@ def _run_case(name, precision):
     out, mae = m(inp["x"].to(dev), inp["t"], inp["ctx"].to(dev), context_mask=inp["mask"].to(dev), gt=gt, mae_mask_infer=gm)
     torch.cuda.synchronize()
     ref = torch.from_numpy(g["out"])
-    err = (out.cpu() - ref).abs()
+    err = (helpers.golden_view(g, out.cpu()) - ref).abs()
     assert torch.isfinite(out).all()
     print(f"[parity] {name} [{precision}]: max-abs {float(err.max()):.3e} mean-abs {float(err.mean()):.3e} (ref std {float(ref.std()):.3f})")
     return float(err.max()), float(err.mean())

@@ -53,7 +53,7 @@ def test_dit_folded_matches_reference(name):
         counts[fold] = _launches() - n0
         outs[fold] = out.cpu()
     ref = torch.from_numpy(g["out"])
-    err = (outs[1] - ref).abs()
+    err = (helpers.golden_view(g, outs[1]) - ref).abs()
     print(f"[parity] {name} [bf16, LayerNorm folded]: max-abs {float(err.max()):.3e} mean-abs {float(err.mean()):.3e}; launches {counts[1]} vs {counts[0]} unfolded; "
           f"folded vs unfolded max-abs {float((outs[1] - outs[0]).abs().max()):.3e}")
     assert float(err.max()) < 6e-2 and float(err.mean()) < 1.2e-2
@@ -93,7 +93,7 @@ def test_controlnet_folded_matches_reference(name):
     s0, s1 = torch.from_numpy(g["skip0"]), torch.from_numpy(g["skip_last"])
     e0 = float((skips[0][:, ::stride].cpu() - s0).abs().max())
     e1 = float((skips[-1][:, ::stride].cpu() - s1).abs().max())
-    eo = float((out.cpu() - torch.from_numpy(g["out"])).abs().max())
+    eo = float((helpers.golden_view(g, out.cpu()) - torch.from_numpy(g["out"])).abs().max())
     print(f"[parity] {name} [bf16, LayerNorm folded]: skip0 {e0:.3e} skip_last {e1:.3e} (std {float(s1.std()):.2f}) out {eo:.3e}")
     assert e0 < 6e-2 * max(1.0, float(s0.std())) and e1 < 6e-2 * max(1.0, float(s1.std())) and eo < 6e-2
 
@@ -132,7 +132,7 @@ def test_loop_graphs_and_short_clips_with_fold():
         assert e_ref < 0.25 and e_pair < 0.25
 
 
-DEFAULTS = {"ln_fold": FOLD_DEFAULT, "attn6": 5, "attn_pp": 0, "dhp80": 1, "heads_direct": 0, "ln_tail": 0, "mlp_fused": 0, "ln_variant": 2, "ksub2": 1, "cq_single": 0, "mlp2_pair": 0,
+DEFAULTS = {"ln_fold": FOLD_DEFAULT, "attn6": 5, "attn_pp": 0, "dhp80": 1, "heads_direct": 0, "ln_tail": 0, "mlp_fused": 0, "ln_variant": 2, "ksub2": 0, "cq_single": 0, "mlp2_pair": 0,
             "attn_res": 0, "w_prefetch": 0, "attn7": 0}
 
 
@@ -151,12 +151,12 @@ def options(**kw):
 
 OPTION_SETS = [("heads_direct", dict(heads_direct=1)), ("dhp128", dict(dhp80=0)), ("attn_gen4", dict(attn6=0)), ("all", dict(attn6=7, dhp80=1, heads_direct=1, ln_fold=1)),
                ("ln_tail", dict(ln_tail=1)), ("ln_variant1", dict(ln_variant=1)), ("mlp_fused", dict(mlp_fused=1)), ("mlp_fused+ln_tail+dhp80", dict(mlp_fused=1, ln_tail=1, dhp80=1)),
-               ("attn_gen4_token", dict(attn6=0, attn_pp=1)), ("ksub2_qkv", dict(ksub2=3)), ("ksub2_off", dict(ksub2=0)), ("ln_variant0", dict(ln_variant=0)),
+               ("attn_gen4_token", dict(attn6=0, attn_pp=1)), ("ksub2_qkv", dict(ksub2=3)), ("ksub2_off", dict(ksub2=0)), ("ksub2_geglu", dict(ksub2=1)), ("ln_variant0", dict(ln_variant=0)),
                ("cq_single", dict(cq_single=1)), ("mlp2_pair", dict(mlp2_pair=1)), ("attn_gen4_res", dict(attn6=0, attn_res=1)), ("attn6_plain", dict(attn6=1)),
                ("attn6_token", dict(attn6=3)), ("w_prefetch", dict(w_prefetch=1)), ("attn7", dict(attn7=1))]
 # every option set on the tiny models and on EzAudio-XL (the benchmarked configuration); the two other large goldens (30-s inpainting: L = 1500, 12 key tiles;
 # EzAudio-L: dh = 64) only with the sets that change what those shapes exercise -- the full cross product costs 8 GPU-minutes of weight loading
-HEAVY_KEYS = {"attn_gen4", "all", "mlp_fused", "attn6_plain", "attn7", "ksub2_off"}
+HEAVY_KEYS = {"attn_gen4", "all", "mlp_fused", "attn6_plain", "attn7", "ksub2_off", "ksub2_geglu"}
 OPTION_CASES = [pytest.param(name, opts, id=f"{name}-{oid}") for oid, opts in OPTION_SETS
                 for name in ("dit_tiny72", "dit_tiny64", "dit_tiny72_inpaint", "dit_XL", "dit_XL_inpaint_30s", "dit_L_c1")
                 if name not in ("dit_XL_inpaint_30s", "dit_L_c1") or oid in HEAVY_KEYS]
@@ -164,7 +164,7 @@ OPTION_CASES = [pytest.param(name, opts, id=f"{name}-{oid}") for oid, opts in OP
 
 @pytest.mark.parametrize("name,opts", OPTION_CASES)
 def test_fast_path_options_keep_parity(name, opts):
-    """Every fast-path variant behind a runtime switch (q/k epilogue without smem staging, 80-element q/k rows, attention generations 4 / 6 and their modes, folded LayerNorm)
+    """Every fast-path variant behind a runtime switch (q/k epilogue without smem staging, 80-element q/k rows, attention generations 4 / 6 / 7 and their options, folded LayerNorm)
     holds the fast mode's tolerance against the reference goldens, alone and all together."""
     from ezaudio_b200.dit import MaskDiT
     cfg, sd, inp, g = helpers.dit_case_inputs(name)
@@ -179,7 +179,7 @@ def test_fast_path_options_keep_parity(name, opts):
             out2, _ = m(inp["x"].cuda(), inp["t"], inp["ctx"].cuda(), context_mask=inp["mask"].cuda(), gt=gt, mae_mask_infer=gm)
             torch.cuda.synchronize()
             assert torch.equal(out, out2)
-    err = (out.cpu() - torch.from_numpy(g["out"])).abs()
+    err = (helpers.golden_view(g, out.cpu()) - torch.from_numpy(g["out"])).abs()
     print(f"[parity] {name} [bf16, {opts}]: max-abs {float(err.max()):.3e} mean-abs {float(err.mean()):.3e}")
     assert float(err.max()) < 6e-2 and float(err.mean()) < 1.2e-2
 
@@ -223,4 +223,4 @@ def test_ln_tail_bit_identical_and_controlnet():
             res[tail] = (out.clone(), plain.clone(), skips[-1].clone(), lat.clone())
     for a, b in zip(res[0], res[1]):
         assert torch.equal(a, b)
-    assert float((res[1][0].cpu() - torch.from_numpy(g["out"])).abs().max()) < 6e-2
+    assert float((helpers.golden_view(g, res[1][0].cpu()) - torch.from_numpy(g["out"])).abs().max()) < 6e-2

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM kernel vs a plain PyTorch fp32 reference of the same op (bf16-rounded operands, fp32 math).
+"""wgmma GEMM kernel vs a plain PyTorch fp32 reference of the same op (bf16-rounded operands, fp32 math).
 Tolerance: the kernel accumulates the same bf16 products in fp32, so only summation order differs:
 |err| <= 2e-3 * sqrt(K/1024) on O(1..30) outputs for fp32 out; bf16 outputs add one bf16 rounding (rel 2^-8)."""
 import ctypes as C
@@ -118,7 +118,7 @@ def test_gemm_conv_addressing(Cin, Cout, taps, dil, T, B):
 @pytest.mark.parametrize("M,N,K,bn", [(4000, 1152, 1152, 128), (300, 144, 144, 128), (4000, 1152, 4608, 128), (1000, 3456, 1152, 256), (129, 256, 64, 256),
                                       (777, 2304, 264, 128)])
 def test_pair_gemm_f32_out(M, N, K, bn):
-    """CTA-pair (tcgen05 cta_group::2) kernel, same oracle as the single-CTA one."""
+    """2-CTA cluster kernel (W tile multicast to both CTAs), same oracle as the single-CTA one."""
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     A = torch.randn(M, K, device="cuda", generator=g).bfloat16()
     W = (torch.randn(N, K, device="cuda", generator=g) / math.sqrt(K)).bfloat16()

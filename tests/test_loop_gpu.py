@@ -68,7 +68,7 @@ def test_controlnet_matches_reference_golden(name, precision, tol):
     s0, s1 = torch.from_numpy(g["skip0"]), torch.from_numpy(g["skip_last"])
     e0 = float((skips[0][:, ::stride].cpu() - s0).abs().max())
     e1 = float((skips[-1][:, ::stride].cpu() - s1).abs().max())
-    eo = float((out.cpu() - torch.from_numpy(g["out"])).abs().max())
+    eo = float((helpers.golden_view(g, out.cpu()) - torch.from_numpy(g["out"])).abs().max())
     print(f"[parity] {name} [{precision}]: skip0 {e0:.3e} (std {float(s0.std()):.2f}) skip_last {e1:.3e} (std {float(s1.std()):.2f}) out {eo:.3e}")
     # the tolerances are stated for tensors of std ~ 1 (the DiT output); the deepest ControlNet skip of the XL model has std ~ 1.9
     assert e0 < tol * max(1.0, float(s0.std())) and e1 < tol * max(1.0, float(s1.std())) and eo < tol, (e0, e1, eo)
