@@ -38,6 +38,14 @@ class TestEpilogue(C.Structure):
                 ("split_stride", C.c_int32), ("act", C.c_int32), ("act_a", C.c_void_p), ("act_b", C.c_void_p)]
 
 
+class TestHeadsArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("B", "L", "D", "H", "dh", "nsec")] + [("kinds", C.c_int32 * 3)] + \
+               [(n, C.c_void_p) for n in ("norm_q", "norm_k", "inv_freq")] + [("rope", C.c_int32)] + \
+               [(n, C.c_void_p) for n in ("q", "k", "vt")] + [(n, C.c_int32) for n in ("ld_qk", "dvp", "Lpad")] + \
+               [("fold_st", C.c_void_p), ("fold_slots", C.c_int32), ("fold_ld_st", C.c_int32), ("fold_u", C.c_void_p),
+                ("fold_v", C.c_void_p), ("variant", C.c_int32)]
+
+
 _lib = None
 
 _VP, _I, _F = C.c_void_p, C.c_int, C.c_float
@@ -78,6 +86,8 @@ _SIGS = {
     "ezb_prof_gemm_stats": ([C.c_double, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
     "ezb_test_gemm": ([_I, _VP, _I, _VP, _I, _I, _I, _I, _I, _I, C.POINTER(TestEpilogue), _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_test_attention": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_test_heads": ([_I, _VP, _VP, C.POINTER(TestHeadsArgs), _VP], _I),
+    "ezb_test_mlp": ([_I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP], _I),
 }
 EXPORTS = tuple(_SIGS)
 

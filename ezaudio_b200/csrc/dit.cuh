@@ -605,27 +605,17 @@ struct Dit {
     e.out[0] = qo; e.out[1] = ko; e.out[2] = vto;
     e.ld_qk = DHP; e.dvp = DVP; e.Lpad = Lpad;
     const bool direct = opt_heads_direct() != 0, fo = fin != nullptr;
-#define EZB_HEADS(BN_, DH_, HPT_, N_)                                                                                                          \
-  (fo ? (direct ? gemm2<BN_, EpiHeads<DH_, HPT_, true, true>>(*dev, st, A, D, W, D, M, N_, D, e) : gemm2<BN_, EpiHeads<DH_, HPT_, false, true>>(*dev, st, A, D, W, D, M, N_, D, e)) \
-      : (direct ? gemm2<BN_, EpiHeads<DH_, HPT_, true, false>>(*dev, st, A, D, W, D, M, N_, D, e) : gemm2<BN_, EpiHeads<DH_, HPT_, false, false>>(*dev, st, A, D, W, D, M, N_, D, e)))
-    if (qkv3_bn > 0 && N == 3 * D && dh == 72 && opt_heads_dbg() && !fo) {   // profiling instantiation: parts of the epilogue removed
-      e.dbg = opt_heads_dbg();
-      return gemm2<224, EpiHeads<72, 3, false, false, true>>(*dev, st, A, D, W, D, M, H * 224, D, e);
-    }
+    int variant;
     if (qkv3_bn > 0 && N == 3 * D) {  // packed self-attention QKV: three heads per tile
-      if (dh == 72 && (opt_ksub2() & 2) && !fo) return gemm2<224, EpiHeads<72, 3, true, false>, 2>(*dev, st, A, D, W, D, M, H * 224, D, e);   // 128-deep slots (needs the staging-free epilogue)
-      if (dh == 72) return EZB_HEADS(224, 72, 3, H * 224);
-      return EZB_HEADS(192, 64, 3, H * 192);
+      if (dh == 72 && opt_heads_dbg() && !fo) { e.dbg = opt_heads_dbg(); variant = HEADS_PACKED3; }   // profiling instantiation
+      else if (dh == 72 && (opt_ksub2() & 2) && !fo) variant = HEADS_PACKED3_KSUB2;
+      else variant = direct ? HEADS_PACKED3_DIRECT : HEADS_PACKED3;
+    } else if (!pair || (opt_cq_single() && !fo && N == D && dh == 72)) {   // cross-Q as 256 single-CTA tiles of 128 x 144 (1.73 waves of half-size tiles)
+      variant = HEADS_SINGLE;
+    } else {
+      variant = direct ? HEADS_PAIR_DIRECT : HEADS_PAIR;
     }
-    if (pair && opt_cq_single() && !fo && N == D && dh == 72)   // cross-Q as 256 single-CTA tiles of 128 x 144 (1.73 waves of half-size tiles)
-      return gemm<144, EpiHeads<72>>(*dev, st, A, D, W, D, M, N, D, e);
-    if (pair) {
-      if (dh == 72) return EZB_HEADS(144, 72, 2, N);
-      return EZB_HEADS(128, 64, 2, N);
-    }
-#undef EZB_HEADS
-    if (dh == 72) return gemm<144, EpiHeads<72>>(*dev, st, A, D, W, D, M, N, D, e);
-    return gemm<128, EpiHeads<64>>(*dev, st, A, D, W, D, M, N, D, e);
+    return heads_gemm(*dev, st, A, W, M, N, dh, variant, e);
   }
   // GEMM whose output feeds qk_prep: bf16 [M,N] in fast mode, fp32 in parity mode
   int lin_to_qkv(cudaStream_t st, const bf16* A, int K, const bf16* W, int M, int N) {

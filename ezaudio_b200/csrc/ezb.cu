@@ -69,6 +69,13 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
     }
     return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm pair: bn=%d", bn);
   }
+  if (epi_kind == 12) {  // the MLP's GEGLU GEMM with 128-deep ring slots (option ksub2 bit 0)
+    if (cp || bn != 256) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm: 128-deep slots exist for the plain bn=256 cluster GEGLU only");
+    EpiGegluParams p;
+    memset(&p, 0, sizeof p);
+    p.bias = e->bias; p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(e->out_bf16); p.ld16 = e->ld16; p.split_stride = e->split_stride;
+    return gemm2<256, EpiGeglu<256>, 2>(dev, st, a, lda, w, ldw, M, N, K, p);
+  }
   if (epi_kind == 0) {
     EpiLinearParams p = to_epi(e);
     if (bn == 64) return gemm<64, EpiLinear<64>>(dev, st, a, lda, w, ldw, M, N, K, p, cp);
@@ -82,6 +89,117 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
     if (bn == 256) return gemm<256, EpiGeglu<256>>(dev, st, a, lda, w, ldw, M, N, K, p, cp);
   }
   return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm: bn=%d epi=%d", bn, epi_kind);
+}
+
+__attribute__((visibility("default"))) int ezb_test_heads(int device, const void* A, const float* W, const ezb_test_heads_args* a, void* stream) {
+  if (!A || !W || !a) return fail(EZB_ERR_ARG, "ezb_test_heads: null pointer");
+  const int B = a->B, L = a->L, D = a->D, H = a->H, dh = a->dh, nsec = a->nsec, variant = a->variant;
+  if (dh != 64 && dh != 72) return fail(EZB_ERR_SHAPE, "ezb_test_heads: head dimension %d (64 or 72)", dh);
+  if (H < 2 || H % 2) return fail(EZB_ERR_SHAPE, "ezb_test_heads: %d heads (a positive even count)", H);
+  if (D != H * dh) return fail(EZB_ERR_SHAPE, "ezb_test_heads: D %d != H %d x dh %d", D, H, dh);
+  if (B < 1 || L < 1 || (long long)B * L > (1 << 24)) return fail(EZB_ERR_SHAPE, "ezb_test_heads: B %d L %d", B, L);
+  if (nsec < 1 || nsec > 3) return fail(EZB_ERR_SHAPE, "ezb_test_heads: %d sections", nsec);
+  if (a->ld_qk < dh || a->ld_qk % 8) return fail(EZB_ERR_SHAPE, "ezb_test_heads: q / k pitch %d (>= dh %d, a multiple of 8)", a->ld_qk, dh);
+  if (a->Lpad < L) return fail(EZB_ERR_SHAPE, "ezb_test_heads: V^T pitch %d < L %d", a->Lpad, L);
+  if (a->dvp < dh) return fail(EZB_ERR_SHAPE, "ezb_test_heads: V^T rows %d < dh %d", a->dvp, dh);
+  if (variant < HEADS_PACKED3 || variant > HEADS_SINGLE) return fail(EZB_ERR_ARG, "ezb_test_heads: variant %d", variant);
+  const bool packed = variant <= HEADS_PACKED3_KSUB2;
+  if (packed && nsec != 3) return fail(EZB_ERR_SHAPE, "ezb_test_heads: the packed-3 layout needs q, k and v sections");
+  for (int s = 0; s < nsec; ++s) {
+    const int kd = a->kinds[s];
+    if (kd < 0 || kd > 2) return fail(EZB_ERR_ARG, "ezb_test_heads: section %d kind %d", s, kd);
+    if ((kd == 0 && (!a->q || !a->norm_q)) || (kd == 1 && (!a->k || !a->norm_k)) || (kd == 2 && !a->vt))
+      return fail(EZB_ERR_ARG, "ezb_test_heads: section %d (kind %d) without its output or LayerNorm parameters", s, kd);
+  }
+  if (a->rope < 0 || a->rope > 2 || (a->rope && !a->inv_freq)) return fail(EZB_ERR_ARG, "ezb_test_heads: rope mode %d", a->rope);
+  const int M = B * L, N = nsec * D, bn3 = dh == 72 ? 224 : 192;
+  if (a->fold_st && (!a->fold_u || !a->fold_v || a->fold_slots < 1 || a->fold_ld_st < M))
+    return fail(EZB_ERR_ARG, "ezb_test_heads: fold needs u, v and %d-row partials", M);
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  dev.tmaps.trim();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  EpiHeadsParams e;
+  memset(&e, 0, sizeof e);
+  // by-value parameters (the model copies them to the host once, at finalize)
+  EZB_CUDA(cudaStreamSynchronize(st));
+  if (a->norm_q) { EZB_CUDA(cudaMemcpy(e.nw[0], a->norm_q, dh * sizeof(float), cudaMemcpyDeviceToHost)); EZB_CUDA(cudaMemcpy(e.nb[0], a->norm_q + dh, dh * sizeof(float), cudaMemcpyDeviceToHost)); }
+  if (a->norm_k) { EZB_CUDA(cudaMemcpy(e.nw[1], a->norm_k, dh * sizeof(float), cudaMemcpyDeviceToHost)); EZB_CUDA(cudaMemcpy(e.nb[1], a->norm_k + dh, dh * sizeof(float), cudaMemcpyDeviceToHost)); }
+  if (a->rope) EZB_CUDA(cudaMemcpy(e.inv_freq, a->inv_freq, (dh / 2) * sizeof(float), cudaMemcpyDeviceToHost));
+  e.D = D; e.H = H; e.L = L;
+  for (int s = 0; s < 3; ++s) e.kind[s] = s < nsec ? a->kinds[s] : 0;
+  e.rope_kinds = 3; e.rope_ld = L; e.rope_mufu = a->rope == 2;
+  e.out[0] = reinterpret_cast<__nv_bfloat16*>(a->q); e.out[1] = reinterpret_cast<__nv_bfloat16*>(a->k); e.out[2] = reinterpret_cast<__nv_bfloat16*>(a->vt);
+  e.ld_qk = a->ld_qk; e.dvp = a->dvp; e.Lpad = a->Lpad;
+  if (a->fold_st) {
+    e.fin.st0 = reinterpret_cast<const float2*>(a->fold_st); e.fin.slots0 = a->fold_slots; e.fin.ld_st = a->fold_ld_st;
+    e.fin.inv_dim = 1.0f / (float)D; e.fin.u = a->fold_u; e.fin.v = a->fold_v;
+  }
+  // the weight packed as Dit::init packs it (packed-3: zero-filled pad rows), the RoPE table as Dit::finalize fills it
+  const int rows = packed ? H * bn3 : N;
+  __nv_bfloat16* Wp = nullptr;
+  float2* cs = nullptr;
+  EZB_CUDA(cudaMallocAsync(&Wp, (size_t)rows * D * sizeof(__nv_bfloat16), st));
+  EZB_CUDA(cudaMemsetAsync(Wp, 0, (size_t)rows * D * sizeof(__nv_bfloat16), st));
+  const unsigned grid_w = (unsigned)(((size_t)D * D + 255) / 256);
+  if (packed) {
+    for (int s = 0; s < 3; ++s) pack_weight_kernel<<<grid_w, 256, 0, st>>>(W + (size_t)s * D * D, D, D, Wp, D, 1, 0, 0, 0, dh, s * H, bn3);
+  } else {
+    pack_weight_kernel<<<grid_w * nsec, 256, 0, st>>>(W, N, D, Wp, D, 1, 0, 0, 0, 0, 0, 0);
+  }
+  EZB_CUDA(cudaGetLastError());
+  if (a->rope) {
+    EZB_CUDA(cudaMallocAsync(&cs, (size_t)L * (dh / 2) * sizeof(float2), st));
+    rope_table_kernel<<<(L * (dh / 2) + 255) / 256, 256, 0, st>>>(a->inv_freq, cs, L, dh / 2);
+    EZB_CUDA(cudaGetLastError());
+    e.rope = cs;
+  }
+  const int rc = heads_gemm(dev, st, reinterpret_cast<const __nv_bfloat16*>(A), Wp, M, N, dh, variant, e);
+  EZB_CUDA(cudaFreeAsync(Wp, st));
+  if (cs) EZB_CUDA(cudaFreeAsync(cs, st));
+  return rc;
+}
+
+__attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* A, const float* W1, const float* b1, const void* W2, const float* b2, float* x,
+                                                        const float* gate, int gate_bstride, int rows_per_batch, void* mid, void* bar, int M, int D, int inner,
+                                                        int variant, void* stream) {
+  if (!A || !W1 || !b1 || !W2 || !b2 || !x || !mid || !bar) return fail(EZB_ERR_ARG, "ezb_test_mlp: null pointer");
+  if (M < 1 || D < 64 || D % 8 || inner < 128 || inner % 128) return fail(EZB_ERR_SHAPE, "ezb_test_mlp: M %d D %d inner %d", M, D, inner);
+  // the swap-AB epilogue looks up the gates of at most two clips per 32-token chunk (the model takes this path for clips of >= 32 tokens)
+  if (gate && rows_per_batch < 32) return fail(EZB_ERR_SHAPE, "ezb_test_mlp: %d rows per clip (>= 32)", rows_per_batch);
+  if (variant < 0 || variant > 2) return fail(EZB_ERR_ARG, "ezb_test_mlp: variant %d", variant);
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  dev.tmaps.trim();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  constexpr int half = 128;   // GEGLU packing group of the 256-wide N-tiles
+  __nv_bfloat16* W1p = nullptr;
+  float* b1p = nullptr;
+  EZB_CUDA(cudaMallocAsync(&W1p, (size_t)2 * inner * D * sizeof(__nv_bfloat16), st));
+  EZB_CUDA(cudaMallocAsync(&b1p, (size_t)2 * inner * sizeof(float), st));
+  pack_weight_kernel<<<(unsigned)(((size_t)2 * inner * D + 255) / 256), 256, 0, st>>>(W1, 2 * inner, D, W1p, D, 1, 0, inner, half, 0, 0, 0);
+  pack_geglu_bias_kernel<<<(2 * inner + 255) / 256, 256, 0, st>>>(b1, b1p, inner, half);
+  EZB_CUDA(cudaGetLastError());
+  EpiGegluParams g;
+  memset(&g, 0, sizeof g);
+  g.bias = b1p; g.out_bf16 = reinterpret_cast<__nv_bfloat16*>(mid); g.ld16 = inner;
+  EpiLinearParams p;
+  memset(&p, 0, sizeof p);
+  p.bias = b2; p.resid = x; p.ldr = D; p.gate = gate; p.gate_bstride = gate_bstride; p.rows_per_batch = rows_per_batch > 0 ? rows_per_batch : 1;
+  p.out_f32 = x; p.ld32 = D;
+  const __nv_bfloat16* a16 = reinterpret_cast<const __nv_bfloat16*>(A);
+  const __nv_bfloat16* w2 = reinterpret_cast<const __nv_bfloat16*>(W2);
+  const __nv_bfloat16* m16 = reinterpret_cast<const __nv_bfloat16*>(mid);
+  int rc;
+  if (variant == 0) {
+    rc = mlp_fused<EpiGeglu<256>, EpiLinearT<256>>(dev, st, a16, W1p, M, 2 * inner, D, g, m16, w2, D, inner, p, reinterpret_cast<GridBarrier*>(bar));
+  } else {
+    rc = variant == 2 ? gemm2<256, EpiGeglu<256>, 2>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g) : gemm2<256, EpiGeglu<256>>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g);
+    if (rc == EZB_OK) rc = gemm_swapped<EpiLinearT<256>>(dev, st, m16, inner, w2, inner, M, D, inner, p);
+  }
+  EZB_CUDA(cudaFreeAsync(W1p, st));
+  EZB_CUDA(cudaFreeAsync(b1p, st));
+  return rc;
 }
 
 

@@ -541,4 +541,52 @@ int gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __
   return launch_gemm_t<BN, Epi>(dev, st, tA, tB, g, ep);
 }
 
+// Kernel instantiations of the fused heads epilogue (gemm.cuh EpiHeads).  Dit::lin_heads picks one from the options and the ezb_test_heads
+// hook from its argument, and both launch through heads_gemm, so the kernel-level tests run exactly what the model dispatches.
+enum HeadsVariant {
+  HEADS_PACKED3 = 0,         // three heads per N-tile (W packed by pack_weight_kernel's h3 mode), shared-memory staged q / k stores
+  HEADS_PACKED3_DIRECT = 1,  // the same without staging (every thread stores its own q / k row)
+  HEADS_PACKED3_KSUB2 = 2,   // DIRECT with 128-deep ring slots (dh = 72, no fold)
+  HEADS_PAIR = 3,            // two heads per N-tile of the reference column order, 2-CTA clusters, staged stores
+  HEADS_PAIR_DIRECT = 4,
+  HEADS_SINGLE = 5,          // two heads per N-tile on the single-CTA kernel, staged stores (no fold)
+};
+// A [M, D] bf16; W packed for the variant (packed-3: H * BN rows; otherwise N = sections * D rows).  The LayerNorm fold is on when e.fin.u
+// is set; e.dbg selects the profiling instantiation (packed-3, dh = 72, no fold).
+inline int heads_gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, const __nv_bfloat16* W, int M, int N, int dh, int variant,
+                      const EpiHeadsParams& e) {
+  const int D = e.D, H = e.H;
+  const bool fo = e.fin.u != nullptr;
+  const bool packed = variant == HEADS_PACKED3 || variant == HEADS_PACKED3_DIRECT || variant == HEADS_PACKED3_KSUB2;
+  const bool direct = variant == HEADS_PACKED3_DIRECT || variant == HEADS_PAIR_DIRECT;
+  if (dh != 72 && dh != 64) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: head dimension %d", dh);
+  if (packed && N != 3 * D) return fail(EZB_ERR_SHAPE, "heads_gemm: the packed-3 layout holds q, k and v (N %d, D %d)", N, D);
+#define EZB_HEADS(BN_, DH_, HPT_, N_)                                                                                                          \
+  (fo ? (direct ? gemm2<BN_, EpiHeads<DH_, HPT_, true, true>>(dev, st, A, D, W, D, M, N_, D, e) : gemm2<BN_, EpiHeads<DH_, HPT_, false, true>>(dev, st, A, D, W, D, M, N_, D, e)) \
+      : (direct ? gemm2<BN_, EpiHeads<DH_, HPT_, true, false>>(dev, st, A, D, W, D, M, N_, D, e) : gemm2<BN_, EpiHeads<DH_, HPT_, false, false>>(dev, st, A, D, W, D, M, N_, D, e)))
+  if (e.dbg) {   // profiling instantiation: parts of the epilogue removed
+    if (variant != HEADS_PACKED3 || dh != 72 || fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: the profiling epilogue is packed-3, dh 72, unfolded");
+    return gemm2<224, EpiHeads<72, 3, false, false, true>>(dev, st, A, D, W, D, M, H * 224, D, e);
+  }
+  switch (variant) {
+    case HEADS_PACKED3_KSUB2:   // 128-deep slots (needs the staging-free epilogue)
+      if (dh != 72 || fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: 128-deep slots exist for dh 72 without fold only");
+      return gemm2<224, EpiHeads<72, 3, true, false>, 2>(dev, st, A, D, W, D, M, H * 224, D, e);
+    case HEADS_PACKED3:
+    case HEADS_PACKED3_DIRECT:
+      if (dh == 72) return EZB_HEADS(224, 72, 3, H * 224);
+      return EZB_HEADS(192, 64, 3, H * 192);
+    case HEADS_PAIR:
+    case HEADS_PAIR_DIRECT:
+      if (dh == 72) return EZB_HEADS(144, 72, 2, N);
+      return EZB_HEADS(128, 64, 2, N);
+    case HEADS_SINGLE:
+      if (fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: the single-CTA heads kernel has no fold");
+      if (dh == 72) return gemm<144, EpiHeads<72>>(dev, st, A, D, W, D, M, N, D, e);
+      return gemm<128, EpiHeads<64>>(dev, st, A, D, W, D, M, N, D, e);
+  }
+#undef EZB_HEADS
+  return fail(EZB_ERR_ARG, "heads_gemm: variant %d", variant);
+}
+
 }  // namespace ezb

@@ -154,10 +154,41 @@ typedef struct {
   int32_t act; const float* act_a; const float* act_b;
 } ezb_test_epilogue;
 /* C = A[M,K] W[N,K]^T through the wgmma GEMM; epi_kind 0 = linear epilogue, 1 = GEGLU (packed W); 10 / 11 = the same on 2-CTA
-   clusters; 20 = swap-AB. conv_* = 0 for plain. */
+   clusters; 12 = the cluster GEGLU with 128-deep ring slots (two 64-wide k-blocks per slot); 20 = swap-AB. conv_* = 0 for plain. */
 int ezb_test_gemm(int device, const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K, int bn, int epi_kind,
                   const ezb_test_epilogue* e, int conv_taps, int conv_center, int conv_dil, int conv_cin_pad, int conv_T,
                   int conv_B, void* stream);
+/* Q/K/V-type projection with the fused per-head LayerNorm(dh) + RoPE + attention-layout epilogue (the fast mode's Q/K/V, cross-Q and
+   cross-K/V GEMMs).  Device pointers.  A [B*L, D] bf16; W [nsec*D, D] fp32 in the reference layout (section s = rows s*D ..), packed and
+   rounded to bf16 by the library as the model packs it.  Section s has kind kinds[s]: 0 q, 1 k (both LayerNorm(dh) -> optional RoPE at the
+   position within the clip -> bf16 rows [b*H + h, l, 0..dh) of pitch ld_qk), 2 v (bf16 V^T [b*H + h, 0..dvp, 0..Lpad): rows dh..dvp written
+   as zeros, columns L..Lpad not written). */
+typedef struct {
+  int32_t B, L, D, H, dh, nsec;
+  int32_t kinds[3];
+  const float* norm_q;        /* [2][dh] LayerNorm weight | bias of kind 0 (NULL when no section is kind 0) */
+  const float* norm_k;        /* the same for kind 1 */
+  const float* inv_freq;      /* [dh/2] RoPE frequencies */
+  int32_t rope;               /* 0 none, 1 (cos, sin) table filled by the library, 2 __sincosf from inv_freq */
+  void* q; void* k; void* vt;
+  int32_t ld_qk, dvp, Lpad;
+  /* LayerNorm folded in (NULL fold_st: off): float2 [fold_slots][fold_ld_st] per-row (sum x, sum x^2) partials of the D-wide x, and u, v
+     in the packed output-column order (packed-3: H * N-tile entries, 0 in the pad columns) */
+  const void* fold_st; int32_t fold_slots, fold_ld_st;
+  const float* fold_u; const float* fold_v;
+  /* 0 / 1 / 2: three heads per N-tile with staged / direct q, k stores / direct with 128-deep ring slots (nsec 3);
+     3 / 4: two heads per N-tile on 2-CTA clusters, staged / direct; 5: two heads per N-tile on the single-CTA kernel */
+  int32_t variant;
+} ezb_test_heads_args;
+int ezb_test_heads(int device, const void* A_bf16, const float* W_f32, const ezb_test_heads_args* args, void* stream);
+/* MLP of a DiT block: x += (1 - gate[b]) * (bf16(GEGLU(A W1^T + b1)) W2^T + b2), b = row / rows_per_batch (gate NULL: plain residual).
+   Device pointers.  A [M, D] bf16; W1 [2*inner, D] and b1 [2*inner] fp32 in the reference layout ([hidden; gate] rows), packed by the
+   library; W2 [D, inner] bf16; b2 [D]; x [M, D] fp32 updated in place; gate row stride gate_bstride; mid [M, inner] bf16 receives the GEGLU
+   output; grid_barrier: two zeroed uint32 (count, generation), left with count 0.  variant 0: one persistent launch (GEGLU, grid barrier,
+   swap-AB output projection); 1: the same two GEMMs as two launches; 2: as 1 with 128-deep ring slots in the GEGLU GEMM. */
+int ezb_test_mlp(int device, const void* A_bf16, const float* W1_f32, const float* b1_f32, const void* W2_bf16, const float* b2, float* x,
+                 const float* gate, int gate_bstride, int rows_per_batch, void* mid_bf16, void* grid_barrier, int M, int D, int inner,
+                 int variant, void* stream);
 /* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7: that
    generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,

@@ -146,6 +146,82 @@ def test_pair_gemm_geglu():
     assert (out.float() - ref).abs().max().item() < 2e-2 * max(1.0, ref.abs().max().item() / 4)
 
 
+def _geglu_ref(A, W, bias, inner):
+    """fp64 h * gelu_erf(g), [h; g] = A W^T + bias in the reference row order."""
+    u = A.double() @ W.double().t() + bias.double()
+    return u[:, :inner] * torch.nn.functional.gelu(u[:, inner:])
+
+
+@pytest.mark.parametrize("M,K", [(900, 64), (300, 1088), (1000, 1216), (257, 1152)])
+def test_pair_gemm_geglu_ksub2_matches_ksub1(M, K):
+    """128-deep ring slots (two 64-wide k-blocks per slot, option ksub2) in the MLP's GEGLU GEMM.  An odd number of k-blocks leaves the last
+    slot half full.  Same MMAs in the same k order as the 64-deep kernel: bit-identical output.  Against fp64: one bf16 rounding of the output
+    (2^-8 relative) plus 2e-4 for the fp32 accumulation and the fast erf (|err| <= 1.5e-7 + 2 MUFU ulp, on |h gelu(g)| <~ 30)."""
+    inner, bn = 1024, 256
+    g = torch.Generator(device="cuda").manual_seed(M + K)
+    A = torch.randn(M, K, device="cuda", generator=g).bfloat16()
+    W = (torch.randn(2 * inner, K, device="cuda", generator=g) / math.sqrt(K)).bfloat16()
+    bias = torch.randn(2 * inner, device="cuda", generator=g) * 0.1
+    half = bn // 2
+    Wp = torch.stack([W[:inner].view(inner // half, half, K), W[inner:].view(inner // half, half, K)], 1).reshape(2 * inner, K).contiguous()
+    bp = torch.stack([bias[:inner].view(-1, half), bias[inner:].view(-1, half)], 1).reshape(-1).contiguous()
+    outs = {}
+    for kind in (11, 12):
+        outs[kind] = torch.full((M, inner), float("nan"), device="cuda", dtype=torch.bfloat16)
+        _run(A, Wp, _epi(bias=bp, out_bf16=outs[kind], ld16=inner), M, 2 * inner, K, bn, kind=kind)
+    assert torch.equal(outs[11].view(torch.int16), outs[12].view(torch.int16))
+    ref = _geglu_ref(A, W, bias, inner)
+    err = (outs[12].double() - ref).abs()
+    assert bool((err <= 2.0 ** -8 * ref.abs() + 2e-4).all()), float(err.max())
+
+
+@pytest.mark.parametrize("M,L,D,inner", [(64, 32, 1152, 4608), (300, 100, 1152, 512), (1000, 40, 1152, 4608), (4000, 500, 1152, 4608),
+                                         (1000, 250, 384, 512)])
+def test_mlp_fused_matches_two_launch_and_fp64(M, L, D, inner):
+    """The persistent MLP kernel (GEGLU GEMM on 2-CTA clusters, grid barrier, swap-AB output projection with the gated residual) against
+    the same two GEMMs as two launches (the same tiles and k order: bit-identical), the two-launch path with 128-deep GEGLU slots (also
+    bit-identical) and fp64.  Clips of L rows do not align to the 128-row / 256-token tiles.  The reference takes the kernel's own bf16
+    `mid` (checked separately to one bf16 rounding) so that the second GEMM is held to the swap-AB bound 3e-3 sqrt(K / 1024)."""
+    from ezaudio_b200 import _lib
+    lib = _lib.lib()
+    g = torch.Generator(device="cuda").manual_seed(M + L + D + inner)
+    A = torch.randn(M, D, device="cuda", generator=g).bfloat16()
+    W1 = torch.randn(2 * inner, D, device="cuda", generator=g) / math.sqrt(D)      # reference layout [hidden; gate], packed by the hook
+    b1 = torch.randn(2 * inner, device="cuda", generator=g) * 0.1
+    W2 = (torch.randn(D, inner, device="cuda", generator=g) / math.sqrt(inner)).bfloat16()
+    b2 = torch.randn(D, device="cuda", generator=g)
+    x = torch.randn(M, D, device="cuda", generator=g)
+    nb = (M + L - 1) // L
+    gate = torch.randn(nb, 6 * D, device="cuda", generator=g) * 0.3
+    bar = torch.zeros(2, dtype=torch.int32, device="cuda")
+
+    def run(variant):
+        xo = x.clone()
+        mid = torch.full((M, inner), float("nan"), device="cuda", dtype=torch.bfloat16)
+        _lib.check(lib.ezb_test_mlp(0, _lib.ptr(A), _lib.ptr(W1), _lib.ptr(b1), _lib.ptr(W2), _lib.ptr(b2), _lib.ptr(xo), _lib.ptr(gate[:, 5 * D:]),
+                                    6 * D, L, _lib.ptr(mid), _lib.ptr(bar), M, D, inner, variant, _lib.stream_ptr()))
+        torch.cuda.synchronize()
+        return xo, mid
+
+    x2, mid2 = run(1)
+    xk, midk = run(2)
+    assert torch.equal(midk.view(torch.int16), mid2.view(torch.int16)) and torch.equal(xk, x2)
+    for i in range(3):   # the barrier resets itself: count back to 0, one generation per launch
+        gen = int(bar[1])
+        xf, midf = run(0)
+        assert int(bar[0]) == 0 and int(bar[1]) == gen + 1, (i, bar.tolist())
+        assert torch.equal(midf.view(torch.int16), mid2.view(torch.int16)), i
+        assert torch.equal(xf, x2), i
+    mid_ref = _geglu_ref(A, W1.bfloat16(), b1, inner)
+    err = (mid2.double() - mid_ref).abs()
+    assert bool((err <= 2.0 ** -8 * mid_ref.abs() + 2e-4).all()), float(err.max())
+    keep = 1 - gate[:, 5 * D:].double().repeat_interleave(L, 0)[:M]
+    ref = x.double() + keep * (mid2.double() @ W2.double().t() + b2.double())
+    err = float((x2.double() - ref).abs().max())
+    print(f"[mlp] M {M} L {L} D {D} inner {inner}: mid max-abs err {float((mid2.double() - mid_ref).abs().max()):.3e}, x max-abs err {err:.3e}")
+    assert err < 3e-3 * max(1.0, math.sqrt(inner / 1024)), err
+
+
 @pytest.mark.parametrize("M,N,K,L", [(4000, 1152, 1152, 500), (1000, 1152, 4608, 250), (300, 144, 144, 100), (777, 1024, 264, 259), (4000, 1152, 2304, 500)])
 def test_swap_ab_gemm_gated_residual(M, N, K, L):
     """Swap-AB kernel (features on accumulator rows): bias + gated residual in place, and plain bias -> f32."""
