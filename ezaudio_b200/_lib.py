@@ -35,7 +35,10 @@ class TestEpilogue(C.Structure):
     _fields_ = [("bias", C.c_void_p), ("bias_mod", C.c_int32), ("resid", C.c_void_p), ("ldr", C.c_int32),
                 ("gate", C.c_void_p), ("gate_bstride", C.c_int32), ("rows_per_batch", C.c_int32),
                 ("out_f32", C.c_void_p), ("ld32", C.c_int32), ("out_bf16", C.c_void_p), ("ld16", C.c_int32),
-                ("split_stride", C.c_int32), ("act", C.c_int32), ("act_a", C.c_void_p), ("act_b", C.c_void_p)]
+                ("split_stride", C.c_int32), ("act", C.c_int32), ("act_a", C.c_void_p), ("act_b", C.c_void_p),
+                ("fin_st", C.c_void_p), ("fin_slots", C.c_int32), ("fin_ld_st", C.c_int32), ("fin_inv_dim", C.c_float), ("fin_u", C.c_void_p),
+                ("fin_v", C.c_void_p), ("fout_st", C.c_void_p), ("fout_ld_st", C.c_int32), ("fout_a0", C.c_void_p), ("fout_ld0", C.c_int32),
+                ("fout_g0", C.c_void_p), ("fout_a1", C.c_void_p), ("fout_ld1", C.c_int32), ("fout_g1", C.c_void_p)]
 
 
 class TestHeadsArgs(C.Structure):

@@ -530,16 +530,16 @@ struct Dit {
   // kernel (gemm_ln.cuh) and *tail_done is set, otherwise the caller launches it separately.
   int lin(cudaStream_t st, const bf16* A, int K, const bf16* W, int M, int N, const EpiLinearParams& e, const LnParams* tail = nullptr, bool* tail_done = nullptr) {
     if ((opt_skip() & 8) && e.out_f32 != nullptr && e.out_bf16 == nullptr) return EZB_OK;
-    // fp32-output layers (residual / gated-residual / plain): swap-AB 128 x 256 tiles -- one full wave for N = 1152 at M = 4000
+    // fp32-output layers (residual / gated-residual / plain): swap-AB tiles of 128 features x 256 or 288 tokens (host.cuh swapped_bn)
     const bool folded = e.fin.u != nullptr || e.fout.st != nullptr;   // fold epilogues exist in the swap-AB kernel only
     const bool short_clips = e.gate != nullptr && e.rows_per_batch < 32;  // per-token gate lookup lives in the generic (non swap-AB) epilogue
     if (pair && swap_ab && kmul == 1 && e.out_bf16 == nullptr && e.out_f32 != nullptr && e.out_scale == 0.f && e.bias_mod == 0 && !short_clips &&
         (M >= 512 || folded)) {
-      if (folded) return gemm_swapped<EpiLinearTF<256>>(*dev, st, A, K, W, K, M, N, K, e);
+      if (folded) return gemm_swapped<EpiLinearTF>(*dev, st, A, K, W, K, M, N, K, e);
       if (tail != nullptr && tail_done != nullptr && opt_ln_tail() && !(opt_skip() & 9))
-        return gemm_swapped_ln<EpiLinearT<256>>(*dev, st, A, K, W, K, M, N, K, e, *tail, grid_bar, tail_done);
-      return opt_swap_mc() ? gemm_swapped_mc<EpiLinearT<256>, 3>(*dev, st, A, K, W, K, M, N, K, e)
-                           : gemm_swapped<EpiLinearT<256>>(*dev, st, A, K, W, K, M, N, K, e);
+        return gemm_swapped_ln<EpiLinearT>(*dev, st, A, K, W, K, M, N, K, e, *tail, grid_bar, tail_done);
+      return opt_swap_mc() ? gemm_swapped_mc<EpiLinearT, 3>(*dev, st, A, K, W, K, M, N, K, e)
+                           : gemm_swapped<EpiLinearT>(*dev, st, A, K, W, K, M, N, K, e);
     }
     if (folded) return fail(EZB_ERR_STATE, "folded LayerNorm epilogue requested on a GEMM that is not a swap-AB launch");
     if (pair) return gemm2<128, EpiLinear<128>>(*dev, st, A, kmul * K, W, kmul * K, M, N, kmul * K, e);

@@ -28,6 +28,15 @@ EpiLinearParams to_epi(const ezb_test_epilogue* e) {
   p.gate_bstride = e->gate_bstride; p.rows_per_batch = e->rows_per_batch; p.out_f32 = e->out_f32; p.ld32 = e->ld32;
   p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(e->out_bf16); p.ld16 = e->ld16; p.split_stride = e->split_stride;
   p.act = e->act; p.act_a = e->act_a; p.act_b = e->act_b; p.out_scale = 0.f; p.phase_cols = 0; p.phase_ld16 = 0;
+  if (e->fin_u) {
+    p.fin.st0 = static_cast<const float2*>(e->fin_st); p.fin.slots0 = e->fin_slots; p.fin.ld_st = e->fin_ld_st; p.fin.inv_dim = e->fin_inv_dim;
+    p.fin.u = e->fin_u; p.fin.v = e->fin_v;
+  }
+  if (e->fout_st) {
+    p.fout.st = static_cast<float2*>(e->fout_st); p.fout.ld_st = e->fout_ld_st;
+    p.fout.a0 = static_cast<__nv_bfloat16*>(e->fout_a0); p.fout.ld0 = e->fout_ld0; p.fout.g0 = e->fout_g0;
+    p.fout.a1 = static_cast<__nv_bfloat16*>(e->fout_a1); p.fout.ld1 = e->fout_ld1; p.fout.g1 = e->fout_g1;
+  }
   return p;
 }
 }  // namespace
@@ -49,11 +58,22 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
   ConvAddr conv;
   conv.taps = conv_taps; conv.center = conv_center; conv.dilation = conv_dil; conv.cin_pad = conv_cin_pad; conv.T = conv_T; conv.B = conv_B;
   const ConvAddr* cp = conv_taps > 0 ? &conv : nullptr;
-  if (epi_kind == 20) {  // swap-AB: 128 features x 256 tokens tiles, fp32 output
+  if (epi_kind == 20 || epi_kind == 21) {  // swap-AB: tiles of 128 features x 256 / 288 tokens, fp32 output
     if (cp) return fail(EZB_ERR_UNSUPPORTED, "swap-AB GEMM has no conv addressing");
     EpiLinearParams p = to_epi(e);
-    if (opt_swap_mc()) return gemm_swapped_mc<EpiLinearT<256>, 3>(dev, st, a, lda, w, ldw, M, N, K, p);
-    return gemm_swapped<EpiLinearT<256>>(dev, st, a, lda, w, ldw, M, N, K, p);
+    if ((p.fin.u && (!p.fin.st0 || !p.fin.v)) || (p.fout.st && !p.fout.a0))
+      return fail(EZB_ERR_ARG, "ezb_test_gemm: fold-in needs its partials and v, fold-out its first operand");
+    const bool fold = p.fin.u || p.fout.st;
+    if (epi_kind == 20) {   // what Dit::lin dispatches
+      if (fold) return gemm_swapped<EpiLinearTF>(dev, st, a, lda, w, ldw, M, N, K, p);
+      if (opt_swap_mc()) return gemm_swapped_mc<EpiLinearT, 3>(dev, st, a, lda, w, ldw, M, N, K, p);
+      return gemm_swapped<EpiLinearT>(dev, st, a, lda, w, ldw, M, N, K, p);
+    }
+    if (bn == 256) return fold ? gemm_swapped_at<256, EpiLinearTF<256>>(dev, st, a, lda, w, ldw, M, N, K, p)
+                               : gemm_swapped_at<256, EpiLinearT<256>>(dev, st, a, lda, w, ldw, M, N, K, p);
+    if (bn == 288) return fold ? gemm_swapped_at<288, EpiLinearTF<288>>(dev, st, a, lda, w, ldw, M, N, K, p)
+                               : gemm_swapped_at<288, EpiLinearT<288>>(dev, st, a, lda, w, ldw, M, N, K, p);
+    return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm swap-AB: bn=%d (256 or 288)", bn);
   }
   if (epi_kind == 10 || epi_kind == 11) {  // 2-CTA cluster kernel with the W tile multicast (bn is the tile's N)
     if (cp) return fail(EZB_ERR_UNSUPPORTED, "cluster GEMM has no conv addressing");
@@ -195,7 +215,7 @@ __attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* 
     rc = mlp_fused<EpiGeglu<256>, EpiLinearT<256>>(dev, st, a16, W1p, M, 2 * inner, D, g, m16, w2, D, inner, p, reinterpret_cast<GridBarrier*>(bar));
   } else {
     rc = variant == 2 ? gemm2<256, EpiGeglu<256>, 2>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g) : gemm2<256, EpiGeglu<256>>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g);
-    if (rc == EZB_OK) rc = gemm_swapped<EpiLinearT<256>>(dev, st, m16, inner, w2, inner, M, D, inner, p);
+    if (rc == EZB_OK) rc = gemm_swapped<EpiLinearT>(dev, st, m16, inner, w2, inner, M, D, inner, p);
   }
   EZB_CUDA(cudaFreeAsync(W1p, st));
   EZB_CUDA(cudaFreeAsync(b1p, st));

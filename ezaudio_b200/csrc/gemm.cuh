@@ -27,6 +27,9 @@ constexpr int GEMM_BK = 64;
 #define EZB_DBG(...)
 #endif
 constexpr int GEMM_SMEM_BUDGET = 227 * 1024 - 2048;  // dynamic smem per CTA minus alignment slack and barriers
+// Rows of one TMA box of the BN-row operand tile: boxes and wgmma N stop at 256, so a wider tile (the 288-token swap-AB tile) is loaded
+// as two boxes and multiplied as two halves.
+constexpr int gemm_b_box(int bn) { return bn > 256 ? bn / 2 : bn; }
 
 struct GemmShape {
   int M, N;
@@ -437,16 +440,22 @@ struct EpiGeglu {
 // ---------------------------------------------------------------------------------------------------------------
 // Transposed ("swap-AB") linear epilogue.  For N_out = 1152-wide layers the natural 128/144-column tiles spend more operand
 // bytes per flop and a 256-column tile does not divide 1152.  Computing C^T = W A^T instead puts the 1152 output features on the
-// accumulator ROWS (9 tiles of 128) and 256 tokens on the columns (the widest wgmma tile).  A thread now owns one output feature; for a given token the 32 lanes of a warp hold
-// 32 consecutive features, so residual loads and stores are 128-byte coalesced without any staging.
+// accumulator ROWS (9 tiles of 128) and 256 or 288 tokens on the columns (host.cuh swapped_bn picks the width).  A thread now owns one output
+// feature; for a given token the 32 lanes of a warp hold 32 consecutive features, so residual loads and stores are 128-byte coalesced without
+// any staging.  Each of the two warps of a 32-feature group owns BN / 2 tokens, walked in chunks of up to 32: at BN = 288 that is 4.5 chunks,
+// and the half chunk stops at the warp's range so that no warp writes another warp's tokens.
+__device__ __forceinline__ int swap_chunk_tokens(int c, int c_end, int t0, int N) {   // tokens of the chunk at tile column c (first token t0)
+  int n = c_end - c;
+  if (N - t0 < n) n = N - t0;
+  return n < 32 ? n : 32;
+}
 template <int BN>
 struct EpiLinearT {
   using Params = EpiLinearParams;   // bias/gate indexed by feature, resid/out_f32 [token, feature]; bf16/act/split unsupported
   static constexpr int EPI_WARPS = 8;
   static constexpr int STAGE_FLOATS = 0;
-  // residual values of one 32-token chunk (feature f of tokens t0 .. t0+31)
-  static __device__ __forceinline__ void load_resid(const Params& ep, float (&x)[32], int t0, int N, int f, bool f_ok) {
-    const int nt = (N - t0) < 32 ? (N - t0) : 32;
+  // residual values of one chunk of nt <= 32 tokens (feature f of tokens t0 .. t0+nt-1)
+  static __device__ __forceinline__ void load_resid(const Params& ep, float (&x)[32], int t0, int nt, int f, bool f_ok) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) x[j] = (f_ok && j < nt) ? ep.resid[(size_t)(t0 + j) * ep.ldr + f] : 0.f;
   }
@@ -457,18 +466,18 @@ struct EpiLinearT {
     const bool f_ok = lane < nvalid;
     const float bias = (ep.bias != nullptr && f_ok) ? ep.bias[f] : 0.f;
     bool waited = false;
-    // The kernel is one wave, so this epilogue is exposed: the residual of chunk c + 1 is fetched while chunk c is processed (and the first
-    // chunk's before the accumulator wait), instead of one L2 round trip per chunk on the critical path.
+    // The epilogue does not overlap the next tile's mainloop, so it is exposed: the residual of chunk c + 1 is fetched while chunk c is
+    // processed (and the first chunk's before the accumulator wait), instead of one L2 round trip per chunk on the critical path.
     float x[32];
-    if (ep.resid != nullptr && n0 + c_begin < N) load_resid(ep, x, n0 + c_begin, N, f, f_ok);
+    if (ep.resid != nullptr && n0 + c_begin < N) load_resid(ep, x, n0 + c_begin, swap_chunk_tokens(c_begin, c_end, n0 + c_begin, N), f, f_ok);
 #pragma unroll 1
     for (int c = c_begin; c < c_end; c += 32) {
       const int t0 = n0 + c;                   // first token of this chunk
       if (t0 >= N) break;                      // warp-uniform
-      const int nt = (N - t0) < 32 ? (N - t0) : 32;
+      const int nt = swap_chunk_tokens(c, c_end, t0, N);
       float xn[32];
       const bool more = ep.resid != nullptr && c + 32 < c_end && t0 + 32 < N;
-      if (more) load_resid(ep, xn, t0 + 32, N, f, f_ok);
+      if (more) load_resid(ep, xn, t0 + 32, swap_chunk_tokens(c + 32, c_end, t0 + 32, N), f, f_ok);
       float g0 = 1.f, g1 = 1.f;
       int btok = 0x7fffffff;                   // first token that belongs to the second batch item of this chunk
       if (ep.gate != nullptr && f_ok) {
@@ -525,7 +534,7 @@ struct EpiLinearTF {
     for (int c = c_begin; c < c_end; c += 32) {
       const int t0 = n0 + c;                   // first token of this chunk
       if (t0 >= N) break;                      // warp-uniform
-      const int nt = (N - t0) < 32 ? (N - t0) : 32;
+      const int nt = swap_chunk_tokens(c, c_end, t0, N);
       float x[32];
       if (ep.resid != nullptr) {
 #pragma unroll
@@ -612,7 +621,17 @@ struct GemmCfg {
   static constexpr int NSUB = MMA_WG == 2 ? 1 : 2;                // 64-row halves per warpgroup
   static constexpr int WN0 = MMA_WG == 3 ? (BN == 224 ? 72 : BN / 3) : BN;   // columns of warpgroups 0 .. MMA_WG - 2
   static constexpr int WNL = MMA_WG == 3 ? BN - 2 * WN0 : BN;                 // columns of the last one
-  static constexpr int THREADS = 32 * EPI_WARPS + 32;             // consumer warpgroups + the producer warp
+  // Consumer warpgroups + the producer warp.  A CTA of 9..12 warps puts three warps on one SM sub-partition, which caps every thread at 168
+  // registers: too few for the 144 accumulators of a 288-wide tile (ptxas spills and serialises the wgmma).  BN > 256 therefore runs a whole
+  // producer warpgroup (one active warp) that hands registers to the consumers with setmaxnreg: 384 x 168 = 128 x 40 + 256 x 232.
+  static constexpr bool PRODUCER_WG = BN > 256;
+  static constexpr int THREADS = 32 * EPI_WARPS + (PRODUCER_WG ? 128 : 32);
+  static constexpr int REGS_LAUNCH = (65536 / THREADS) & ~7;                        // what __launch_bounds__(THREADS, 1) lets ptxas allocate
+  static constexpr int REGS_PRODUCER = 40;
+  static constexpr int REGS_CONSUMER = ((THREADS * REGS_LAUNCH - 128 * REGS_PRODUCER) / (32 * EPI_WARPS)) & ~7;
+  // setmaxnreg.inc waits for free registers: the split must not ask for more than the launch allocated
+  static_assert(!PRODUCER_WG || (EPI_WARPS == 8 && 128 * REGS_PRODUCER + 32 * EPI_WARPS * REGS_CONSUMER <= THREADS * REGS_LAUNCH &&
+                                 REGS_CONSUMER >= 224), "register split");
   static constexpr int ACC_PITCH = BN + 4;
   static constexpr int ACC_BYTES = GEMM_BM * ACC_PITCH * 4;
   static constexpr int STAGE_BYTES = EPI_WARPS * Epi::STAGE_FLOATS * 4;   // one transpose tile per epilogue warp
@@ -638,7 +657,10 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
       else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
     }
   };
-  float d[NSUB][WN / 2];
+  constexpr int NH = WN > 256 ? 2 : 1;   // wgmma N stops at 256: a wider share is issued as two halves, HN columns each
+  constexpr int HN = WN / NH;
+  static_assert(HN <= 256 && HN % 8 == 0, "WN");   // HN % 8: the second half starts on a 1024-byte swizzle atom
+  float d[NSUB][NH][HN / 2];
   uint32_t prev = 0;
   for (int kb = 0; kb < num_k_blocks; kb += KSUB) {
     mbar_wait(&full[stage], phase);
@@ -653,7 +675,9 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
       for (int k = 0; k < GEMM_BK / 16; ++k) {
 #pragma unroll
         for (int s = 0; s < NSUB; ++s)
-          Wgmma<WN>::mma(d[s], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0) + 2 * k, (kb | sub | k) != 0);
+#pragma unroll
+          for (int h = 0; h < NH; ++h)
+            Wgmma<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | sub | k) != 0);
       }
     }
     wgmma_commit();
@@ -664,16 +688,21 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
   wgmma_wait<0>();
   release(prev);
 #pragma unroll
-  for (int s = 0; s < NSUB; ++s) wgmma_fence_regs(d[s]);
+  for (int s = 0; s < NSUB; ++s)
+#pragma unroll
+    for (int h = 0; h < NH; ++h) wgmma_fence_regs(d[s][h]);
   named_bar_sync(1, 32 * SM::EPI_WARPS);   // every MMA of the tile has completed: the ring may now hold the accumulator
   // m64nN fragment: register 4i + {0,1} -> row 16 * (warp % 4) + lane / 4, columns 8i + 2 (lane % 4) + {0,1}; 4i + {2,3} -> row + 8
 #pragma unroll
   for (int s = 0; s < NSUB; ++s) {
-    float* r0 = sAcc + (size_t)((row64 + s) * 64 + 16 * lg + (lane >> 2)) * SM::ACC_PITCH + col0 + 2 * (lane & 3);
 #pragma unroll
-    for (int i = 0; i < WN / 8; ++i) {
-      *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(d[s][4 * i], d[s][4 * i + 1]);
-      *reinterpret_cast<float2*>(r0 + 8 * SM::ACC_PITCH + 8 * i) = make_float2(d[s][4 * i + 2], d[s][4 * i + 3]);
+    for (int h = 0; h < NH; ++h) {
+      float* r0 = sAcc + (size_t)((row64 + s) * 64 + 16 * lg + (lane >> 2)) * SM::ACC_PITCH + col0 + h * HN + 2 * (lane & 3);
+#pragma unroll
+      for (int i = 0; i < HN / 8; ++i) {
+        *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(d[s][h][4 * i], d[s][h][4 * i + 1]);
+        *reinterpret_cast<float2*>(r0 + 8 * SM::ACC_PITCH + 8 * i) = make_float2(d[s][h][4 * i + 2], d[s][h][4 * i + 3]);
+      }
     }
   }
 }
@@ -688,11 +717,17 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
 // phase may lay out its own in the same shared memory.
 template <int BN>
 struct McSub { static constexpr int ROWS = BN % 32 == 0 ? 32 : 16; };
+// Per-thread register budget of the executing warpgroup (all its threads execute it); inc waits until the pool has the registers.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, int KSUB = 1>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw) {
-  static_assert(BN % 16 == 0 && BN >= 64 && BN <= 256, "BN");
-  static_assert(MC >= 1 && MC <= 8 && BN % McSub<BN>::ROWS == 0, "MC");
   using SM = GemmCfg<BN, Epi, KSUB>;
+  // BN > 256: two TMA boxes and two wgmma halves per warpgroup, single CTA, one 64-row half per MMA warpgroup (the 288-token swap-AB tile)
+  static_assert(BN % 16 == 0 && BN >= 64 && (BN <= 256 || (BN <= 512 && BN % 32 == 0 && MC == 1 && SM::MMA_WG == 2)), "BN");
+  static_assert(MC >= 1 && MC <= 8 && BN % McSub<BN>::ROWS == 0, "MC");
   constexpr int STAGES = SM::STAGES, EPI_WARPS = SM::EPI_WARPS, NSUB = SM::NSUB;
   constexpr uint16_t MC_MASK = static_cast<uint16_t>((1u << MC) - 1u);
   // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array (a round trip through uintptr_t loses the
@@ -731,11 +766,13 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
   pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
   EZB_DBG(const bool dbg = g.dbg != nullptr && blockIdx.x == 0; const long long t_start = clock64(); long long w0 = 0, w1 = 0, w4 = 0;)
 
-  if (warp == PRODUCER) {
-    // ------------------------------------------------ TMA producer (warp-uniform loop, copies issued under elect.sync)
+  if (warp >= PRODUCER) {
+    // ------------------------------------------------ TMA producer (warp-uniform loop, copies issued under elect.sync); the other warps of a
+    // producer warpgroup (GemmCfg::PRODUCER_WG) only give their registers away
+    if constexpr (SM::PRODUCER_WG) setmaxnreg_dec<SM::REGS_PRODUCER>();
     uint32_t stage = 0, phase = 0, af_phase = 0;
     bool first = true;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    for (int tile = warp == PRODUCER ? (int)blockIdx.x : num_tiles; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
       const int n0 = nt * BN;
       if (!first) { mbar_wait(acc_free, af_phase); af_phase ^= 1; }   // the ring held the previous tile's accumulator
@@ -765,7 +802,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
             }
           }
           if (MC == 1) {
-            tma_load_2d(dB, &tmB, &full[stage], kb * GEMM_BK, n0);
+            constexpr int BOX = gemm_b_box(BN);
+#pragma unroll
+            for (int j = 0; j < BN / BOX; ++j) tma_load_2d(dB + j * BOX * 128, &tmB, &full[stage], kb * GEMM_BK, n0 + j * BOX);
           } else {
             constexpr int SR = McSub<BN>::ROWS;
             for (int j = (int)cluster_ctarank(); j < BN / SR; j += MC)
@@ -777,8 +816,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
+    if constexpr (SM::PRODUCER_WG) setmaxnreg_inc<SM::REGS_LAUNCH>();   // back to the launch split for whatever follows (gemm_ln_kernel's tail)
   } else {
     // ------------------------------------------------ consumers: wgmma mainloop (MMA warpgroups), accumulator -> smem, epilogue (all)
+    if constexpr (SM::PRODUCER_WG) setmaxnreg_inc<SM::REGS_CONSUMER>();
     const int wg = warp >> 2, lg = warp & 3;
     uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -813,6 +854,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
         else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(acc_free), r));
       }
     }
+    if constexpr (SM::PRODUCER_WG) setmaxnreg_dec<SM::REGS_LAUNCH>();
   }
   EZB_DBG(if (dbg && lane == 0) {
     if (warp == PRODUCER) atomicAdd(&g.dbg[2], (unsigned long long)w0);

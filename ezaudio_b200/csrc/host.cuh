@@ -324,14 +324,13 @@ int launch_gemm_t(Device& dev, cudaStream_t st, const CUtensorMap* tA, const CUt
   return EZB_OK;
 }
 
-// Swap-AB launch: C[tokens, features] = A[tokens, K] W[features, K]^T computed as C^T tiles of 128 features x 256 tokens
+// Swap-AB launch: C[tokens, features] = A[tokens, K] W[features, K]^T computed as C^T tiles of 128 features x BN tokens
 // (single-CTA kernel; W plays the M-side operand, the activations the N-side operand).
-template <class Epi>
-int gemm_swapped(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M_tokens, int N_features, int K,
-                 const typename Epi::Params& ep) {
+template <int BN, class Epi>
+int gemm_swapped_at(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M_tokens, int N_features, int K,
+                    const typename Epi::Params& ep) {
   if (M_tokens <= 0 || N_features <= 0 || K <= 0) return fail(EZB_ERR_SHAPE, "gemm_swapped: empty problem");
   if ((K % 8) || (lda % 8) || (ldw % 8)) return fail(EZB_ERR_SHAPE, "gemm_swapped: K/ld must be multiples of 8");
-  constexpr int BN = 256;
   GemmShape g;
   memset(&g, 0, sizeof g);
   g.M = N_features;
@@ -342,21 +341,39 @@ int gemm_swapped(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, 
   dev.next_weights(W, (size_t)N_features * ldw * 2, &g.pf, &g.pf_bytes);
   const CUtensorMap *tA, *tB;
   EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N_features, (uint64_t)ldw, GEMM_BM, &tA));
-  EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M_tokens, (uint64_t)lda, BN, &tB));
+  EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M_tokens, (uint64_t)lda, gemm_b_box(BN), &tB));
   return launch_gemm_t<BN, Epi>(dev, st, tA, tB, g, ep);
 }
 
-// Swap-AB launch with the activation tile multicast across clusters of MC feature tiles (gemm_wgmma_kernel<.., MC>): the one-wave
+// Token width of the swap-AB tiles, from the compiled set {256, 288}.  The grid is one persistent CTA per SM and the epilogue does not overlap
+// the next tile, so a launch lasts about ceil(tiles / SMs) tile times, and a tile's time grows with its width: take the width with the smaller
+// ceil(tiles / SMs) x width, 256 on a tie.  On 132 SMs with 1152 features (9 feature tiles): 4000 tokens -> 288 (126 tiles in one wave instead
+// of 144 in two), 8000 -> 288 (252 tiles in two waves instead of 288 in three), 6000 -> 256 (two waves either way); 1024 features at 4000
+// tokens -> 256 (128 tiles, one wave).
+inline int swapped_bn(const Device& dev, int M_tokens, int N_features) {
+  const long long mt = (N_features + GEMM_BM - 1) / GEMM_BM;
+  auto span = [&](long long bn) { return (mt * ((M_tokens + bn - 1) / bn) + dev.num_sms - 1) / dev.num_sms * bn; };
+  return span(288) < span(256) ? 288 : 256;
+}
+template <template <int> class Epi>
+int gemm_swapped(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M_tokens, int N_features, int K,
+                 const typename Epi<256>::Params& ep) {
+  if (swapped_bn(dev, M_tokens, N_features) == 288) return gemm_swapped_at<288, Epi<288>>(dev, st, A, lda, W, ldw, M_tokens, N_features, K, ep);
+  return gemm_swapped_at<256, Epi<256>>(dev, st, A, lda, W, ldw, M_tokens, N_features, K, ep);
+}
+
+// Swap-AB launch with the activation tile multicast across clusters of MC feature tiles (gemm_wgmma_kernel<.., MC>, 256-token tiles): the
 // swap-AB GEMMs are L2-feed bound (48 KB per CTA per k-block); sharing the 32 KB token tile between MC = 3 CTAs leaves 26.7 KB.
 // Falls back to the plain launch whenever the shape does not split into whole clusters or the device cannot host them in one wave.
 inline int& opt_swap_mc() {
   static int v = 0;   // off by default
   return v;
 }
-template <class Epi, int MC>
+template <template <int> class EpiT, int MC>
 int gemm_swapped_mc(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M_tokens, int N_features, int K,
-                    const typename Epi::Params& ep) {
+                    const typename EpiT<256>::Params& ep) {
   constexpr int BN = 256;
+  using Epi = EpiT<BN>;
   const int mt = (N_features + GEMM_BM - 1) / GEMM_BM, nt = (M_tokens + BN - 1) / BN, tiles = mt * nt;
   auto kern = gemm_wgmma_kernel<BN, Epi, MC>;
   constexpr int smem = GemmCfg<BN, Epi>::BYTES;
@@ -378,7 +395,7 @@ int gemm_swapped_mc(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int ld
     (void)cudaGetLastError();
   }
   if (mc <= 0 || (mt % MC) || tiles > mc * MC || (K % 8) || (lda % 8) || (ldw % 8))
-    return gemm_swapped<Epi>(dev, st, A, lda, W, ldw, M_tokens, N_features, K, ep);
+    return gemm_swapped<EpiT>(dev, st, A, lda, W, ldw, M_tokens, N_features, K, ep);
   GemmShape g;
   memset(&g, 0, sizeof g);
   g.M = N_features; g.N = M_tokens;

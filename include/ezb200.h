@@ -152,9 +152,15 @@ typedef struct {
   float* out_f32; int32_t ld32;
   void* out_bf16; int32_t ld16; int32_t split_stride;
   int32_t act; const float* act_a; const float* act_b;
+  /* swap-AB kinds only: LayerNorm folded into the epilogue (gemm.cuh FoldIn / FoldOut), null fin_u and fout_st: none.  fin_st / fout_st
+     are float2 (sum, sum of squares) partials, slot-major with pitch fin_ld_st / fout_ld_st. */
+  const void* fin_st; int32_t fin_slots; int32_t fin_ld_st; float fin_inv_dim; const float* fin_u; const float* fin_v;
+  void* fout_st; int32_t fout_ld_st; void* fout_a0; int32_t fout_ld0; const float* fout_g0; void* fout_a1; int32_t fout_ld1; const float* fout_g1;
 } ezb_test_epilogue;
 /* C = A[M,K] W[N,K]^T through the wgmma GEMM; epi_kind 0 = linear epilogue, 1 = GEGLU (packed W); 10 / 11 = the same on 2-CTA
-   clusters; 12 = the cluster GEGLU with 128-deep ring slots (two 64-wide k-blocks per slot); 20 = swap-AB. conv_* = 0 for plain. */
+   clusters; 12 = the cluster GEGLU with 128-deep ring slots (two 64-wide k-blocks per slot); 20 = swap-AB as the model dispatches it
+   (token width chosen from the shape, fold epilogue when a fold is set); 21 = the same with the token width bn (256 or 288).
+   conv_* = 0 for plain. */
 int ezb_test_gemm(int device, const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K, int bn, int epi_kind,
                   const ezb_test_epilogue* e, int conv_taps, int conv_center, int conv_dil, int conv_cin_pad, int conv_T,
                   int conv_B, void* stream);
