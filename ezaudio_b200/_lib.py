@@ -61,9 +61,9 @@ _SIGS = {
     "ezb_dit_finalize_weights": ([_VP, _VP], _I),
     "ezb_dit_set_context": ([_VP, _VP, _VP, _I, _I, _VP], _I),
     "ezb_dit_set_timesteps": ([_VP, C.POINTER(C.c_int64), _I, _VP], _I),
-    "ezb_dit_forward": ([_VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _I, C.POINTER(_VP), _VP, _I, _I, _VP], _I),
+    "ezb_dit_forward": ([_VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _I, C.POINTER(_VP), _VP, _I, _I, _VP, _VP], _I),
     "ezb_controlnet_forward": ([_VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _I, _VP, _F, C.POINTER(_VP), _I, _I, _VP], _I),
-    "ezb_cfg_ddim_step": ([_I, _VP, _VP, _VP, _I, _I, _I, _F, _F, C.POINTER(C.c_float), _VP], _I),
+    "ezb_cfg_ddim_step": ([_I, _VP, _VP, _VP, _I, _I, _I, _F, _F, C.POINTER(C.c_float), _VP, _VP], _I),
     "ezb_option_epoch": ([], C.c_ulonglong),
     "ezb_vae_create": ([C.POINTER(_VP), C.POINTER(VaeDesc), _I], _I),
     "ezb_vae_destroy": ([_VP], _I),
@@ -89,6 +89,7 @@ _SIGS = {
     "ezb_prof_gemm_stats": ([C.c_double, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
     "ezb_test_gemm": ([_I, _VP, _I, _VP, _I, _I, _I, _I, _I, _I, C.POINTER(TestEpilogue), _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_test_attention": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_test_attention_lens": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_test_heads": ([_I, _VP, _VP, C.POINTER(TestHeadsArgs), _VP], _I),
     "ezb_test_mlp": ([_I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP], _I),
 }

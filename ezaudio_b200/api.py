@@ -171,6 +171,7 @@ class EzAudio(_Base):
         p = self.params
         latent_sr = p["autoencoder"]["latent_sr"]
         max_len = int(round(max_length_s * latent_sr))
+        self.max_length_s = float(max_length_s)   # longest clip (seconds) the workspace holds; the batching front-end caps padding at it
         self.noise_scheduler = DDIMScheduler(**p["diff"])
         self.unet = MaskDiT(precision=precision, max_batch=2 * max_batch, max_len=max_len, max_ctx_len=p["text_encoder"]["max_length"],
                             max_timesteps=1000, device=device, **p["model"])
@@ -186,11 +187,20 @@ class EzAudio(_Base):
         self.encode_text = self._make_text_encoder(text_encoder, p, device)
 
     def generate_audio(self, text, length=10, guidance_scale=5, guidance_rescale=0.75, ddim_steps=100, eta=1, random_seed=None,
-                       randomize_seed=False):
-        """api/ezaudio.py:101-130.  Returns (sr, float32 waveform); a list of prompts returns (sr, [waveforms])."""
+                       randomize_seed=False, *, pad_length=None):
+        """api/ezaudio.py:101-130.  Returns (sr, float32 waveform); a list of prompts returns (sr, [waveforms]).
+        With a list of prompts, `length` may list one length (seconds) per prompt: the prompts run as one batch padded to `pad_length`
+        seconds (default: the longest; at most max_length_s), and waveform b has hop * frames(length[b]) samples, equal to that prompt's
+        solo call with the same seed (pass one seed per prompt in `random_seed` to make the batch reproduce solo calls)."""
         batched = not isinstance(text, str)
         prompts = list(text) if batched else [text]
-        length = length * self.params["autoencoder"]["latent_sr"]
+        latent_sr = self.params["autoencoder"]["latent_sr"]
+        if isinstance(length, (list, tuple)):
+            return self._generate_varlen(prompts, batched, length, pad_length, guidance_scale, guidance_rescale, ddim_steps, eta, random_seed,
+                                         randomize_seed)
+        if pad_length is not None:
+            raise ValueError("pad_length applies to a list of per-prompt lengths")
+        length = length * latent_sr
         if all(t == "" for t in prompts):
             guidance_scale = None
             print("empyt input")
@@ -204,6 +214,29 @@ class EzAudio(_Base):
         if batched:
             return sr, [pred[i, 0] for i in range(pred.shape[0])]
         return sr, pred.squeeze(0).squeeze(0)
+
+    def _generate_varlen(self, prompts, batched, length, pad_length, guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, randomize_seed):
+        latent_sr = self.params["autoencoder"]["latent_sr"]
+        if len(length) != len(prompts):
+            raise ValueError(f"length lists one value per prompt: got {len(length)} for {len(prompts)} prompts")
+        frames = [int(v * latent_sr) for v in length]
+        max_frames = int(round(self.max_length_s * latent_sr))
+        L = max(frames) if pad_length is None else int(pad_length * latent_sr)
+        if pad_length is not None and pad_length > self.max_length_s:
+            raise ValueError(f"pad_length {pad_length} s exceeds max_length_s {self.max_length_s} s")
+        if L > max_frames or any(f < 1 or f > L for f in frames):
+            raise ValueError(f"lengths {list(length)} s must be positive and fit the padded length ({L} frames, at most {max_frames})")
+        if all(t == "" for t in prompts):
+            guidance_scale = None
+            print("empyt input")
+        if randomize_seed:
+            random_seed = random.randint(0, MAX_SEED)
+        embeds = self._text_embeds(prompts, [""])
+        wavs = inference(self.autoencoder, self.unet, None, None, None, None, self.params, self.noise_scheduler, prompts, None, L, guidance_scale,
+                         guidance_rescale, ddim_steps, eta, random_seed, self.device, text_embeds=embeds, lengths=frames)
+        sr = self.params["autoencoder"]["sr"]
+        out = [w[0].cpu().numpy() for w in wavs]
+        return (sr, out) if batched else (sr, out[0])
 
     def editing_audio(self, text, boundary, gt_file, mask_start, mask_length, guidance_scale=3.5, guidance_rescale=0, ddim_steps=100,
                       eta=1, random_seed=None, randomize_seed=False):

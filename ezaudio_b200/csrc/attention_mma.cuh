@@ -13,6 +13,10 @@
 //   generation 7            4 warps, 128-key blocks (half as many block barriers and rescales per key)
 // Layouts as produced by the QKV GEMM epilogue: Q, K [B*H, L, DHP] bf16; V^T [B*H, DVP, Lkpad] bf16.  Output [B, Lq, H*dh] bf16
 // token-major.
+// Padded batches (self-attention of clips of different lengths, p.lens): sample b holds len = lens[b] valid tokens.  Keys at or past len are
+// zero-filled like the keys past Lk of a solo run, so valid rows see exactly what a run at Lq = Lk = len sees (bit-identical) and nothing
+// in the padded tokens (not even NaN) reaches them; query rows at or past len are written as zeros.  Those kernels are the VARLEN = true
+// instantiations; without lens the VARLEN = false ones run, compiled without any of this.
 #pragma once
 #include "host.cuh"
 
@@ -36,6 +40,7 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a
 struct AttnMmaParams {
   const __nv_bfloat16 *q, *k, *vt;
   const uint8_t* key_mask;  // [B, Lk] or null
+  const int32_t* lens;      // [B] valid tokens per sample (device; clamped to [1, min(Lq, Lk)]) or null: all Lq / Lk valid
   __nv_bfloat16* out;       // [B, Lq, H*dh]
   int H, Lq, Lk, Lkpad, dh, dhp, dvp;
   float scale_log2;         // (1/sqrt(dh)) * log2(e)
@@ -64,7 +69,7 @@ struct AttnMmaSmem {
   static constexpr int K_ELEMS = KB * KP, V_ELEMS = DK * VP;
   static constexpr size_t bytes(int nbuf) { return (size_t)nbuf * (K_ELEMS + V_ELEMS) * sizeof(__nv_bfloat16); }
 };
-template <int DK, int WARPS, int KB, bool RES>
+template <int DK, int WARPS, int KB, bool RES, bool VARLEN>
 __global__ void __launch_bounds__(WARPS * 32) attn_mma_kernel(const AttnMmaParams p) {
   using SM = AttnMmaSmem<DK, KB>;
   constexpr int KP = SM::KP, VP = SM::VP;
@@ -79,22 +84,29 @@ __global__ void __launch_bounds__(WARPS * 32) attn_mma_kernel(const AttnMmaParam
   const __nv_bfloat16* kb = p.k + (size_t)bh * p.Lk * p.dhp;
   const __nv_bfloat16* vb = p.vt + (size_t)bh * p.dvp * p.Lkpad;
   const uint8_t* mask = p.key_mask != nullptr ? p.key_mask + (size_t)b * p.Lk : nullptr;
-  const int nblk = (p.Lk + KB - 1) / KB;
+  // valid keys / query rows of this sample.  The 128-key-block variants have no register to spare across the key loop (ptxas spills): they
+  // re-read the length where it is needed instead of holding it.
+  auto valid = [&](int n) { return VARLEN ? min(max(p.lens[b], 1), n) : n; };
+  const int lk0 = valid(p.Lk), lq0 = valid(p.Lq);
+  auto klen = [&] { return KB == 128 ? valid(p.Lk) : lk0; };
+  auto qlen = [&] { return KB == 128 ? valid(p.Lq) : lq0; };
+  const int nblk = (lk0 + KB - 1) / KB;
   const int nqt = (p.Lq + QROWS - 1) / QROWS;
   const bool use_poly = p.poly == 1 || (p.poly == 2 && (warp & 1));   // warp-uniform
   const bool no_exp = p.dbg & 1, no_pv = p.dbg & 8, no_s = p.dbg & 16;
 
   auto load_block = [&](int buf, int k0) {
+    const int lk = klen();
     __nv_bfloat16* dK = sK + buf * SM::K_ELEMS;
     __nv_bfloat16* dV = sV + buf * SM::V_ELEMS;
     for (int c = threadIdx.x; c < KB * (DK / 8); c += WARPS * 32) {   // K rows: 8-column chunks
       const int r = c / (DK / 8), col = (c - r * (DK / 8)) * 8, key = k0 + r;
-      const bool ok = key < p.Lk && col < p.dh;
+      const bool ok = key < lk && col < p.dh;
       cp_async16(dK + r * KP + col, ok ? kb + (size_t)key * p.dhp + col : kb, ok ? 16 : 0);
     }
     for (int c = threadIdx.x; c < DK * (KB / 8); c += WARPS * 32) {   // V^T rows: 8-key chunks
       const int d = c / (KB / 8), key = k0 + (c - d * (KB / 8)) * 8;
-      const int n = d < p.dh ? (p.Lk - key < 8 ? p.Lk - key : 8) : 0;
+      const int n = d < p.dh ? (lk - key < 8 ? lk - key : 8) : 0;
       cp_async16(dV + d * VP + key - k0, n > 0 ? vb + (size_t)d * p.Lkpad + key : vb, n > 0 ? 2 * n : 0);
     }
     cp_async_commit();
@@ -107,17 +119,26 @@ __global__ void __launch_bounds__(WARPS * 32) attn_mma_kernel(const AttnMmaParam
 
   for (int qt = RES ? 0 : blockIdx.x; qt < (RES ? nqt : blockIdx.x + 1); ++qt) {
     const int q0 = qt * QROWS + warp * 16;
+    if (VARLEN && qt * QROWS >= qlen()) {   // a tile of padded query rows (CTA-uniform): zeros, no key block is loaded
+      __nv_bfloat16* ob = p.out + (size_t)b * p.Lq * (p.H * p.dh) + (size_t)h * p.dh;
+      for (int i = threadIdx.x; i < QROWS * (p.dh / 2); i += WARPS * 32) {
+        const int r = qt * QROWS + i / (p.dh / 2), col = 2 * (i % (p.dh / 2));
+        if (r < p.Lq) *reinterpret_cast<uint32_t*>(ob + (size_t)r * (p.H * p.dh) + col) = 0u;
+      }
+      continue;
+    }
     if (!RES) load_block(0, 0);
-    // Q fragments of this warp's 16 rows, zero beyond Lq and beyond dh
+    // Q fragments of this warp's 16 rows, zero beyond the sample's valid rows and beyond dh
     uint32_t qa[DK / 16][4];
     {
+      const int lq = qlen();
       const __nv_bfloat16* qb = p.q + (size_t)bh * p.Lq * p.dhp;
 #pragma unroll
       for (int ks = 0; ks < DK / 16; ++ks) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int row = q0 + g + 8 * (i & 1), col = ks * 16 + 2 * t + 8 * (i >> 1);
-          qa[ks][i] = (row < p.Lq && col < p.dh) ? *reinterpret_cast<const uint32_t*>(qb + (size_t)row * p.dhp + col) : 0u;
+          qa[ks][i] = (row < lq && col < p.dh) ? *reinterpret_cast<const uint32_t*>(qb + (size_t)row * p.dhp + col) : 0u;
         }
       }
     }
@@ -148,12 +169,13 @@ __global__ void __launch_bounds__(WARPS * 32) attn_mma_kernel(const AttnMmaParam
       }
       // scale, key mask, block row max
       float bm0 = -INFINITY, bm1 = -INFINITY;
+      const int lk = klen();
 #pragma unroll
       for (int j = 0; j < KB / 8; ++j) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int key = k0 + 8 * j + 2 * t + e;
-          const bool ok = key < p.Lk && (mask == nullptr || mask[key] != 0);
+          const bool ok = key < lk && (mask == nullptr || mask[key] != 0);
           s[j][e] = ok ? s[j][e] * p.scale_log2 : -INFINITY;
           s[j][2 + e] = ok ? s[j][2 + e] * p.scale_log2 : -INFINITY;
           bm0 = fmaxf(bm0, s[j][e]);
@@ -220,14 +242,14 @@ __global__ void __launch_bounds__(WARPS * 32) attn_mma_kernel(const AttnMmaParam
     }
     const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
     const int ld = p.H * p.dh;
-    const int r0 = q0 + g, r1 = q0 + g + 8;
+    const int r0 = q0 + g, r1 = q0 + g + 8, lq = qlen();
     __nv_bfloat16* ob = p.out + (size_t)b * p.Lq * ld + (size_t)h * p.dh;
 #pragma unroll
     for (int j = 0; j < NT; ++j) {
       const int col = 8 * j + 2 * t;
       if (col < p.dh) {
-        if (r0 < p.Lq) *reinterpret_cast<uint32_t*>(ob + (size_t)r0 * ld + col) = pack_bf16(o[j][0] * i0, o[j][1] * i0);
-        if (r1 < p.Lq) *reinterpret_cast<uint32_t*>(ob + (size_t)r1 * ld + col) = pack_bf16(o[j][2] * i1, o[j][3] * i1);
+        if (r0 < p.Lq) *reinterpret_cast<uint32_t*>(ob + (size_t)r0 * ld + col) = (!VARLEN || r0 < lq) ? pack_bf16(o[j][0] * i0, o[j][1] * i0) : 0u;
+        if (r1 < p.Lq) *reinterpret_cast<uint32_t*>(ob + (size_t)r1 * ld + col) = (!VARLEN || r1 < lq) ? pack_bf16(o[j][2] * i1, o[j][3] * i1) : 0u;
       }
     }
   }
@@ -265,14 +287,14 @@ inline int attention_variant() { return opt_attn7() ? 7 : (opt_attn6() & 1) ? 6 
 
 template <int DK, int WARPS, int KB, bool RES>
 int attn_mma_launch(cudaStream_t st, const AttnMmaParams& p, int B, int H) {
-  auto kern = attn_mma_kernel<DK, WARPS, KB, RES>;
+  auto kern = p.lens ? attn_mma_kernel<DK, WARPS, KB, RES, true> : attn_mma_kernel<DK, WARPS, KB, RES, false>;
   const size_t smem = AttnMmaSmem<DK, KB>::bytes(RES ? AM_RES_KEYS / KB : 2);
-  static int attr_set = -1;   // function attributes are per device
+  static int attr_set[2] = {-1, -1};   // function attributes are per device and kernel
   int dev = 0;
   EZB_CUDA(cudaGetDevice(&dev));
-  if (smem > 48 * 1024 && attr_set != dev) {
+  if (smem > 48 * 1024 && attr_set[p.lens != nullptr] != dev) {
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = dev;
+    attr_set[p.lens != nullptr] = dev;
   }
   const dim3 grid(RES ? 1 : (p.Lq + 16 * WARPS - 1) / (16 * WARPS), B * H);
   ++launch_counter();
@@ -291,14 +313,16 @@ int attn_mma_dispatch(cudaStream_t st, const AttnMmaParams& p, int B, int H, int
 }
 
 // variant: 4, 6 or 7 (see the file comment); 0 = the one the options select
+// lens: [B] valid tokens per sample (device) or null, see the file comment
 inline int attention_mma(Device& dev, cudaStream_t st, const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, const uint8_t* key_mask,
-                         __nv_bfloat16* out, int B, int H, int Lq, int Lk, int Lkpad, int dh, int dhp, int dvp, float scale, int variant = 0) {
+                         __nv_bfloat16* out, int B, int H, int Lq, int Lk, int Lkpad, int dh, int dhp, int dvp, float scale, int variant = 0,
+                         const int32_t* lens = nullptr) {
   (void)dev;
   if (dh % 8 || dh > 80) return fail(EZB_ERR_UNSUPPORTED, "attention: head dimension %d (multiples of 8 up to 80)", dh);
   if (dhp < dh || dhp % 8 || dvp < dh || Lkpad < Lk || Lkpad % 8) return fail(EZB_ERR_SHAPE, "attention: pitches dhp %d dvp %d Lkpad %d", dhp, dvp, Lkpad);
   if (B < 1 || H < 1 || Lq < 1 || Lk < 1) return fail(EZB_ERR_SHAPE, "attention: empty problem");
   AttnMmaParams p;
-  p.q = q; p.k = k; p.vt = vt; p.key_mask = key_mask; p.out = out;
+  p.q = q; p.k = k; p.vt = vt; p.key_mask = key_mask; p.lens = lens; p.out = out;
   p.H = H; p.Lq = Lq; p.Lk = Lk; p.Lkpad = Lkpad; p.dh = dh; p.dhp = dhp; p.dvp = dvp;
   p.scale_log2 = scale * 1.4426950408889634f;
   if (variant == 0) variant = attention_variant();

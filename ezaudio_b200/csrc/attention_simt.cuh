@@ -2,6 +2,9 @@
 // with scale 1 and a relative-position bias: T5Attention).
 // Used by the bf16x3 parity mode (fp32-grade numerics) and as the on-device comparator of the tensor-core kernel.
 // q,k,v fp32 [B,H,L,dh]; out bf16 [B, Lq, H*dh] token-major (A operand of the output projection).
+// lens ([B] device, or null): sample b holds lens[b] valid tokens (padded batch of clips of different lengths).  Keys at or past it are
+// skipped like the keys past Lk of a solo run (same bits for the valid rows, nothing from the padded tokens reaches them); query rows at
+// or past it are written as zeros.  VARLEN = false (lens null) compiles the uniform-length kernel without any of this.
 #pragma once
 #include "elementwise.cuh"
 
@@ -16,9 +19,10 @@ constexpr int SA_WARPS = 4;
 // (dh % 4 == 0): K rows at a 16-byte-aligned pitch whose quarter-warp LDS.128 phases are conflict-free, q / k / p read as float4 (10 LDS.128 per 64
 // FMAs), and the probabilities go through a per-warp shared tile and come back as broadcast LDS.128 (no shuffles).  Every accumulator still sums in the
 // same order (d ascending, keys ascending), so the output bits are unchanged.
+template <bool VARLEN>
 __global__ void __launch_bounds__(SA_WARPS * 32) attn_simt_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                                                                   const uint8_t* __restrict__ key_mask, __nv_bfloat16* __restrict__ out, int H, int Lq,
-                                                                  int Lk, int dh, float scale, int kmul,
+                                                                  int Lk, int dh, float scale, int kmul, const int32_t* __restrict__ lens,
                                                                   const float* __restrict__ bias = nullptr /* [H, Lq, Lk] added to the scores (T5) */) {
   extern __shared__ __align__(16) float sm[];
   const int ldk = ((dh >> 2) & 1) ? dh : dh + 4;   // pitch / 4 odd: the 8 lanes of an LDS.128 phase hit 8 different 16-byte bank groups
@@ -29,27 +33,40 @@ __global__ void __launch_bounds__(SA_WARPS * 32) attn_simt_kernel(const float* _
   const int bh = blockIdx.y, b = bh / H, h = bh - b * H;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * (SA_WARPS * SA_QW);
+  const int D = H * dh;
+  int lk = Lk, lq = Lq;   // valid keys / query rows of this sample
+  if (VARLEN) {
+    const int n = max(lens[b], 1);
+    lk = min(n, lk); lq = min(n, lq);
+  }
+  if (VARLEN && q0 >= lq) {   // a tile of padded query rows (CTA-uniform): zeros
+    for (int i = threadIdx.x; i < SA_WARPS * SA_QW * dh; i += blockDim.x) {
+      const int qrow = q0 + i / dh;
+      if (qrow < Lq) store_act(out + ((size_t)b * Lq + qrow) * kmul * D, h * dh + i % dh, D, kmul, 0.f);
+    }
+    return;
+  }
   const float* qb = q + (size_t)bh * Lq * dh;
   const float* kb = k + (size_t)bh * Lk * dh;
   const float* vb = v + (size_t)bh * Lk * dh;
   for (int i = threadIdx.x; i < SA_WARPS * SA_QW * dh; i += blockDim.x) {
     const int r = i / dh, d = i - r * dh;
-    sQ[i] = (q0 + r < Lq) ? qb[(size_t)(q0 + r) * dh + d] * scale : 0.f;
+    sQ[i] = (q0 + r < lq) ? qb[(size_t)(q0 + r) * dh + d] * scale : 0.f;
   }
   float m[SA_QW], l[SA_QW], acc[SA_QW][3];
 #pragma unroll
   for (int i = 0; i < SA_QW; ++i) { m[i] = -INFINITY; l[i] = 0.f; acc[i][0] = acc[i][1] = acc[i][2] = 0.f; }
   float* sPw = sP + warp * (SA_QW * SA_TK);
-  for (int k0 = 0; k0 < Lk; k0 += SA_TK) {
+  for (int k0 = 0; k0 < lk; k0 += SA_TK) {
     __syncthreads();
     for (int i = threadIdx.x; i < SA_TK * dh; i += blockDim.x) {
       const int r = i / dh, d = i - r * dh;
-      const bool ok = k0 + r < Lk;
+      const bool ok = k0 + r < lk;
       sK[r * ldk + d] = ok ? kb[(size_t)(k0 + r) * dh + d] : 0.f;
       sV[r * dh + d] = ok ? vb[(size_t)(k0 + r) * dh + d] : 0.f;
     }
     __syncthreads();
-    bool ok0 = k0 + lane < Lk, ok1 = k0 + lane + 32 < Lk;
+    bool ok0 = k0 + lane < lk, ok1 = k0 + lane + 32 < lk;
     if (key_mask) {
       ok0 = ok0 && key_mask[(size_t)b * Lk + k0 + lane];
       ok1 = ok1 && key_mask[(size_t)b * Lk + k0 + lane + 32];
@@ -119,16 +136,16 @@ __global__ void __launch_bounds__(SA_WARPS * 32) attn_simt_kernel(const float* _
     }
     __syncwarp();   // the probabilities of this tile are consumed before the next tile overwrites them
   }
-  const int D = H * dh;
 #pragma unroll
   for (int qi = 0; qi < SA_QW; ++qi) {
     const int qrow = q0 + warp * SA_QW + qi;
     if (qrow >= Lq) continue;
     const float inv = 1.f / l[qi];
+    const bool valid = !VARLEN || qrow < lq;
     __nv_bfloat16* o = out + ((size_t)b * Lq + qrow) * kmul * D;
 #pragma unroll
     for (int i = 0; i < 3; ++i)
-      if (lane + 32 * i < dh) store_act(o, h * dh + lane + 32 * i, D, kmul, acc[qi][i] * inv);
+      if (lane + 32 * i < dh) store_act(o, h * dh + lane + 32 * i, D, kmul, valid ? acc[qi][i] * inv : 0.f);
   }
 }
 

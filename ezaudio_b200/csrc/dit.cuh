@@ -97,6 +97,7 @@ struct Dit {
   std::vector<bf16*> cat;   // MaskDiT: per in-block [Mx, 2D] = [x of the paired out-block * snw[:D] | this block's output * snw[D:]]; ControlNet: [Mx, D] plain cast
   int geglu_bn = 128;     // N-tile of the GEGLU GEMM: packing group = geglu_bn / 2
   int qkv3_bn = 0;        // >0: self-attention QKV weight packed three heads per N-tile of this width (EpiHeads<DH,3>)
+  const int32_t* lens = nullptr;   // forward(): valid frames per sample of the padded batch (device [Be]) or null; read by self-attention and the final conv
 
   ~Dit() {
     for (void* p : allocs) cudaFree(p);
@@ -624,22 +625,28 @@ struct Dit {
     else { e.out_bf16 = reinterpret_cast<bf16*>(qkv); e.ld16 = N; }
     return lin(st, A, K, W, M, N, e);
   }
+  // lens_: valid tokens per sample (self-attention of a padded batch) or null
   int attention(cudaStream_t st, const float* q32_, const float* k32_, const float* v32_, const bf16* q16_, const bf16* k16_, const bf16* vt16_,
-                const uint8_t* mask, int B, int Lq, int Lk, int Lkpad) {
+                const uint8_t* mask, int B, int Lq, int Lk, int Lkpad, const int32_t* lens_ = nullptr) {
     const float scale = 1.0f / sqrtf((float)dh);
     if (opt_skip() & 2) return EZB_OK;
     if (!use_tc_attention) {
       if (dh % 4) return fail(EZB_ERR_UNSUPPORTED, "fp32 attention: head dimension %d is not a multiple of 4", dh);
       const size_t smem = attn_simt_smem(dh);
       static bool set[16] = {};  // function attributes are per device
-      if (!set[dev->id & 15]) { EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); set[dev->id & 15] = true; }
+      if (!set[dev->id & 15]) {
+        EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        set[dev->id & 15] = true;
+      }
       dim3 grid((Lq + SA_WARPS * SA_QW - 1) / (SA_WARPS * SA_QW), B * H);
       ++launch_counter();
-      attn_simt_kernel<<<grid, SA_WARPS * 32, smem, st>>>(q32_, k32_, v32_, mask, attn_out, H, Lq, Lk, dh, scale, kmul);
+      auto kern = lens_ ? attn_simt_kernel<true> : attn_simt_kernel<false>;
+      kern<<<grid, SA_WARPS * 32, smem, st>>>(q32_, k32_, v32_, mask, attn_out, H, Lq, Lk, dh, scale, kmul, lens_, nullptr);
       EZB_CUDA(cudaGetLastError());
       return EZB_OK;
     }
-    return attention_mma(*dev, st, q16_, k16_, vt16_, mask, attn_out, B, H, Lq, Lk, Lkpad, dh, DHP, DVP, scale);
+    return attention_mma(*dev, st, q16_, k16_, vt16_, mask, attn_out, B, H, Lq, Lk, Lkpad, dh, DHP, DVP, scale, 0, lens_);
   }
 
   // ---------------------------------------------------------------- step-invariant precompute
@@ -784,7 +791,7 @@ struct Dit {
       const int Lp = (L + 7) / 8 * 8;
       FoldIn f1 = fold_in(st1, nullptr, D, w.u1 + (size_t)fc.t * n_qkv, w.v1 + (size_t)fc.t * n_qkv);
       EZB_TRY(lin_heads(st, act, w.qkv, M, 3 * D, kinds, w.h_nq, w.h_nk, true, L, q16, k16, vt16, Lp, fold1 ? &f1 : nullptr));
-      EZB_TRY(attention(st, q32, k32, v32, q16, k16, vt16, nullptr, Be, L, L, Lp));
+      EZB_TRY(attention(st, q32, k32, v32, q16, k16, vt16, nullptr, Be, L, L, Lp, lens));
     } else {
       EZB_TRY(lin_to_qkv(st, act, D, w.qkv, M, 3 * D));
       const int off[3] = {0, D, 2 * D}, kinds[3] = {0, 1, 2};
@@ -792,7 +799,7 @@ struct Dit {
       bf16* bfo[3] = {q16, k16, vt16};
       const int Lp = (L + 7) / 8 * 8;
       EZB_TRY(qk_prep(st, 3 * D, 3, off, kinds, w.nqw, w.nqb, w.nkw, w.nkb, w.inv_freq, Be, L, f32o, bfo, Lp));
-      EZB_TRY(attention(st, q32, k32, v32, q16, k16, vt16, nullptr, Be, L, L, Lp));
+      EZB_TRY(attention(st, q32, k32, v32, q16, k16, vt16, nullptr, Be, L, L, Lp, lens));
     }
     {
       EpiLinearParams e = epi();
@@ -880,10 +887,14 @@ struct Dit {
     return EZB_OK;
   }
 
+  // lens_ (device [Be] or null): sample b is a clip of lens_[b] <= L frames padded to L.  Only self-attention and the final conv mix
+  // frames; both stop at the clip end, so its frames come out as a solo forward at that length computes them.  Every other kernel works
+  // per token.
   int forward(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const float* const* cskips, float* out, int Be, int L,
-              cudaStream_t st) {
+              const int32_t* lens_, cudaStream_t st) {
     if (d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_dit_forward called on a controlnet handle");
     EZB_TRY(check_call(Be, L));
+    lens = lens_;
     dev->tmaps.trim();
     WeightSeqScope ws(dev, this, cskips ? 1 : 0, ((long long)Be << 32) | (unsigned)L);   // L2 prefetch of the next GEMM's weights (host.cuh)
     const float *modr, *modf;
@@ -943,7 +954,7 @@ struct Dit {
     static bool fc_attr[16] = {};   // function attributes are per device
     if (!fc_attr[dev->id & 15]) { EZB_CUDA(cudaFuncSetAttribute(final_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); fc_attr[dev->id & 15] = true; }
     if (smem > 160 * 1024) return fail(EZB_ERR_UNSUPPORTED, "final conv: %d channels exceed the shared-memory tile", C);
-    EZB_TRY(launch_k(final_conv_kernel, grid, dim3(128 * FC_GROUPS), smem, st, 1, (const float*)ybuf, (const float*)fc_w, (const float*)fc_b, out, Be, C, L));
+    EZB_TRY(launch_k(final_conv_kernel, grid, dim3(128 * FC_GROUPS), smem, st, 1, (const float*)ybuf, (const float*)fc_w, (const float*)fc_b, out, Be, C, L, lens));
     ws.ok = true;
     return EZB_OK;
   }
@@ -961,6 +972,7 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
                                    float* const* skips_out, int Be, int L, cudaStream_t st) {
   if (!d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_controlnet_forward called on a DiT handle");
   EZB_TRY(check_call(Be, L));
+  lens = nullptr;   // the stem convs cross clip ends: ControlNet batches are uniform in length
   dev->tmaps.trim();
   WeightSeqScope ws(dev, this, 2, ((long long)Be << 32) | (unsigned)L);
   const float *modr, *modf;

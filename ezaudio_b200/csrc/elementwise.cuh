@@ -399,18 +399,22 @@ __global__ void patch_pack_kernel(const float* __restrict__ x, const float* __re
 // thread = 4 output channels x 8 positions, so one input channel costs 10 broadcast LDS + 3 coalesced float4 weight loads for 96 FMAs; the four
 // groups' partial sums meet in shared memory.  (Four warps per SM walking all 128 input channels cannot hide the L2 latency of the weight
 // loads; this one: 16 warps.)
+// lens ([B] device, or null): clip b ends at lens[b] frames of the padded L.  Frames at or past it are the zero halo a solo run of that
+// length sees, and are not written.
 constexpr int FC_GROUPS = 4;
 __global__ void __launch_bounds__(128 * FC_GROUPS) final_conv_kernel(const float* __restrict__ y, const float* __restrict__ wp, const float* __restrict__ bias,
-                                                                     float* __restrict__ out, int B, int C, int L) {
+                                                                     float* __restrict__ out, int B, int C, int L, const int32_t* __restrict__ lens) {
   pdl_launch();
   pdl_wait();
   constexpr int TL = 32, TP = TL + 2 + 2;  // 34 positions (+2 so that the 10-wide window of the last thread group stays in bounds)
   extern __shared__ float sy[];             // [C][TP] channel-major, then [FC_GROUPS - 1][128][32] partial sums
   float* red = sy + (size_t)C * TP;
   const int b = blockIdx.y, l0 = blockIdx.x * TL;
+  const int len = lens != nullptr ? min(max(lens[b], 1), L) : L;
+  if (l0 >= len) return;   // CTA-uniform: a tile of padding only
   for (int i = threadIdx.x; i < (TL + 2) * C; i += blockDim.x) {
     const int r = i / C, c = i - r * C, l = l0 + r - 1;
-    sy[c * TP + r] = (l >= 0 && l < L) ? y[((size_t)b * L + l) * C + c] : 0.f;
+    sy[c * TP + r] = (l >= 0 && l < len) ? y[((size_t)b * L + l) * C + c] : 0.f;
   }
   __syncthreads();
   const int gq = threadIdx.x >> 7, t128 = threadIdx.x & 127;
@@ -463,7 +467,7 @@ __global__ void __launch_bounds__(128 * FC_GROUPS) final_conv_kernel(const float
 #pragma unroll
         for (int t = 0; t < 8; ++t) {
           const int l = l0 + tq * 8 + t;
-          if (l < L) out[((size_t)b * C + co + e) * L + l] = acc[t][e];
+          if (l < len) out[((size_t)b * C + co + e) * L + l] = acc[t][e];
         }
     }
     __syncthreads();
@@ -583,6 +587,9 @@ __global__ void permute3_kernel(const float* __restrict__ src, float* __restrict
 // One CLUSTER of CFG_CLUSTER CTAs per sample (one CTA per sample would leave all but a handful of SMs idle):
 // every CTA reduces the four sums of its slice (double accumulation, fixed order -> deterministic), the partials are exchanged
 // through distributed shared memory, every CTA forms the same ratio and updates its slice.
+// Tensors are [B, C, L].  lens ([B] device, or null = L): sample b covers the first lens[b] frames of each channel.  Its n = C * lens[b]
+// elements are walked in the order of a solo call on a [1, C, lens[b]] tensor (element i at (i / lens[b]) * L + i % lens[b]), so sums and
+// updates are bit-identical to that call; the padded frames are not touched.
 constexpr int CFG_CLUSTER = 8;
 __device__ __forceinline__ double ld_dsmem_f64(const double* local, uint32_t rank) {
   double v;
@@ -590,15 +597,19 @@ __device__ __forceinline__ double ld_dsmem_f64(const double* local, uint32_t ran
   return v;
 }
 __global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
-                                                        const float* __restrict__ noise, int n, float gs, float gr, float c0, float c1, float c2, float c3,
-                                                        float c4) {
+                                                        const float* __restrict__ noise, const int32_t* __restrict__ lens, int C, int L, float gs, float gr,
+                                                        float c0, float c1, float c2, float c3, float c4) {
   __shared__ double red[4][32];
   __shared__ double part[4];
   pdl_launch();
   pdl_wait();
   const uint32_t rank = cluster_ctarank();
   const int sample = blockIdx.x / CFG_CLUSTER;
-  const size_t base = (size_t)sample * n;
+  const size_t base = (size_t)sample * C * L;
+  const int len = lens != nullptr ? min(max(lens[sample], 1), L) : L;
+  const int n = C * len;
+  const bool packed = len == L;   // element i lives at i
+  auto at = [&](int i) { return packed ? i : (i / len) * L + i % len; };
   const int per = (((n + CFG_CLUSTER - 1) / CFG_CLUSTER) + 3) & ~3;   // slice of this CTA, multiple of 4 elements
   const int lo = (int)rank * per, hi = (lo + per < n) ? lo + per : n;
   const float* t = out_text + base;
@@ -608,7 +619,8 @@ __global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict_
   if (rescale) {
     double st = 0, st2 = 0, sc = 0, sc2 = 0;
     for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-      const float a = t[i], c = u[i] + gs * (a - u[i]);
+      const int j = at(i);
+      const float a = t[j], c = u[j] + gs * (a - u[j]);
       st += a; st2 += (double)a * a; sc += c; sc2 += (double)c * c;
     }
     double v[4] = {st, st2, sc, sc2};
@@ -635,16 +647,17 @@ __global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict_
   float* x = latents + base;
   const float* z = noise ? noise + base : nullptr;
   for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-    float v = t[i];
+    const int j = at(i);
+    float v = t[j];
     if (u) {
-      v = u[i] + gs * (v - u[i]);
+      v = u[j] + gs * (v - u[j]);
       if (gr > 0.f) v = gr * (v * ratio) + (1.f - gr) * v;
     }
-    const float xi = x[i];
+    const float xi = x[j];
     const float x0 = c0 * xi - c1 * v, eps = c0 * v + c1 * xi;
     float prev = c2 * x0 + c3 * eps;
-    if (z) prev += c4 * z[i];
-    x[i] = prev;
+    if (z) prev += c4 * z[j];
+    x[j] = prev;
   }
 }
 

@@ -43,7 +43,7 @@ EpiLinearParams to_epi(const ezb_test_epilogue* e) {
 
 extern "C" {
 
-__attribute__((visibility("default"))) int ezb_version(void) { return 1; }
+__attribute__((visibility("default"))) int ezb_version(void) { return 2; }
 __attribute__((visibility("default"))) const char* ezb_last_error(void) { return last_error().c_str(); }
 
 __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void* A, int lda, const void* W, int ldw, int M, int N, int K, int bn, int epi_kind,
@@ -257,9 +257,9 @@ EZB_API int ezb_dit_set_timesteps(ezb_dit* h, const int64_t* ts, int n, void* st
   return reinterpret_cast<Dit*>(h)->set_timesteps(ts, n, ST(stream));
 }
 EZB_API int ezb_dit_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall,
-                            const float* const* cskips, float* out, int Be, int L, void* stream) {
+                            const float* const* cskips, float* out, int Be, int L, void* stream, const int32_t* lens) {
   if (!h || !x || !out) return fail(EZB_ERR_ARG, "ezb_dit_forward: null argument");
-  return reinterpret_cast<Dit*>(h)->forward(x, gt, gt_mask, tidx, tall, cskips, out, Be, L, ST(stream));
+  return reinterpret_cast<Dit*>(h)->forward(x, gt, gt_mask, tidx, tall, cskips, out, Be, L, lens, ST(stream));
 }
 EZB_API int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall,
                                    const float* condition, float scale, float* const* skips_out, int Be, int L, void* stream) {
@@ -267,14 +267,13 @@ EZB_API int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, 
   return reinterpret_cast<Dit*>(h)->controlnet_forward(x, gt, gt_mask, tidx, tall, condition, scale, skips_out, Be, L, ST(stream));
 }
 EZB_API int ezb_cfg_ddim_step(int device, const float* model_out, float* latents, const float* noise, int B, int C, int L, float gs, float gr,
-                              const float* coef, void* stream) {
+                              const float* coef, void* stream, const int32_t* lens) {
   if (!model_out || !latents || !coef || B < 1 || C < 1 || L < 1) return fail(EZB_ERR_ARG, "ezb_cfg_ddim_step: bad argument");
   if (coef[4] != 0.f && !noise) return fail(EZB_ERR_ARG, "ezb_cfg_ddim_step: sigma != 0 needs a noise tensor");
   EZB_CUDA(cudaSetDevice(device));
-  const int n = C * L;
-  const float* uncond = gs != 0.f ? model_out + (size_t)B * n : nullptr;
+  const float* uncond = gs != 0.f ? model_out + (size_t)B * C * L : nullptr;
   return launch_k(cfg_ddim_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, uncond, latents,
-                  coef[4] != 0.f ? noise : (const float*)nullptr, n, gs, gr, coef[0], coef[1], coef[2], coef[3], coef[4]);
+                  coef[4] != 0.f ? noise : (const float*)nullptr, lens, C, L, gs, gr, coef[0], coef[1], coef[2], coef[3], coef[4]);
 }
 EZB_API int ezb_vae_create(ezb_vae** out, const ezb_vae_desc* desc, int device) {
   if (!out || !desc) return fail(EZB_ERR_ARG, "ezb_vae_create: null argument");
@@ -372,20 +371,24 @@ EZB_API int ezb_vae_decode(ezb_vae* h, const float* z, float* wav, int B, int L,
   if (!h || !z || !wav) return fail(EZB_ERR_ARG, "ezb_vae_decode: null argument");
   return reinterpret_cast<Vae*>(h)->decode(z, wav, B, L, ST(stream));
 }
+}  // extern "C"
+
+namespace {
 // impl 0: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]); impl 1/4/6/7 (+100): tensor-core kernel (q,k bf16 [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad])
-EZB_API int ezb_test_attention(int device, const void* q, const void* k, const void* v, const uint8_t* key_mask, void* out, int B, int H, int Lq,
-                               int Lk, int dh, int impl, void* stream) {
+int test_attention(int device, const void* q, const void* k, const void* v, const uint8_t* key_mask, const int32_t* lens, void* out, int B, int H,
+                   int Lq, int Lk, int dh, int impl, void* stream) {
   if (!q || !k || !v || !out) return fail(EZB_ERR_ARG, "ezb_test_attention: null pointer");
   EZB_CUDA(cudaSetDevice(device));
   const float scale = 1.0f / sqrtf((float)dh);
   if (impl == 0) {
     if (dh % 4) return fail(EZB_ERR_UNSUPPORTED, "fp32 attention: head dimension %d is not a multiple of 4", dh);
-    EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    auto kern = lens ? attn_simt_kernel<true> : attn_simt_kernel<false>;
+    EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     dim3 grid((Lq + SA_WARPS * SA_QW - 1) / (SA_WARPS * SA_QW), B * H);
     ++launch_counter();
-    attn_simt_kernel<<<grid, SA_WARPS * 32, attn_simt_smem(dh), ST(stream)>>>(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
+    kern<<<grid, SA_WARPS * 32, attn_simt_smem(dh), ST(stream)>>>(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
                                                                             reinterpret_cast<const float*>(v), key_mask,
-                                                                            reinterpret_cast<__nv_bfloat16*>(out), H, Lq, Lk, dh, scale, 1);
+                                                                            reinterpret_cast<__nv_bfloat16*>(out), H, Lq, Lk, dh, scale, 1, lens, nullptr);
     EZB_CUDA(cudaGetLastError());
     return EZB_OK;
   }
@@ -396,7 +399,20 @@ EZB_API int ezb_test_attention(int device, const void* q, const void* k, const v
   const int dhp = (row80 && dh == 72) ? 80 : (dh + 63) / 64 * 64;
   const int dvp = (dh + 15) / 16 * 16, lkpad = (Lk + 7) / 8 * 8;
   return attention_mma(device_ctx(device), ST(stream), reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-                       reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale, variant == 1 ? 0 : variant);
+                       reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale, variant == 1 ? 0 : variant,
+                       lens);
+}
+}  // namespace
+
+extern "C" {
+EZB_API int ezb_test_attention(int device, const void* q, const void* k, const void* v, const uint8_t* key_mask, void* out, int B, int H, int Lq,
+                               int Lk, int dh, int impl, void* stream) {
+  return test_attention(device, q, k, v, key_mask, nullptr, out, B, H, Lq, Lk, dh, impl, stream);
+}
+EZB_API int ezb_test_attention_lens(int device, const void* q, const void* k, const void* v, const int32_t* lens, void* out, int B, int H, int L, int dh,
+                                    int impl, void* stream) {
+  if (!lens) return fail(EZB_ERR_ARG, "ezb_test_attention_lens: null lengths");
+  return test_attention(device, q, k, v, nullptr, lens, out, B, H, L, L, dh, impl, stream);
 }
 
 

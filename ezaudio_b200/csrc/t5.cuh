@@ -247,7 +247,7 @@ struct T5 {
     EpiLinearParams z;
     memset(&z, 0, sizeof z);
     static bool attr[16] = {};  // function attributes are per device
-    if (!attr[dev->id & 15]) { EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr[dev->id & 15] = true; }
+    if (!attr[dev->id & 15]) { EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr[dev->id & 15] = true; }
     for (int i = 0; i < nl; ++i) {
       const Layer& w = layers[i];
       ++launch_counter();
@@ -258,7 +258,7 @@ struct T5 {
       launch_counter() += 2;
       t5_heads_kernel<<<grid((size_t)M * 3 * inner), 256, 0, st>>>(qkv32, q32, k32, v32, B, L, H, dk);
       dim3 ga((L + SA_WARPS * SA_QW - 1) / (SA_WARPS * SA_QW), B * H);
-      attn_simt_kernel<<<ga, SA_WARPS * 32, attn_simt_smem(dk), st>>>(q32, k32, v32, mask, attn, H, L, L, dk, 1.0f /* T5: no 1/sqrt(d) */, kmul, bias);
+      attn_simt_kernel<false><<<ga, SA_WARPS * 32, attn_simt_smem(dk), st>>>(q32, k32, v32, mask, attn, H, L, L, dk, 1.0f /* T5: no 1/sqrt(d) */, kmul, nullptr, bias);
       EZB_CUDA(cudaGetLastError());
       e = z;
       e.resid = x; e.ldr = D; e.out_f32 = x; e.ld32 = D;

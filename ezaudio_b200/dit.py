@@ -175,16 +175,24 @@ class MaskDiT:
     def set_timesteps(self, ts):
         self._h.set_timesteps(ts)
 
-    def forward_step(self, x, step_index: int, gt=None, gt_mask_u8=None, controlnet_skips=None, out=None):
-        """One denoiser forward at table row `step_index` (all samples share it).  x (Be,C,L) fp32 cuda."""
+    def forward_step(self, x, step_index: int, gt=None, gt_mask_u8=None, controlnet_skips=None, out=None, lengths=None):
+        """One denoiser forward at table row `step_index` (all samples share it).  x (Be,C,L) fp32 cuda.
+        `lengths`: None, or a cuda int32 tensor (Be,) of clip lengths in 1..L (padded batch): frames < lengths[b] of sample b come out as a
+        forward of that clip alone computes them; frames past it are not written.  The values are read on the device when the kernels run
+        (so a captured graph follows later copies into the tensor) and are not checked here: the caller validates them."""
         Be, Cc, L = x.shape
+        if lengths is not None:
+            if gt is not None or controlnet_skips is not None:
+                raise NotImplementedError("per-sample lengths with inpainting (gt) or ControlNet skips")
+            if lengths.dtype != torch.int32 or not lengths.is_cuda or tuple(lengths.shape) != (Be,) or not lengths.is_contiguous():
+                raise ValueError(f"lengths must be a contiguous cuda int32 tensor of shape ({Be},)")
         out = torch.empty_like(x) if out is None else out
         sk = None
         if controlnet_skips is not None:
             sk = (C.c_void_p * len(controlnet_skips))(*[s.data_ptr() for s in controlnet_skips])
         with torch.cuda.device(self._h.dev_index):
             _lib.check(_lib.lib().ezb_dit_forward(self._h.h, _lib.ptr(x), _lib.ptr(gt), _lib.ptr(gt_mask_u8), None, int(step_index),
-                                                  sk, _lib.ptr(out), Be, L, _lib.stream_ptr()))
+                                                  sk, _lib.ptr(out), Be, L, _lib.stream_ptr(), _lib.ptr(lengths)))
         return out
 
     def _forward_raw(self, x, gt, gt_mask, timesteps, context, context_mask, controlnet_skips, gt_is_final=False):
@@ -208,7 +216,7 @@ class MaskDiT:
             self._keep_sk = sks
         with torch.cuda.device(h.dev_index):
             _lib.check(_lib.lib().ezb_dit_forward(h.h, _lib.ptr(x), _lib.ptr(gtc), _lib.ptr(m8), arr, 0, sk, _lib.ptr(out), Be, L,
-                                                  _lib.stream_ptr()))
+                                                  _lib.stream_ptr(), None))
         return out
 
     def __call__(self, x, timesteps, context, x_mask=None, context_mask=None, cls_token=None, gt=None, mae_mask_infer=None,

@@ -7,12 +7,17 @@ ranks (prompts are independent units: `ezaudio_b200.shard`), runs them through `
 the waveforms back in completion order (`stream`) or in request order (`run`).  Per-request seeds are honoured: prompt i of a batch
 draws from torch.Generator(seed_i), so a request's audio does not depend on what it was batched with.
 
+With `length_bucket_s` set, requests of different lengths share a batch: they group by ceil(length / bucket) instead of the exact
+length, and the batch is padded to its bucket's top (capped at the backend's `max_length_s`), so there is one graph shape per bucket.
+The backend then gets `length=[per-request lengths]` and `pad_length=`, and each request still gets exactly its solo audio.
+
 Pure host logic: the backend is any object with the reference-shaped `generate_audio(text, length=, guidance_scale=, guidance_rescale=,
 ddim_steps=, eta=, random_seed=)`; tests drive it with a stub on CPU."""
 from __future__ import annotations
 
 import collections
 import dataclasses
+import math
 from typing import Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
 
@@ -27,10 +32,16 @@ class Request:
     eta: float = 1
     random_seed: Optional[int] = None
 
-    def group_key(self) -> Tuple:
+    def group_key(self, length_bucket_s: Optional[float] = None) -> Tuple:
         # "" switches guidance off for the whole call (api/ezaudio.py:109-111): empty prompts only batch with empty prompts
-        return (self.length, float(self.guidance_scale or 0.0), float(self.guidance_rescale or 0.0), int(self.ddim_steps), float(self.eta or 0.0),
+        size = self.length if length_bucket_s is None else ("bucket", length_bucket_bin(self.length, length_bucket_s))
+        return (size, float(self.guidance_scale or 0.0), float(self.guidance_rescale or 0.0), int(self.ddim_steps), float(self.eta or 0.0),
                 self.prompt == "")
+
+
+def length_bucket_bin(length: float, length_bucket_s: float) -> int:
+    """Bucket index of a clip length: ceil(length / bucket), so bucket k holds lengths in ((k - 1) * bucket, k * bucket]."""
+    return max(1, math.ceil(length / length_bucket_s - 1e-9))
 
 
 @dataclasses.dataclass
@@ -38,20 +49,26 @@ class Batch:
     key: Tuple
     tickets: List[int]
     requests: List[Request]
+    pad_length: Optional[float] = None   # bucketed plans: the top of the bucket (seconds)
 
 
-def plan_batches(requests: Sequence[Request], max_batch: int) -> List[Batch]:
-    """Stable grouping: requests keep their arrival order inside a group; groups are emitted in order of their first request."""
+def plan_batches(requests: Sequence[Request], max_batch: int, length_bucket_s: Optional[float] = None) -> List[Batch]:
+    """Stable grouping: requests keep their arrival order inside a group; groups are emitted in order of their first request.
+    `length_bucket_s`: group lengths by bucket instead of exactly (see the module docstring); None keeps exact-length grouping."""
     if max_batch < 1:
         raise ValueError("max_batch must be >= 1")
+    if length_bucket_s is not None and not length_bucket_s > 0:
+        raise ValueError("length_bucket_s must be positive")
     groups: Dict[Tuple, List[int]] = collections.OrderedDict()
     for i, r in enumerate(requests):
-        groups.setdefault(r.group_key(), []).append(i)
+        groups.setdefault(r.group_key(length_bucket_s), []).append(i)
     out: List[Batch] = []
     for key, idx in groups.items():
         for s in range(0, len(idx), max_batch):
             part = idx[s:s + max_batch]
-            out.append(Batch(key, part, [requests[i] for i in part]))
+            reqs = [requests[i] for i in part]
+            pad = None if length_bucket_s is None else length_bucket_bin(reqs[0].length, length_bucket_s) * length_bucket_s
+            out.append(Batch(key, part, reqs, pad))
     return out
 
 
@@ -63,8 +80,9 @@ def batches_of_rank(batches: Sequence[Batch], world: int, rank: int) -> List[Bat
 
 
 class BatchingFrontEnd:
-    def __init__(self, backend, max_batch: int = 4, world: int = 1, rank: int = 0):
+    def __init__(self, backend, max_batch: int = 4, world: int = 1, rank: int = 0, length_bucket_s: Optional[float] = None):
         self.backend, self.max_batch, self.world, self.rank = backend, int(max_batch), int(world), int(rank)
+        self.length_bucket_s = length_bucket_s
         self._queue: List[Request] = []
 
     def submit(self, prompt: str, **kw) -> int:
@@ -78,8 +96,14 @@ class BatchingFrontEnd:
         seed_arg = seeds if any(s is not None for s in seeds) else None
         if seed_arg is not None and any(s is None for s in seeds):
             raise ValueError("a batch mixes seeded and unseeded requests: give every request a seed or none")
-        sr, wavs = self.backend.generate_audio([r.prompt for r in b.requests], length=r0.length, guidance_scale=r0.guidance_scale,
-                                               guidance_rescale=r0.guidance_rescale, ddim_steps=r0.ddim_steps, eta=r0.eta, random_seed=seed_arg)
+        kw = dict(guidance_scale=r0.guidance_scale, guidance_rescale=r0.guidance_rescale, ddim_steps=r0.ddim_steps, eta=r0.eta, random_seed=seed_arg)
+        if b.pad_length is None:
+            sr, wavs = self.backend.generate_audio([r.prompt for r in b.requests], length=r0.length, **kw)
+        else:
+            cap = getattr(self.backend, "max_length_s", None)
+            pad = b.pad_length if cap is None else min(b.pad_length, cap)
+            pad = max(pad, max(r.length for r in b.requests))
+            sr, wavs = self.backend.generate_audio([r.prompt for r in b.requests], length=[r.length for r in b.requests], pad_length=pad, **kw)
         if len(wavs) != len(b.requests):
             raise RuntimeError("backend returned a different number of waveforms than prompts")
         return sr, wavs
@@ -89,7 +113,7 @@ class BatchingFrontEnd:
         reqs = list(requests) if requests is not None else self._queue
         if requests is None:
             self._queue = []
-        for b in batches_of_rank(plan_batches(reqs, self.max_batch), self.world, self.rank):
+        for b in batches_of_rank(plan_batches(reqs, self.max_batch, self.length_bucket_s), self.world, self.rank):
             sr, wavs = self._run_batch(b)
             for t, w in zip(b.tickets, wavs):
                 yield t, sr, w

@@ -4,7 +4,9 @@ Differences from the reference loop, all additive:
   * batched prompts (the reference hard-codes batch 1, src/inference.py:67; SURVEY 0.8): prompt i gets its own
     torch.Generator(seed + i), so prompt 0 of a batch reproduces the reference's B=1 run with the same seed;
   * step-invariant work (context embedding, cross-attention K/V, timestep/AdaLN tables) is computed once per clip;
-  * CFG + rescale + DDIM update is one fused kernel (ezb_cfg_ddim_step).
+  * CFG + rescale + DDIM update is one fused kernel (ezb_cfg_ddim_step);
+  * clips of different lengths in one batch (`lengths=`): the batch is padded to `audio_frames` and every prompt's frames come out as
+    that prompt run alone at its own length computes them (same seed, same bits).
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -35,22 +37,46 @@ def encode_text(tokenizer, text_encoder, params, text_raw, neg_text, device):
     return text, mask, utext, umask
 
 
-def _ddim_step(model_out, latents, noise, B, Cc, L, gs, gr, coef):
+def _ddim_step(model_out, latents, noise, B, Cc, L, gs, gr, coef, lens=None):
     arr = (C.c_float * 5)(*coef)
     _lib.check(_lib.lib().ezb_cfg_ddim_step(latents.device.index, _lib.ptr(model_out), _lib.ptr(latents), _lib.ptr(noise), B, Cc, L, float(gs or 0.0), float(gr or 0.0),
-                                            arr, _lib.stream_ptr()))
+                                            arr, _lib.stream_ptr(), _lib.ptr(lens)))
+
+
+def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None):
+    """Validates per-prompt clip lengths (frames) against the batch size and the padded length L, on the host, before any device work."""
+    if gt is not None:
+        raise NotImplementedError("per-prompt lengths with inpainting (gt) are not supported")
+    if controlnet is not None:
+        raise NotImplementedError("per-prompt lengths with a ControlNet are not supported: its stem convolutions cross the clip ends")
+    lens = [int(v) for v in lengths]
+    if any(v != w for v, w in zip(lens, lengths)):
+        raise ValueError(f"lengths must be whole frame counts, got {list(lengths)}")
+    if len(lens) != B:
+        raise ValueError(f"lengths lists one length per prompt: got {len(lens)} for {B} prompts")
+    if any(v < 1 or v > L for v in lens):
+        raise ValueError(f"every length must lie in 1..{L} (the padded length), got {lens}")
+    return lens
 
 
 @torch.no_grad()
 def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, gt=None, gt_mask=None,
                    audio_frames=500, guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024,
                    controlnet=None, condition=None, conditioning_scale=1.0, init_noise=None, step_noise=None, device=None,
-                   use_graphs=True, paste_gt=True):
+                   use_graphs=True, paste_gt=True, lengths=None):
     """Denoising loop on cached text embeddings.  text (B,Lc,ctx) / text_mask (B,Lc); uncond_* (1 or B rows) when
     guidance_scale is truthy.  gt / gt_mask (B,C,L) for inpainting.  Returns the final latents (B,C,L) fp32 on device.
     `init_noise` / `step_noise` inject the RNG draws (parity tests); otherwise per-prompt generators are used.
     `paste_gt`: apply the final `pred[~gt_mask] = gt[~gt_mask]` here (standalone use); `inference()` passes False and pastes after
-    scale_shift_re like src/inference.py:102-105."""
+    scale_shift_re like src/inference.py:102-105.
+    `lengths`: one clip length (frames, 1..audio_frames) per prompt, or None.  The batch is padded to `audio_frames`; prompt b's initial
+    noise and per-step draws are made at its own shape (1, C, lengths[b]), so its frames < lengths[b] of the result equal a run of that
+    prompt alone at audio_frames = lengths[b] with the same seed (random_seed must then be per-prompt or None; injected noise is not
+    accepted).  Frames past a prompt's length are zero.  One captured graph serves every mix of lengths at the same padded length."""
+    if lengths is not None:
+        lengths = check_lengths(lengths, text.shape[0], int(audio_frames), gt, controlnet)
+        if init_noise is not None or step_noise is not None:
+            raise ValueError("lengths draws the noise per prompt: init_noise / step_noise cannot be injected")
     dev_index = unet._h.dev_index   # the loop runs where the denoiser's weights live
     if device is not None:
         d = torch.device(device)
@@ -61,7 +87,7 @@ def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, unc
     with torch.cuda.device(device):
         lat = _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
                                         guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, init_noise,
-                                        step_noise, device, use_graphs)
+                                        step_noise, device, use_graphs, lengths)
         if gt is not None and paste_gt:
             lat = torch.where(gt_mask.to(device).bool().expand_as(lat), lat, gt.to(device=device, dtype=lat.dtype))
         return lat
@@ -69,7 +95,7 @@ def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, unc
 
 def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
                               guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, init_noise, step_noise,
-                              device, use_graphs):
+                              device, use_graphs, lengths=None):
     B = text.shape[0]
     Cc = unet.cfg["out_chans"]
     L = int(audio_frames)
@@ -92,7 +118,12 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
             else:
                 g.seed()
             gens.append(g)
-        latents = torch.cat([torch.randn((1, Cc, L), generator=g, device=device) for g in gens], 0)
+        if lengths is None:
+            latents = torch.cat([torch.randn((1, Cc, L), generator=g, device=device) for g in gens], 0)
+        else:   # each prompt's draw at its own shape, placed into the zeroed padded batch
+            latents = torch.zeros((B, Cc, L), device=device)
+            for b, g in enumerate(gens):
+                latents[b, :, :lengths[b]] = torch.randn((1, Cc, lengths[b]), generator=g, device=device)[0]
     else:
         latents = init_noise.to(device=device, dtype=torch.float32).clone()
     latents = latents.contiguous()
@@ -133,7 +164,7 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
     # tensor maps), the schedule, the guidance constants, which ControlNet handle (its serial, not id(): ids are recycled) and the
     # library's option epoch (ezb_set_option changes kernel selection).
     nsteps = len(timesteps)
-    key = (B, Be, L, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), float(eta or 0.0),
+    key = (B, Be, L, lengths is not None, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), float(eta or 0.0),
            gt is not None, controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()))
     cache = unet.__dict__.setdefault("_loop_cache", {})
     st = cache.get(key) if use_graphs else None
@@ -143,7 +174,10 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
                   out=torch.empty(Be, Cc, L, device=device, dtype=torch.float32),
                   noise=torch.empty(nsteps, B, Cc, L, device=device, dtype=torch.float32) if (eta and eta > 0) else None,
                   gt=None if gt_c is None else torch.empty_like(gt_c), m8=None if m8 is None else torch.empty_like(m8),
-                  cond=None, skips=None, graph=None, launches=0)
+                  cond=None, skips=None, graph=None, launches=0,
+                  lens=torch.empty(Be, device=device, dtype=torch.int32) if lengths is not None else None)   # [lengths | lengths] under CFG
+        if st["noise"] is not None and lengths is not None:
+            st["noise"].zero_()   # the padded frames are never read; keep them finite
         if controlnet is not None:
             st["cond"] = torch.empty_like(cond_c)
             st["skips"] = skips
@@ -157,14 +191,20 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         st["m8"].copy_(m8)
     if controlnet is not None:
         st["cond"].copy_(cond_c)
+    lens = st["lens"]
+    if lens is not None:   # read by the kernels when they run: a replayed graph follows the new lengths
+        lens.copy_(torch.tensor(lengths * (Be // B), dtype=torch.int32))
     lat, x_in, out, noise_all = st["lat"], st["x_in"], st["out"], st["noise"]
     if noise_all is not None:  # RNG stays in PyTorch, outside the graph: step i, prompt b draws (1, C, L) from prompt b's generator, in step order
         for i in range(nsteps):
             if step_noise is not None:
                 noise_all[i].copy_(step_noise[i])
-            else:
+            elif lengths is None:
                 for b, g in enumerate(gens):
                     noise_all[i, b:b + 1].normal_(generator=g)
+            else:   # the draw a solo run makes: a contiguous (1, C, lengths[b]) tensor
+                for b, g in enumerate(gens):
+                    noise_all[i, b, :, :lengths[b]] = torch.empty((1, Cc, lengths[b]), device=device).normal_(generator=g)[0]
 
     def one_step(i, t):
         if use_cfg:
@@ -176,9 +216,10 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         sk = None
         if controlnet is not None:
             sk = controlnet.forward_step(xi, i, st["cond"], conditioning_scale, gt=st["gt"], gt_mask_u8=st["m8"], outs=st["skips"])
-        unet.forward_step(xi, i, gt=st["gt"], gt_mask_u8=st["m8"], controlnet_skips=sk, out=out)
+        unet.forward_step(xi, i, gt=st["gt"], gt_mask_u8=st["m8"], controlnet_skips=sk, out=out, lengths=lens)
         coef = noise_scheduler.step_coefficients(t, float(eta or 0.0))
-        _ddim_step(out, lat, None if noise_all is None else noise_all[i], B, Cc, L, guidance_scale if use_cfg else 0.0, guidance_rescale, coef)
+        _ddim_step(out, lat, None if noise_all is None else noise_all[i], B, Cc, L, guidance_scale if use_cfg else 0.0, guidance_rescale, coef,
+                   None if lens is None else lens[:B])
 
     L_ = _lib.lib()
     if use_graphs and st["graph"] is not None:
@@ -203,8 +244,13 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
 @torch.no_grad()
 def inference(autoencoder, unet, gt, gt_mask, tokenizer, text_encoder, params, noise_scheduler, text_raw, neg_text=None,
               audio_frames=500, guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device="cuda",
-              text_embeds=None, controlnet=None, condition=None, conditioning_scale=1.0):
-    """Signature of src/inference.py:26-37 (+ keyword-only extensions).  Returns the waveform tensor (B,1,480*L)."""
+              text_embeds=None, controlnet=None, condition=None, conditioning_scale=1.0, lengths=None):
+    """Signature of src/inference.py:26-37 (+ keyword-only extensions).  Returns the waveform tensor (B,1,480*L).
+    With `lengths` (one clip length in frames per prompt, batch padded to audio_frames; see sample_latents) it returns a list of B
+    waveforms (1, 480*lengths[b]): the VAE decodes each group of equal lengths at that length, because its receptive field crosses the
+    clip end."""
+    if lengths is not None:
+        lengths = check_lengths(lengths, len(text_raw) if text_embeds is None else text_embeds[0].shape[0], int(audio_frames), gt, controlnet)
     if neg_text is None:
         neg_text = [""]
     if text_embeds is not None:
@@ -214,8 +260,17 @@ def inference(autoencoder, unet, gt, gt_mask, tokenizer, text_encoder, params, n
     else:  # src/inference.py:51-53
         raise ValueError("either tokenizer/text_encoder or text_embeds is required (the denoiser is text-conditioned)")
     latents = sample_latents(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
-                             guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, device=device, paste_gt=False)
+                             guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, device=device, paste_gt=False,
+                             lengths=lengths)
     pred = scale_shift_re(latents, params["autoencoder"]["scale"], params["autoencoder"]["shift"])
+    if lengths is not None:
+        wavs = [None] * len(lengths)
+        for n in sorted(set(lengths)):
+            idx = [b for b, v in enumerate(lengths) if v == n]
+            w = autoencoder(embedding=pred[idx, :, :n].contiguous())
+            for j, b in enumerate(idx):
+                wavs[b] = w[j]
+        return wavs
     if gt is not None:  # src/inference.py:104-105: pred[~gt_mask] = gt[~gt_mask], with the raw gt, after the rescale
         pred = torch.where(gt_mask.to(pred.device).bool().expand_as(pred), pred, gt.to(device=pred.device, dtype=pred.dtype))
     return autoencoder(embedding=pred)

@@ -39,7 +39,7 @@ typedef struct {
   int32_t precision;          /* 0: bf16 operands / fp32 accumulate; 1: bf16x3 split operands (fp32-grade parity mode) */
 } ezb_dit_desc;
 
-int ezb_version(void);
+int ezb_version(void); /* 2: ezb_dit_forward / ezb_cfg_ddim_step take per-sample lengths */
 const char* ezb_last_error(void);
 
 /* --- model lifetime / weights: replaces MaskDiT(...).load_state_dict(torch.load(ckpt)['model']) (api/ezaudio.py:83-85) */
@@ -64,9 +64,14 @@ int ezb_dit_set_timesteps(ezb_dit* h, const int64_t* timesteps_host, int n, void
  * NULL: 1 = position is regenerated (gt replaced by mask_embed there, mask channel = 1; conditioners.py:150-153,176);
  * t_index_host[Be]: index into the table of ezb_dit_set_timesteps per sample (NULL = all use `t_index_all`);
  * controlnet_skips: NULL or depth/2 device pointers (Be,L,D) fp32 in in-block order (udit.py:345-348);
- * out (Be,C,L) fp32. */
+ * out (Be,C,L) fp32.
+ * lens: NULL (every sample is L frames long) or a DEVICE int32 [Be]: sample b is a clip of lens[b] frames padded to L.  Its frames
+ * < lens[b] come out as a forward of that clip alone at L = lens[b] computes them, whatever the padded frames hold (NaN included); its
+ * frames >= lens[b] of `out` are not written.  Kernels read the lengths when they run (a captured graph replays with new lengths) and
+ * clamp them to [1, L]; validating them is the caller's job.  Not combined with gt / gt_mask or ControlNet skips by the Python layer. */
 int ezb_dit_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_host,
-                    int t_index_all, const float* const* controlnet_skips, float* out, int Be, int L, void* stream);
+                    int t_index_all, const float* const* controlnet_skips, float* out, int Be, int L, void* stream,
+                    const int32_t* lens);
 /* DiTControlNet.forward (controlnet.py:252-315): condition (Be,1,2L) fp32; writes depth/2 skips (Be,L,D) fp32, already
  * multiplied by conditioning_scale, into skips_out[i]. */
 int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_host,
@@ -76,9 +81,12 @@ int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, const ui
 /* --- fused classifier-free guidance + rescale + DDIM update (src/inference.py:12-23,88-100; diffusers DDIMScheduler.step
  * restated, SURVEY Appendix B).  model_out holds B text rows followed by B uncond rows when guidance_scale != 0, else B
  * rows.  coef = {sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-sigma^2), sigma}; noise (B,C,L) may be NULL when
- * sigma == 0.  latents updated in place.  `device`: the CUDA device the pointers live on (the call makes it current). */
+ * sigma == 0.  latents updated in place.  `device`: the CUDA device the pointers live on (the call makes it current).
+ * lens: NULL or a DEVICE int32 [B] (clamped to [1, L]): sample b covers frames < lens[b] of every channel.  The rescale statistics and
+ * the update run over exactly those C * lens[b] elements, in the order of a call on that clip alone (bit-identical to it); the padded
+ * frames of latents are left untouched. */
 int ezb_cfg_ddim_step(int device, const float* model_out, float* latents, const float* noise, int B, int C, int L, float guidance_scale,
-                      float guidance_rescale, const float* coef5_host, void* stream);
+                      float guidance_rescale, const float* coef5_host, void* stream, const int32_t* lens);
 
 /* --- VAE decoder: OobleckDecoder.forward (stable_vae/models/autoencoders.py:149-190) behind
  * Autoencoder(embedding=z) (src/modules/autoencoder_wrapper.py:74-77). */
@@ -199,6 +207,10 @@ int ezb_test_mlp(int device, const void* A_bf16, const float* W1_f32, const floa
    generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
                        int B, int H, int Lq, int Lk, int dh, int impl, void* stream);
+/* Self-attention (Lq = Lk = L, no key mask) of a padded batch, as ezb_test_attention with the same impl codes: lens DEVICE int32 [B],
+   sample b attends over its first lens[b] tokens; output rows >= lens[b] are written as zeros. */
+int ezb_test_attention_lens(int device, const void* q, const void* k, const void* vt, const int32_t* lens, void* out_bf16, int B, int H,
+                            int L, int dh, int impl, void* stream);
 
 /* runtime switches for A/B measurements and profiling (csrc/host.cuh, csrc/ezb.cu list them): e.g. "pair_gemm" (1 = 2-CTA cluster tiles
    sharing the weight tile, default), "attn6" / "attn7" / "attn_res" (attention variant), "ksub2", "ln_variant", "skip" (profiling: kernel classes not launched).  Products never need to call this. */
