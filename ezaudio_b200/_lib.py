@@ -49,6 +49,12 @@ class TestHeadsArgs(C.Structure):
                 ("fold_v", C.c_void_p), ("variant", C.c_int32)]
 
 
+class TestVaeArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "precision", "B", "T", "cin", "cout", "taps", "dil", "stride")] + \
+               [(n, C.c_void_p) for n in ("weight_v", "weight_g", "bias", "alpha", "beta", "x", "resid", "noise", "raw", "act", "out",
+                                          "w_packed")]
+
+
 _lib = None
 
 _VP, _I, _F = C.c_void_p, C.c_int, C.c_float
@@ -92,6 +98,7 @@ _SIGS = {
     "ezb_test_attention_lens": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_test_heads": ([_I, _VP, _VP, C.POINTER(TestHeadsArgs), _VP], _I),
     "ezb_test_mlp": ([_I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP], _I),
+    "ezb_test_vae": ([_I, C.POINTER(TestVaeArgs), _VP], _I),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -222,6 +222,86 @@ __attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* 
   return rc;
 }
 
+namespace {
+int test_vae_run(Device& dev, cudaStream_t st, const ezb_test_vae_args* a, int kmul, float* scratch, size_t part, __nv_bfloat16** wp) {
+  float *norms = scratch, *wfold = scratch + part;
+  const VaeSnake sn{scratch + 2 * part, scratch + 3 * part};
+  const VaeSnake* snake = a->act ? &sn : nullptr;
+  const int kind = a->kind, C = kind == 3 || kind == 6 ? a->cin : a->cout;
+  if (a->act && kind != 6) EZB_TRY(vae_snake_prep(st, a->alpha, a->beta, sn, a->cout));
+  if (kind <= 2) {
+    VaeConv c = kind == 0 ? vae_conv_geom(a->cin, a->cout, a->taps, a->dil, kmul)
+              : kind == 1 ? vae_convT_geom(a->cin, a->cout, a->stride, kmul) : vae_conv_strided_geom(a->cin, a->cout, a->stride, kmul);
+    c.bias = a->bias;
+    const size_t bytes = c.w_elems() * sizeof(__nv_bfloat16);
+    EZB_CUDA(cudaMallocAsync(wp, bytes, st));
+    EZB_CUDA(cudaMemsetAsync(*wp, 0, bytes, st));   // the pad columns, as Vae::alloc zeroes them
+    c.w = *wp;
+    EZB_TRY(kind == 1 ? vae_pack_convT_w(st, c, a->weight_v, a->weight_g, norms, kmul) : vae_pack_conv_w(st, c, a->weight_v, a->weight_g, norms, kmul));
+    EZB_TRY(vae_conv(dev, st, c, kmul, static_cast<const __nv_bfloat16*>(a->x), a->B, a->T, a->resid, a->raw,
+                     static_cast<__nv_bfloat16*>(a->act), snake));
+    if (a->w_packed) EZB_CUDA(cudaMemcpyAsync(a->w_packed, c.w, bytes, cudaMemcpyDeviceToDevice, st));
+    return EZB_OK;
+  }
+  const float* x = static_cast<const float*>(a->x);
+  if (kind == 3) {
+    EZB_TRY(vae_fold_wave_w(st, a->weight_v, a->weight_g, norms, wfold, C));
+    EZB_TRY(vae_wave_out(st, static_cast<const __nv_bfloat16*>(a->x), wfold, a->out, a->B, C, a->T, kmul));
+  } else if (kind == 4) {
+    EZB_TRY(vae_fold_conv_in_w(st, a->weight_v, a->weight_g, norms, wfold, C));
+    EZB_TRY(vae_enc_conv_in(st, x, wfold, a->bias, sn, a->raw, static_cast<__nv_bfloat16*>(a->act), a->B, C, a->T, kmul));
+  } else if (kind == 5) {
+    return vae_sample(st, x, a->noise, a->out, a->B, C, a->T);
+  } else {
+    return vae_latent_pack(st, x, static_cast<__nv_bfloat16*>(a->act), a->B, C, a->T, kmul);
+  }
+  if (a->w_packed) EZB_CUDA(cudaMemcpyAsync(a->w_packed, wfold, (size_t)7 * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return EZB_OK;
+}
+}  // namespace
+
+__attribute__((visibility("default"))) int ezb_test_vae(int device, const ezb_test_vae_args* a, void* stream) {
+  if (!a) return fail(EZB_ERR_ARG, "ezb_test_vae: null arguments");
+  const int kind = a->kind, B = a->B, T = a->T, cin = a->cin, cout = a->cout, s = a->stride;
+  if (kind < 0 || kind > 6) return fail(EZB_ERR_ARG, "ezb_test_vae: kind %d", kind);
+  if (a->precision != 0 && a->precision != 1) return fail(EZB_ERR_ARG, "ezb_test_vae: precision %d", a->precision);
+  if (!a->x) return fail(EZB_ERR_ARG, "ezb_test_vae: null input");
+  const long long rows = (long long)B * T * (kind == 1 || kind == 2 ? (s > 1 ? s : 1) : 1);
+  if (B < 1 || T < 1 || rows > (1 << 26)) return fail(EZB_ERR_SHAPE, "ezb_test_vae: B %d T %d", B, T);
+  if (kind <= 4 && kind != 3 && (!a->weight_v || !a->weight_g || !a->bias)) return fail(EZB_ERR_ARG, "ezb_test_vae: kind %d needs weight_v, weight_g and bias", kind);
+  if (a->act && kind != 6 && (!a->alpha || !a->beta)) return fail(EZB_ERR_ARG, "ezb_test_vae: an activated output needs the snake's alpha and beta");
+  if (kind <= 2) {
+    if (cin < 8 || cin % 8 || cout < 8 || cout % 8 || cin > 8192 || cout > 8192)
+      return fail(EZB_ERR_SHAPE, "ezb_test_vae: cin %d cout %d (multiples of 8, at most 8192)", cin, cout);
+    if (!a->raw && !a->act) return fail(EZB_ERR_ARG, "ezb_test_vae: conv without an output");
+    if (kind == 0 && (a->taps < 1 || a->taps % 2 == 0 || a->dil < 1)) return fail(EZB_ERR_SHAPE, "ezb_test_vae: conv taps %d dilation %d (odd taps)", a->taps, a->dil);
+    if (kind == 1 && (s < 2 || s % 2)) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_vae: conv-transpose stride %d (even, >= 2)", s);
+    if (kind == 2 && s < 2) return fail(EZB_ERR_SHAPE, "ezb_test_vae: strided conv stride %d (>= 2)", s);
+  } else if (kind == 3) {
+    if (cin < 4 || cin % 4 || !a->weight_v || !a->weight_g || !a->out) return fail(EZB_ERR_SHAPE, "ezb_test_vae: wave out over %d channels (multiple of 4) needs weights and out", cin);
+  } else if (kind == 4) {
+    if (cout < 1 || !a->raw || !a->act) return fail(EZB_ERR_ARG, "ezb_test_vae: the stem over %d channels writes raw and act", cout);
+  } else if (kind == 5) {
+    if (cout < 1 || !a->out) return fail(EZB_ERR_ARG, "ezb_test_vae: sample over %d channels needs out", cout);
+  } else if (cin < 1 || !a->act) {
+    return fail(EZB_ERR_ARG, "ezb_test_vae: latent pack over %d channels needs act", cin);
+  }
+  const int C = kind <= 2 ? (cin > cout ? cin : cout) : (kind == 3 || kind == 6 ? cin : cout);
+  if (C > 8192) return fail(EZB_ERR_SHAPE, "ezb_test_vae: %d channels (at most 8192)", C);
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  dev.tmaps.trim();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t part = ((size_t)7 * C + 63) / 64 * 64;   // norms, folded weights, snake a, snake 1/b
+  float* scratch = nullptr;
+  __nv_bfloat16* wp = nullptr;
+  EZB_CUDA(cudaMallocAsync(&scratch, 4 * part * sizeof(float), st));
+  const int rc = test_vae_run(dev, st, a, a->precision == 1 ? 3 : 1, scratch, part, &wp);
+  EZB_CUDA(cudaFreeAsync(scratch, st));
+  if (wp) EZB_CUDA(cudaFreeAsync(wp, st));
+  return rc;
+}
+
 
 #define EZB_API __attribute__((visibility("default")))
 #define ST(s) reinterpret_cast<cudaStream_t>(s)

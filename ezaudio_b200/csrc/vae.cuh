@@ -191,10 +191,141 @@ __global__ void vae_sample_kernel(const float* __restrict__ enc, const float* __
 
 struct VaeConv {  // one packed conv / conv-transpose
   __nv_bfloat16* w = nullptr;
-  float* bias = nullptr;
+  const float* bias = nullptr;
   int cin = 0, cout = 0, taps = 0, center = 0, dil = 1, cin_pad = 0, N = 0, stride = 0;
+  size_t w_elems() const { return (size_t)N * taps * cin_pad; }
 };
 struct VaeSnake { float *a = nullptr, *binv = nullptr; };
+
+// Geometry of the three conv shapes (w and bias left to the caller).  Conv1d(cin -> cout, K taps, dilation, padding dil * (K - 1) / 2):
+inline VaeConv vae_conv_geom(int cin, int cout, int K, int dil, int kmul) {
+  VaeConv c;
+  c.cin = cin; c.cout = cout; c.N = cout; c.taps = K; c.center = (K - 1) / 2; c.dil = dil;
+  c.cin_pad = (kmul * cin + 63) / 64 * 64;
+  return c;
+}
+// ConvTranspose1d(cin -> cout, k = 2s, stride s, padding s / 2) (DecoderBlock): three taps over the input, N = s * cout (one column block per phase)
+inline VaeConv vae_convT_geom(int cin, int cout, int s, int kmul) {
+  VaeConv c = vae_conv_geom(cin, cout, 3, 1, kmul);
+  c.N = s * cout; c.stride = s;
+  return c;
+}
+// strided Conv1d(cin -> cout, k = 2s, stride s, pad ceil(s/2)) (EncoderBlock, autoencoders.py:76-77): same packing as a conv
+inline VaeConv vae_conv_strided_geom(int cin, int cout, int s, int kmul) {
+  VaeConv c = vae_conv_geom(cin, cout, 2 * s, 1, kmul);
+  c.stride = s;
+  c.center = (s + 1) / 2;  // padding
+  return c;
+}
+
+// Weight-norm folding and packing from the reference layouts into caller-provided buffers.  `norms` is scratch of one float per dim-0 row.
+// Conv1d / strided conv: v [cout, cin, taps], g [cout] -> c.w
+inline int vae_pack_conv_w(cudaStream_t st, const VaeConv& c, const float* v, const float* g, float* norms, int kmul) {
+  ++launch_counter();
+  wn_norm_kernel<<<c.cout, 256, 0, st>>>(v, c.cin * c.taps, norms);
+  const size_t n = (size_t)c.cout * c.taps * c.cin;
+  ++launch_counter();
+  pack_conv_w_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(v, g, norms, c.w, c.cout, c.cin, c.taps, c.cin_pad, kmul);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// ConvTranspose1d: v [cin, cout, 2s], g [cin] -> c.w
+inline int vae_pack_convT_w(cudaStream_t st, const VaeConv& c, const float* v, const float* g, float* norms, int kmul) {
+  const int s = c.stride;
+  ++launch_counter();
+  wn_norm_kernel<<<c.cin, 256, 0, st>>>(v, c.cout * 2 * s, norms);
+  const size_t n = (size_t)c.N * 3 * c.cin;
+  ++launch_counter();
+  pack_convT_w_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(v, g, norms, c.w, c.cin, c.cout, s, (s + 1) / 2, c.cin_pad, kmul);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// SnakeBeta(alpha, beta) -> the epilogue's exp(alpha) and 1 / (exp(beta) + 1e-9)
+inline int vae_snake_prep(cudaStream_t st, const float* alpha, const float* beta, const VaeSnake& s, int C) {
+  ++launch_counter();
+  snake_prep_kernel<<<(C + 255) / 256, 256, 0, st>>>(alpha, beta, s.a, s.binv, C);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// the decoder's last conv, v [1, C, 7], g [1] -> w [7][C]
+inline int vae_fold_wave_w(cudaStream_t st, const float* v, const float* g, float* norms, float* w, int C) {
+  ++launch_counter();
+  wn_norm_kernel<<<1, 256, 0, st>>>(v, C * 7, norms);
+  ++launch_counter();
+  fold_wave_w_kernel<<<(7 * C + 255) / 256, 256, 0, st>>>(v, g, norms, w, C);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// the encoder stem, v [C, 1, 7], g [C] -> w [7][C]
+inline int vae_fold_conv_in_w(cudaStream_t st, const float* v, const float* g, float* norms, float* w, int C) {
+  ++launch_counter();
+  wn_norm_kernel<<<C, 256, 0, st>>>(v, 7, norms);
+  ++launch_counter();
+  fold_conv_in_w_kernel<<<(7 * C + 255) / 256, 256, 0, st>>>(v, g, norms, w, C);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+
+// One implicit-GEMM conv: A [B, T_in, kmul*cin] -> raw_out fp32 [B*T, N] (pre-activation, + resid_in when given) and act_out bf16
+// [B, T * phases, kmul*cout] (SnakeBeta(snake) of it, [hi | lo | hi] in bf16x3).  T: input rows, except for a strided conv (output rows,
+// the input has T * stride).  resid_in may alias raw_out.
+inline int vae_conv(Device& dev, cudaStream_t st, const VaeConv& c, int kmul, const __nv_bfloat16* A, int B, int T, const float* resid_in,
+                    float* raw_out, __nv_bfloat16* act_out, const VaeSnake* snake) {
+  EpiLinearParams e;
+  memset(&e, 0, sizeof e);
+  e.bias = c.bias;
+  e.bias_mod = c.cout;
+  e.resid = resid_in; e.ldr = c.N;
+  e.out_f32 = raw_out; e.ld32 = c.N;
+  e.out_bf16 = act_out;
+  const int phases = c.N / c.cout;
+  e.ld16 = phases * kmul * c.cout;
+  e.split_stride = kmul == 3 ? c.cout : 0;
+  e.phase_cols = phases > 1 ? c.cout : 0;
+  e.phase_ld16 = kmul * c.cout;
+  if (snake) { e.act = ACT_SNAKE; e.act_a = snake->a; e.act_b = snake->binv; }
+  ConvAddr ca;
+  ca.taps = c.taps; ca.center = c.center; ca.dilation = c.dil; ca.cin_pad = c.cin_pad; ca.T = T; ca.B = B;
+  if (c.stride > 1 && c.N == c.cout) { ca.stride = c.stride; ca.pad = c.center; }  // strided conv (T = output length); conv-transpose has N = s*cout
+  const int ld = c.taps * c.cin_pad;
+  return gemm<128, EpiLinear<128>>(dev, st, A, kmul * c.cin, c.w, ld, B * T, c.N, kmul * c.cin, e, &ca);
+}
+
+// z (B, C, L) fp32 -> act [B, L, kmul*C]
+inline int vae_latent_pack(cudaStream_t st, const float* z, __nv_bfloat16* act, int B, int C, int L, int kmul) {
+  dim3 grid((L + 31) / 32, (C + 31) / 32, B), blk(32, 8);
+  ++launch_counter();
+  latent_pack_kernel<<<grid, blk, 0, st>>>(z, act, C, L, kmul);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// act [B, T, kmul*C] -> wav [B, T], w folded [7][C]
+inline int vae_wave_out(cudaStream_t st, const __nv_bfloat16* act, const float* w, float* wav, int B, int C, int T, int kmul) {
+  if (C % 4) return fail(EZB_ERR_UNSUPPORTED, "wave_out: %d channels in the last stage (multiple of 4 expected)", C);
+  dim3 g2((T + 127) / 128, B);
+  ++launch_counter();
+  if (kmul == 3) wave_out_kernel<3><<<g2, 128, 0, st>>>(act, w, wav, C, T);
+  else wave_out_kernel<1><<<g2, 128, 0, st>>>(act, w, wav, C, T);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// audio [B, T] -> raw [B, T, C] fp32 and act = SnakeBeta(snake) [B, T, kmul*C], w folded [7][C]
+inline int vae_enc_conv_in(cudaStream_t st, const float* audio, const float* w, const float* bias, const VaeSnake& snake, float* raw,
+                           __nv_bfloat16* act, int B, int C, int T, int kmul) {
+  dim3 grid((unsigned)(((size_t)T * C + 255) / 256), B);
+  ++launch_counter();
+  enc_conv_in_kernel<<<grid, 256, 0, st>>>(audio, w, bias, snake.a, snake.binv, raw, act, C, T, kmul);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// enc [B*L, 2*Cz] (mean | scale) -> z (B, Cz, L)
+inline int vae_sample(cudaStream_t st, const float* enc, const float* noise, float* z, int B, int Cz, int L) {
+  dim3 g2((unsigned)(((size_t)Cz * L + 255) / 256), B);
+  ++launch_counter();
+  vae_sample_kernel<<<g2, 256, 0, st>>>(enc, noise, z, Cz, L);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
 
 struct Vae {
   ezb_vae_desc d;
@@ -242,6 +373,10 @@ struct Vae {
     kmul = d.precision == 1 ? 3 : 1;
     nst = d.n_stages;
     if (nst < 1 || nst > 8 || d.out_channels != 1 || d.latent_dim % 32 || d.channels % 8) return fail(EZB_ERR_UNSUPPORTED, "vae config");
+    // ConvTranspose1d(k = 2s, stride s, padding ceil(s/2)) makes T*s - 1 frames for odd s; the decoder is built for T*s
+    for (int i = 0; i < nst; ++i)
+      if (d.strides[i] < 2 || d.strides[i] % 2)
+        return fail(EZB_ERR_UNSUPPORTED, "vae decoder stage %d: stride %d (an even stride >= 2 expected)", nst - i, d.strides[i]);
     std::vector<int> mults(1, 1);
     for (int i = 0; i < nst; ++i) mults.push_back(d.c_mults[i]);
     for (int i = nst; i >= 1; --i) { cin_s.push_back(mults[i] * d.channels); cout_s.push_back(mults[i - 1] * d.channels); stride_s.push_back(d.strides[i - 1]); }
@@ -301,46 +436,26 @@ struct Vae {
     *out = it->second.first;
     return EZB_OK;
   }
-  int pack_conv(const std::string& k, int cout, int cin, int K, int dil, bool bias, VaeConv* c, cudaStream_t st) {
+  // conv geometry c (from vae_*_geom) + the checkpoint entries of key k -> packed weights of this handle
+  int pack_conv(const std::string& k, bool bias, VaeConv* c, cudaStream_t st) {
     float *g, *v, *b = nullptr, *norms;
-    EZB_TRY(need(k + ".weight_g", {cout, 1, 1}, &g));
-    EZB_TRY(need(k + ".weight_v", {cout, cin, K}, &v));
-    if (bias) EZB_TRY(need(k + ".bias", {cout}, &b));
-    EZB_TRY(alloc(&norms, (size_t)cout));
-    ++launch_counter();
-    wn_norm_kernel<<<cout, 256, 0, st>>>(v, cin * K, norms);
-    c->cin = cin; c->cout = cout; c->N = cout; c->taps = K; c->center = (K - 1) / 2; c->dil = dil; c->bias = b;
-    c->cin_pad = (kmul * cin + 63) / 64 * 64;
-    EZB_TRY(alloc(&c->w, (size_t)cout * K * c->cin_pad));
-    const size_t n = (size_t)cout * K * cin;
-    ++launch_counter();
-    pack_conv_w_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(v, g, norms, c->w, cout, cin, K, c->cin_pad, kmul);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    EZB_TRY(need(k + ".weight_g", {c->cout, 1, 1}, &g));
+    EZB_TRY(need(k + ".weight_v", {c->cout, c->cin, c->taps}, &v));
+    if (bias) EZB_TRY(need(k + ".bias", {c->cout}, &b));
+    EZB_TRY(alloc(&norms, (size_t)c->cout));
+    c->bias = b;
+    EZB_TRY(alloc(&c->w, c->w_elems()));
+    return vae_pack_conv_w(st, *c, v, g, norms, kmul);
   }
-  int pack_convT(const std::string& k, int cin, int cout, int s, VaeConv* c, cudaStream_t st) {
+  int pack_convT(const std::string& k, VaeConv* c, cudaStream_t st) {
     float *g, *v, *b, *norms;
-    EZB_TRY(need(k + ".weight_g", {cin, 1, 1}, &g));
-    EZB_TRY(need(k + ".weight_v", {cin, cout, 2 * s}, &v));
-    EZB_TRY(need(k + ".bias", {cout}, &b));
-    EZB_TRY(alloc(&norms, (size_t)cin));
-    ++launch_counter();
-    wn_norm_kernel<<<cin, 256, 0, st>>>(v, cout * 2 * s, norms);
-    c->cin = cin; c->cout = cout; c->N = s * cout; c->taps = 3; c->center = 1; c->dil = 1; c->bias = b; c->stride = s;
-    c->cin_pad = (kmul * cin + 63) / 64 * 64;
-    EZB_TRY(alloc(&c->w, (size_t)c->N * 3 * c->cin_pad));
-    const size_t n = (size_t)c->N * 3 * cin;
-    ++launch_counter();
-    pack_convT_w_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(v, g, norms, c->w, cin, cout, s, (s + 1) / 2, c->cin_pad, kmul);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
-  }
-  // strided Conv1d(cin -> cout, k = 2s, stride s, pad ceil(s/2)) (EncoderBlock, autoencoders.py:76-77): same packing as a conv
-  int pack_conv_strided(const std::string& k, int cout, int cin, int s_, VaeConv* c, cudaStream_t st) {
-    EZB_TRY(pack_conv(k, cout, cin, 2 * s_, 1, true, c, st));
-    c->stride = s_;
-    c->center = (s_ + 1) / 2;  // padding
-    return EZB_OK;
+    EZB_TRY(need(k + ".weight_g", {c->cin, 1, 1}, &g));
+    EZB_TRY(need(k + ".weight_v", {c->cin, c->cout, 2 * c->stride}, &v));
+    EZB_TRY(need(k + ".bias", {c->cout}, &b));
+    EZB_TRY(alloc(&norms, (size_t)c->cin));
+    c->bias = b;
+    EZB_TRY(alloc(&c->w, c->w_elems()));
+    return vae_pack_convT_w(st, *c, v, g, norms, kmul);
   }
   int finalize_encoder(cudaStream_t st) {
     const std::string e = "encoder.layers.";
@@ -349,11 +464,7 @@ struct Vae {
       float *g, *v, *b, *norms;
       EZB_TRY(need(e + "0.weight_g", {C0, 1, 1}, &g)); EZB_TRY(need(e + "0.weight_v", {C0, 1, 7}, &v)); EZB_TRY(need(e + "0.bias", {C0}, &b));
       EZB_TRY(alloc(&norms, (size_t)C0)); EZB_TRY(alloc(&e_in_w, (size_t)7 * C0));
-      ++launch_counter();
-      wn_norm_kernel<<<C0, 256, 0, st>>>(v, 7, norms);
-      ++launch_counter();
-      fold_conv_in_w_kernel<<<(7 * C0 + 255) / 256, 256, 0, st>>>(v, g, norms, e_in_w, C0);
-      EZB_CUDA(cudaGetLastError());
+      EZB_TRY(vae_fold_conv_in_w(st, v, g, norms, e_in_w, C0));
       e_in_b = b;
     }
     e_res7.resize(3 * nst); e_res1.resize(3 * nst); e_res_s0.resize(3 * nst); e_res_s2.resize(3 * nst); e_down.resize(nst); e_down_snake.resize(nst);
@@ -363,41 +474,46 @@ struct Vae {
       for (int u = 0; u < 3; ++u) {
         const std::string ru = q + std::to_string(u) + ".layers.";
         EZB_TRY(prep_snake(ru + "0", e_cin[j], &e_res_s0[3 * j + u], st));
-        EZB_TRY(pack_conv(ru + "1", e_cin[j], e_cin[j], 7, dils[u], true, &e_res7[3 * j + u], st));
+        e_res7[3 * j + u] = vae_conv_geom(e_cin[j], e_cin[j], 7, dils[u], kmul);
+        EZB_TRY(pack_conv(ru + "1", true, &e_res7[3 * j + u], st));
         EZB_TRY(prep_snake(ru + "2", e_cin[j], &e_res_s2[3 * j + u], st));
-        EZB_TRY(pack_conv(ru + "3", e_cin[j], e_cin[j], 1, 1, true, &e_res1[3 * j + u], st));
+        e_res1[3 * j + u] = vae_conv_geom(e_cin[j], e_cin[j], 1, 1, kmul);
+        EZB_TRY(pack_conv(ru + "3", true, &e_res1[3 * j + u], st));
       }
       EZB_TRY(prep_snake(q + "3", e_cin[j], &e_down_snake[j], st));
-      EZB_TRY(pack_conv_strided(q + "4", e_cout[j], e_cin[j], e_stride[j], &e_down[j], st));
+      e_down[j] = vae_conv_strided_geom(e_cin[j], e_cout[j], e_stride[j], kmul);
+      EZB_TRY(pack_conv(q + "4", true, &e_down[j], st));
     }
     EZB_TRY(prep_snake(e + std::to_string(nst + 1), e_cout[nst - 1], &e_out_snake, st));
-    EZB_TRY(pack_conv(e + std::to_string(nst + 2), d.enc_latent_dim, e_cout[nst - 1], 3, 1, true, &e_out, st));
+    e_out = vae_conv_geom(e_cout[nst - 1], d.enc_latent_dim, 3, 1, kmul);
+    EZB_TRY(pack_conv(e + std::to_string(nst + 2), true, &e_out, st));
     return EZB_OK;
   }
   int prep_snake(const std::string& k, int C, VaeSnake* s, cudaStream_t st) {
     float *al, *be;
     EZB_TRY(need(k + ".alpha", {C}, &al)); EZB_TRY(need(k + ".beta", {C}, &be));
     EZB_TRY(alloc(&s->a, (size_t)C)); EZB_TRY(alloc(&s->binv, (size_t)C));
-    ++launch_counter();
-    snake_prep_kernel<<<(C + 255) / 256, 256, 0, st>>>(al, be, s->a, s->binv, C);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    return vae_snake_prep(st, al, be, *s, C);
   }
   int finalize(cudaStream_t st) {
     const std::string p = "decoder.layers.";
-    EZB_TRY(pack_conv(p + "0", cin_s[0], d.latent_dim, 7, 1, true, &conv_in, st));
+    conv_in = vae_conv_geom(d.latent_dim, cin_s[0], 7, 1, kmul);
+    EZB_TRY(pack_conv(p + "0", true, &conv_in, st));
     up.resize(nst); up_snake.resize(nst); res7.resize(3 * nst); res1.resize(3 * nst); res_s0.resize(3 * nst); res_s2.resize(3 * nst);
     const int dils[3] = {1, 3, 9};
     for (int j = 0; j < nst; ++j) {
       const std::string q = p + std::to_string(j + 1) + ".layers.";
       EZB_TRY(prep_snake(q + "0", cin_s[j], &up_snake[j], st));
-      EZB_TRY(pack_convT(q + "1", cin_s[j], cout_s[j], stride_s[j], &up[j], st));
+      up[j] = vae_convT_geom(cin_s[j], cout_s[j], stride_s[j], kmul);
+      EZB_TRY(pack_convT(q + "1", &up[j], st));
       for (int u = 0; u < 3; ++u) {
         const std::string ru = q + std::to_string(u + 2) + ".layers.";
         EZB_TRY(prep_snake(ru + "0", cout_s[j], &res_s0[3 * j + u], st));
-        EZB_TRY(pack_conv(ru + "1", cout_s[j], cout_s[j], 7, dils[u], true, &res7[3 * j + u], st));
+        res7[3 * j + u] = vae_conv_geom(cout_s[j], cout_s[j], 7, dils[u], kmul);
+        EZB_TRY(pack_conv(ru + "1", true, &res7[3 * j + u], st));
         EZB_TRY(prep_snake(ru + "2", cout_s[j], &res_s2[3 * j + u], st));
-        EZB_TRY(pack_conv(ru + "3", cout_s[j], cout_s[j], 1, 1, true, &res1[3 * j + u], st));
+        res1[3 * j + u] = vae_conv_geom(cout_s[j], cout_s[j], 1, 1, kmul);
+        EZB_TRY(pack_conv(ru + "3", true, &res1[3 * j + u], st));
       }
     }
     const int C0 = cout_s[nst - 1];
@@ -407,11 +523,7 @@ struct Vae {
       const std::string k = p + std::to_string(nst + 2);
       EZB_TRY(need(k + ".weight_g", {1, 1, 1}, &g)); EZB_TRY(need(k + ".weight_v", {1, C0, 7}, &v));
       EZB_TRY(alloc(&norms, (size_t)1)); EZB_TRY(alloc(&out_w, (size_t)7 * C0));
-      ++launch_counter();
-      wn_norm_kernel<<<1, 256, 0, st>>>(v, C0 * 7, norms);
-      ++launch_counter();
-      fold_wave_w_kernel<<<(7 * C0 + 255) / 256, 256, 0, st>>>(v, g, norms, out_w, C0);
-      EZB_CUDA(cudaGetLastError());
+      EZB_TRY(vae_fold_wave_w(st, v, g, norms, out_w, C0));
     }
     if (d.with_encoder) EZB_TRY(finalize_encoder(st));
     EZB_CUDA(cudaStreamSynchronize(st));
@@ -419,27 +531,9 @@ struct Vae {
     return EZB_OK;
   }
 
-  // one implicit-GEMM conv: A [B, T, kmul*cin] -> epilogue
   int run_conv(cudaStream_t st, const VaeConv& c, const __nv_bfloat16* A, int B, int T, const float* resid_in, float* raw_out, __nv_bfloat16* act_out,
                const VaeSnake* snake) {
-    EpiLinearParams e;
-    memset(&e, 0, sizeof e);
-    e.bias = c.bias;
-    e.bias_mod = c.cout;
-    e.resid = resid_in; e.ldr = c.N;
-    e.out_f32 = raw_out; e.ld32 = c.N;
-    e.out_bf16 = act_out;
-    const int phases = c.N / c.cout;
-    e.ld16 = phases * kmul * c.cout;
-    e.split_stride = kmul == 3 ? c.cout : 0;
-    e.phase_cols = phases > 1 ? c.cout : 0;
-    e.phase_ld16 = kmul * c.cout;
-    if (snake) { e.act = ACT_SNAKE; e.act_a = snake->a; e.act_b = snake->binv; }
-    ConvAddr ca;
-    ca.taps = c.taps; ca.center = c.center; ca.dilation = c.dil; ca.cin_pad = c.cin_pad; ca.T = T; ca.B = B;
-    if (c.stride > 1 && c.N == c.cout) { ca.stride = c.stride; ca.pad = c.center; }  // strided conv (T = output length); conv-transpose has N = s*cout
-    const int ld = c.taps * c.cin_pad;
-    return gemm<128, EpiLinear<128>>(*dev, st, A, kmul * c.cin, c.w, ld, B * T, c.N, kmul * c.cin, e, &ca);
+    return vae_conv(*dev, st, c, kmul, A, B, T, resid_in, raw_out, act_out, snake);
   }
 
   // audio (B, 1, T) fp32, T = hop * L; noise (B, latent, L) fp32 or null (-> mean); z (B, latent, L) fp32
@@ -452,12 +546,7 @@ struct Vae {
     if (B < 1 || B > d.max_batch || L < 1 || L > d.max_latent_len) return fail(EZB_ERR_SHAPE, "vae_encode: B %d L %d exceed workspace", B, L);
     const int C0 = e_cin[0];
     __nv_bfloat16 *cur = actA, *oth = actB;
-    {
-      dim3 grid((unsigned)(((size_t)T * C0 + 255) / 256), B);
-      ++launch_counter();
-      enc_conv_in_kernel<<<grid, 256, 0, st>>>(audio, e_in_w, e_in_b, e_res_s0[0].a, e_res_s0[0].binv, resid, cur, C0, T, kmul);
-      EZB_CUDA(cudaGetLastError());
-    }
+    EZB_TRY(vae_enc_conv_in(st, audio, e_in_w, e_in_b, e_res_s0[0], resid, cur, B, C0, T, kmul));
     int Tc = T;
     for (int j = 0; j < nst; ++j) {
       for (int u = 0; u < 3; ++u) {
@@ -473,20 +562,13 @@ struct Vae {
       std::swap(cur, oth);
     }
     EZB_TRY(run_conv(st, e_out, cur, B, Tc, nullptr, resid, nullptr, nullptr));  // (mean | scale), channels-last fp32
-    dim3 g2((unsigned)(((size_t)d.latent_dim * L + 255) / 256), B);
-    ++launch_counter();
-    vae_sample_kernel<<<g2, 256, 0, st>>>(resid, noise, z, d.latent_dim, L);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    return vae_sample(st, resid, noise, z, B, d.latent_dim, L);
   }
 
   int decode(const float* z, float* wav, int B, int L, cudaStream_t st) {
     if (!finalized) return fail(EZB_ERR_STATE, "VAE weights not finalized");
     if (B < 1 || B > d.max_batch || L < 1 || L > d.max_latent_len) return fail(EZB_ERR_SHAPE, "vae_decode: B %d L %d exceed workspace", B, L);
-    dim3 grid((L + 31) / 32, (d.latent_dim + 31) / 32, B), blk(32, 8);
-    ++launch_counter();
-    latent_pack_kernel<<<grid, blk, 0, st>>>(z, actA, d.latent_dim, L, kmul);
-    EZB_CUDA(cudaGetLastError());
+    EZB_TRY(vae_latent_pack(st, z, actA, B, d.latent_dim, L, kmul));
     __nv_bfloat16 *cur = actA, *oth = actB;
     int T = L;
     EZB_TRY(run_conv(st, conv_in, cur, B, T, nullptr, nullptr, oth, &up_snake[0]));
@@ -503,14 +585,7 @@ struct Vae {
         EZB_TRY(run_conv(st, res1[3 * j + u], oth, B, T, resid, last ? nullptr : resid, cur, nxt));
       }
     }
-    const int C0 = cout_s[nst - 1];
-    if (C0 % 4) return fail(EZB_ERR_UNSUPPORTED, "wave_out: %d channels in the last stage (multiple of 4 expected)", C0);
-    dim3 g2((T + 127) / 128, B);
-    ++launch_counter();
-    if (kmul == 3) wave_out_kernel<3><<<g2, 128, 0, st>>>(cur, out_w, wav, C0, T);
-    else wave_out_kernel<1><<<g2, 128, 0, st>>>(cur, out_w, wav, C0, T);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    return vae_wave_out(st, cur, out_w, wav, B, cout_s[nst - 1], T, kmul);
   }
 };
 

@@ -16,6 +16,9 @@ class OobleckDecoder:
 
     def __init__(self, precision="bf16", max_batch=4, max_latent_len=512, device="cuda", encoder_cfg=None, **dec_cfg):
         self.shapes = weights.vae_decoder_param_shapes(dec_cfg)
+        odd = [s for s in dec_cfg["strides"] if s < 2 or s % 2]
+        if odd:  # ConvTranspose1d(k = 2s, stride s, padding ceil(s/2)) yields T*s - 1 frames for odd s, the library T*s
+            raise NotImplementedError(f"VAE decoder strides {list(dec_cfg['strides'])}: only even strides >= 2 are implemented")
         self.encoder_cfg = dict(encoder_cfg) if encoder_cfg else None
         if self.encoder_cfg is not None:
             weights.vae_encoder_param_shapes(self.encoder_cfg)  # validates the switches

@@ -203,6 +203,32 @@ int ezb_test_heads(int device, const void* A_bf16, const float* W_f32, const ezb
 int ezb_test_mlp(int device, const void* A_bf16, const float* W1_f32, const float* b1_f32, const void* W2_bf16, const float* b2, float* x,
                  const float* gate, int gate_bstride, int rows_per_batch, void* mid_bf16, void* grid_barrier, int M, int D, int inner,
                  int variant, void* stream);
+/* One layer of the Oobleck VAE, launched as Vae::decode / Vae::encode launch it (csrc/vae.cuh vae_conv and friends), from reference-layout
+   fp32 weights that the library weight-norms and packs.  Device pointers; kmul = 3 when precision is 1 (bf16x3), else 1.
+   kind 0 conv:       Conv1d(cin -> cout, taps, dilation dil, padding dil * (taps - 1) / 2), taps odd.  x: bf16 A [B, T, kmul*cin];
+                      weight_v [cout, cin, taps], weight_g [cout].  raw: fp32 [B, T, cout] (+ resid [B, T, cout], which may alias raw);
+                      act: bf16 SnakeBeta(alpha, beta)(raw) [B, T, kmul*cout] ([hi | lo | hi] in bf16x3).
+   kind 1 conv-T:     ConvTranspose1d(cin -> cout, k = 2 stride, stride (even), padding stride / 2).  weight_v [cin, cout, 2 stride],
+                      weight_g [cin]; raw [B, T*stride, cout], act [B, T*stride, kmul*cout].
+   kind 2 strided:    Conv1d(cin -> cout, k = 2 stride, stride, padding ceil(stride / 2)).  x [B, T*stride, kmul*cin]; T output rows.
+   kind 3 wave out:   Conv1d(cin -> 1, k = 7, padding 3, no bias) of x [B, T, kmul*cin]; weight_v [1, cin, 7], weight_g [1]; out fp32 [B, T].
+   kind 4 stem:       Conv1d(1 -> cout, k = 7, padding 3) of fp32 audio x [B, T]; weight_v [cout, 1, 7]; raw and act (both required).
+   kind 5 sample:     x fp32 enc [B*T, 2*cout] (mean | scale), noise fp32 [B, cout, T] or NULL -> out z [B, cout, T].
+   kind 6 latent:     x fp32 z [B, cin, T] -> act bf16 [B, T, kmul*cin].
+   bias [cout] (kinds 0, 1, 2, 4).  act needs alpha and beta ([cout], SnakeBeta's log-scale parameters).  w_packed (optional, kinds 0-4)
+   receives the weights the kernel read: kinds 0-2 bf16 [N, taps', cin_pad] with N = stride*cout for kind 1 (row r*cout + co: phase r),
+   cout otherwise, taps' = 3 for kind 1, 2*stride for kind 2, cin_pad = kmul*cin rounded up to 64, each tap [hi(cin) | hi | lo | 0];
+   kinds 3 and 4 fp32 [7][C]. */
+typedef struct {
+  int32_t kind, precision;
+  int32_t B, T, cin, cout, taps, dil, stride;
+  const float* weight_v; const float* weight_g; const float* bias;
+  const float* alpha; const float* beta;
+  const void* x; const float* resid; const float* noise;
+  float* raw; void* act; float* out;
+  void* w_packed;
+} ezb_test_vae_args;
+int ezb_test_vae(int device, const ezb_test_vae_args* args, void* stream);
 /* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7: that
    generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
