@@ -248,6 +248,7 @@ template <int BN>
 struct EpiLinear {
   using Params = EpiLinearParams;
   static constexpr int EPI_WARPS = BN >= 128 ? 8 : 4;       // two warps per 32-row group split the tile's columns
+  static constexpr bool WIDE_REGS = false;                  // true: run with GemmCfg::PRODUCER_WG
   static constexpr int STAGE_FLOATS = EPI_STAGE_FLOATS;
   // row0: global row of this warp's first accumulator row; nvalid: rows of the 32 that exist (<= 0: none);
   // [c_begin, c_end): this warp's column range inside the tile; wait(): blocks until the accumulator is complete.
@@ -358,6 +359,7 @@ struct EpiGeglu {
   using Params = EpiGegluParams;
   static constexpr int HALF = BN / 2;
   static constexpr int EPI_WARPS = BN == 256 ? 8 : 4;   // 8 warps: each takes 64 of the tile's 128 output features
+  static constexpr bool WIDE_REGS = false;
   static constexpr int STAGE_FLOATS = 32 * 32;          // 64 packed bf16 per row
   template <class Wait>
   static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
@@ -453,6 +455,7 @@ template <int BN>
 struct EpiLinearT {
   using Params = EpiLinearParams;   // bias/gate indexed by feature, resid/out_f32 [token, feature]; bf16/act/split unsupported
   static constexpr int EPI_WARPS = 8;
+  static constexpr bool WIDE_REGS = false;
   static constexpr int STAGE_FLOATS = 0;
   // residual values of one chunk of nt <= 32 tokens (feature f of tokens t0 .. t0+nt-1)
   static __device__ __forceinline__ void load_resid(const Params& ep, float (&x)[32], int t0, int nt, int f, bool f_ok) {
@@ -515,6 +518,7 @@ template <int BN>
 struct EpiLinearTF {
   using Params = EpiLinearParams;   // bias/gate indexed by feature, resid/out_f32 [token, feature]; bf16/act/split unsupported
   static constexpr int EPI_WARPS = 8;
+  static constexpr bool WIDE_REGS = false;
   static constexpr int STAGE_FLOATS = 0;
   template <class Wait>
   static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
@@ -614,17 +618,15 @@ struct GemmCfg {
   static constexpr int A_BYTES = KSUB * A_SUB;
   static constexpr int B_BYTES = KSUB * B_SUB;
   static constexpr int EPI_WARPS = Epi::EPI_WARPS;
-  // Every consumer warpgroup issues wgmma.  One warpgroup: both 64-row halves of the tile.  Two: one half each.  Three (EpiHeads, three
-  // heads per tile): all 128 rows of one head's columns each -- 72 / 72 / 80 (the last head plus the 8 zero columns) or 3 x 64 -- which
-  // keeps the accumulator at 80 registers under the 128-register cap of a 416-thread CTA.
+  // Every consumer warpgroup issues wgmma over the full BN columns.  One warpgroup: both 64-row halves of the tile.  Two: one half each.
   static constexpr int MMA_WG = EPI_WARPS / 4;
+  static_assert(MMA_WG == 1 || MMA_WG == 2, "one or two consumer warpgroups");
   static constexpr int NSUB = MMA_WG == 2 ? 1 : 2;                // 64-row halves per warpgroup
-  static constexpr int WN0 = MMA_WG == 3 ? (BN == 224 ? 72 : BN / 3) : BN;   // columns of warpgroups 0 .. MMA_WG - 2
-  static constexpr int WNL = MMA_WG == 3 ? BN - 2 * WN0 : BN;                 // columns of the last one
   // Consumer warpgroups + the producer warp.  A CTA of 9..12 warps puts three warps on one SM sub-partition, which caps every thread at 168
-  // registers: too few for the 144 accumulators of a 288-wide tile (ptxas spills and serialises the wgmma).  BN > 256 therefore runs a whole
+  // registers: too few for the 144 accumulators of a 288-wide tile (ptxas spills and serialises the wgmma), and for the 224-wide heads tile,
+  // whose 112 accumulators and two dh-wide epilogue rows per thread spill 1.4 KB (the epilogue asks with WIDE_REGS).  These run a whole
   // producer warpgroup (one active warp) that hands registers to the consumers with setmaxnreg: 384 x 168 = 128 x 40 + 256 x 232.
-  static constexpr bool PRODUCER_WG = BN > 256;
+  static constexpr bool PRODUCER_WG = BN > 256 || Epi::WIDE_REGS;
   static constexpr int THREADS = 32 * EPI_WARPS + (PRODUCER_WG ? 128 : 32);
   static constexpr int REGS_LAUNCH = (65536 / THREADS) & ~7;                        // what __launch_bounds__(THREADS, 1) lets ptxas allocate
   static constexpr int REGS_PRODUCER = 40;
@@ -643,11 +645,11 @@ struct GemmCfg {
   static_assert(BYTES <= 227 * 1024, "smem budget");
 };
 
-// One consumer warpgroup's share of a tile: WN accumulator columns from col0 over NSUB 64-row halves from 64-row block row64.  Runs the
+// One consumer warpgroup's share of a tile: all BN accumulator columns of NSUB 64-row halves from 64-row block row64.  Runs the
 // k-loop (slot s is released once wgmma.wait_group shows its MMAs complete, while slot s + 1's are in flight), then, after every warpgroup's
 // MMAs have completed, writes its fragments into the accumulator tile in shared memory.
-template <int BN, class Epi, int MC, int WN, int KSUB>
-__device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
+template <int BN, class Epi, int MC, int KSUB>
+__device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
                                               int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane) {
   using SM = GemmCfg<BN, Epi, KSUB>;
   constexpr int NSUB = SM::NSUB;
@@ -657,9 +659,9 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
       else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
     }
   };
-  constexpr int NH = WN > 256 ? 2 : 1;   // wgmma N stops at 256: a wider share is issued as two halves, HN columns each
-  constexpr int HN = WN / NH;
-  static_assert(HN <= 256 && HN % 8 == 0, "WN");   // HN % 8: the second half starts on a 1024-byte swizzle atom
+  constexpr int NH = BN > 256 ? 2 : 1;   // wgmma N stops at 256: a wider tile is issued as two halves, HN columns each
+  constexpr int HN = BN / NH;
+  static_assert(HN <= 256 && HN % 8 == 0, "BN");   // HN % 8: the second half starts on a 1024-byte swizzle atom
   float d[NSUB][NH][HN / 2];
   uint32_t prev = 0;
   for (int kb = 0; kb < num_k_blocks; kb += KSUB) {
@@ -670,7 +672,7 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
     for (int sub = 0; sub < KSUB; ++sub) {
       if (sub >= nsub) break;
       const uint32_t a0 = smem_u32(sA + stage * SM::A_BYTES + sub * SM::A_SUB + row64 * 8192);
-      const uint32_t b0 = smem_u32(sB + stage * SM::B_BYTES + sub * SM::B_SUB + col0 * 128);
+      const uint32_t b0 = smem_u32(sB + stage * SM::B_BYTES + sub * SM::B_SUB);
 #pragma unroll
       for (int k = 0; k < GEMM_BK / 16; ++k) {
 #pragma unroll
@@ -697,7 +699,7 @@ __device__ __forceinline__ void gemm_mma_part(int col0, int row64, const uint8_t
   for (int s = 0; s < NSUB; ++s) {
 #pragma unroll
     for (int h = 0; h < NH; ++h) {
-      float* r0 = sAcc + (size_t)((row64 + s) * 64 + 16 * lg + (lane >> 2)) * SM::ACC_PITCH + col0 + h * HN + 2 * (lane & 3);
+      float* r0 = sAcc + (size_t)((row64 + s) * 64 + 16 * lg + (lane >> 2)) * SM::ACC_PITCH + h * HN + 2 * (lane & 3);
 #pragma unroll
       for (int i = 0; i < HN / 8; ++i) {
         *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(d[s][h][4 * i], d[s][h][4 * i + 1]);
@@ -825,12 +827,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
       EZB_DBG(const long long tm = clock64();)
-      if constexpr (SM::MMA_WG == 3) {
-        if (wg == 2) gemm_mma_part<BN, Epi, MC, SM::WNL, KSUB>(2 * SM::WN0, 0, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
-        else gemm_mma_part<BN, Epi, MC, SM::WN0, KSUB>(wg * SM::WN0, 0, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
-      } else {
-        gemm_mma_part<BN, Epi, MC, BN, KSUB>(0, wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
-      }
+      gemm_mma_part<BN, Epi, MC, KSUB>(wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
       EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
       named_bar_sync(1, 32 * EPI_WARPS);     // accumulator tile complete in shared memory
       EZB_DBG(const long long te = clock64(); w1 += te - ta;)
@@ -908,15 +905,20 @@ struct EpiHeadsParams {
 
 // HPT = 2: tile = two adjacent heads of the reference column order (N-tile 2*dh).  HPT = 3: the packed QKV layout -- the
 // 3H heads of [q | k | v] are regrouped three per tile (N-tile 224 for dh = 72: 3 x 72 + 8 zero columns; 192 for dh = 64), which
-// makes the tile wide enough for the tensor pipe (narrow tiles are operand-bandwidth bound) and keeps one head per warp.
+// makes the tile wide enough for the tensor pipe (narrow tiles are operand-bandwidth bound).
+// Eight epilogue warps, two per 32-row group: warpgroup wg takes heads wg, wg + 2 of the tile on the group's rows, i.e. one head each at HPT = 2;
+// at HPT = 3 warpgroup 0 takes heads 0 and 2 and warpgroup 1 head 1 (12 head x row-group units on 8 warps take two rounds however they are
+// dealt).  The packed tile runs with the producer warpgroup's registers (GemmCfg::PRODUCER_WG): 112 accumulators per thread in the mainloop,
+// two dh-wide rows per thread in the epilogue.
 // DIRECT: every thread stores its own q / k row (dh bf16 = 128 or 144 contiguous bytes) with 16-byte stores instead of transposing it through a
-// per-warp 8 KB shared-memory tile.  The staging tiles of 12 epilogue warps take 96 KB, which leaves the 128 x 224 QKV tile only two 44 KB
-// pipeline stages; without them it gets four.
+// per-warp 8 KB shared-memory tile.  The staging tiles of the 8 epilogue warps take 64 KB, which leaves the 128 x 224 QKV tile three 44 KB
+// pipeline stages; without them it gets five.
 template <int DH, int HPT = 2, bool DIRECT = false, bool FOLD = false, bool DBG = false>
 struct EpiHeads {
   using Params = EpiHeadsParams;
   static constexpr int BN = HPT == 3 ? (DH == 72 ? 224 : 3 * DH) : 2 * DH;
-  static constexpr int EPI_WARPS = 4 * HPT;   // the HPT warps of a 32-row group take one head each
+  static constexpr int EPI_WARPS = 8;
+  static constexpr bool WIDE_REGS = HPT == 3;
   static constexpr int STAGE_FLOATS = DIRECT ? 0 : EPI_STAGE_FLOATS;
   template <class Wait>
   static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
@@ -928,8 +930,8 @@ struct EpiHeads {
     if (fold && row_ok) fold_row_stats(ep.fin, row, f_rstd, f_nmr);   // issued before the accumulator wait
     wait();
     const int b = row_ok ? row / ep.L : 0, l = row_ok ? row - b * ep.L : 0;
-    {
-      const int hh = c_begin / (BN / HPT);    // this warp's head inside the tile
+#pragma unroll 1
+    for (int hh = threadIdx.x >> 7; hh < HPT; hh += 2) {   // gemm_body's consumer warp 4 wg + (32-row group): heads wg, wg + 2
       int sec, head;
       if (HPT == 3) {
         const int g = (n0 / BN) * 3 + hh;     // global head index in [q heads | k heads | v heads]
@@ -937,7 +939,7 @@ struct EpiHeads {
         head = g - sec * ep.H;
       } else {
         const int n = n0 + hh * DH;
-        if (n >= N) return;
+        if (n >= N) break;
         sec = n / ep.D;
         head = (n - sec * ep.D) / DH;
       }
@@ -999,7 +1001,7 @@ struct EpiHeads {
               dst[g] = make_uint4(pack_bf16(v[8 * g], v[8 * g + 1]), pack_bf16(v[8 * g + 2], v[8 * g + 3]), pack_bf16(v[8 * g + 4], v[8 * g + 5]),
                                   pack_bf16(v[8 * g + 6], v[8 * g + 7]));
           }
-          return;
+          continue;
         }
         // bf16 pairs -> staging granules (4 bf16 each) -> coalesced row stores
 #pragma unroll
