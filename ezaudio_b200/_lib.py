@@ -55,6 +55,15 @@ class TestVaeArgs(C.Structure):
                                           "w_packed")]
 
 
+class TestFp8Args(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "M", "D")] + \
+               [(n, C.c_void_p) for n in ("x", "weight", "bias", "shift", "scale", "q", "s")] + [("inner", C.c_int32)] + \
+               [(n, C.c_void_p) for n in ("w", "b", "out")] + [(n, C.c_int32) for n in ("B", "L", "H", "dh")] + \
+               [(n, C.c_void_p) for n in ("norm_q", "norm_k", "inv_freq")] + [("rope", C.c_int32)] + \
+               [(n, C.c_void_p) for n in ("q_out", "k_out", "vt_out")] + [(n, C.c_int32) for n in ("ld_qk", "dvp", "Lpad")] + \
+               [(n, C.c_void_p) for n in ("w_q", "w_s")]
+
+
 _lib = None
 
 _VP, _I, _F = C.c_void_p, C.c_int, C.c_float
@@ -99,6 +108,7 @@ _SIGS = {
     "ezb_test_heads": ([_I, _VP, _VP, C.POINTER(TestHeadsArgs), _VP], _I),
     "ezb_test_mlp": ([_I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP], _I),
     "ezb_test_vae": ([_I, C.POINTER(TestVaeArgs), _VP], _I),
+    "ezb_test_fp8": ([_I, C.POINTER(TestFp8Args), _VP], _I),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -161,8 +161,17 @@ class _Base:
         return NativeTextEncoder(tok, enc, ml, device)
 
 
+def _vae_precision(precision: str) -> str:
+    """The VAE (and T5) have no FP8 mode: precision="fp8" builds them in "bf16"."""
+    return "bf16" if precision == "fp8" else precision
+
+
 class EzAudio(_Base):
-    """api/ezaudio.py:31."""
+    """api/ezaudio.py:31.
+
+    precision: "bf16" (default, throughput), "bf16x3" (fp32-grade parity) or "fp8": the DiT's self-attention QKV and GEGLU up-projections
+    run on H100 FP8 tensor cores (e4m3 operands with per-row scales, fp32 accumulation), everything else as in "bf16"; the VAE and the
+    text encoder run in "bf16".  See DESIGN.md section 3 for its accuracy."""
 
     def __init__(self, model_name, ckpt_path=None, vae_path=None, device="cuda", *, text_encoder: Optional[Callable] = None,
                  precision: str = "bf16", max_batch: int = 4, max_length_s: float = 10.0, config_path=None, vae_config_path=None):
@@ -177,7 +186,8 @@ class EzAudio(_Base):
                             max_timesteps=1000, device=device, **p["model"])
         self.unet.load_state_dict(_state_dict(ckpt_path, weights.dit_param_shapes(p["model"]), "model"))
         dcfg, ecfg = config.load_vae_decoder_config(vae_config_path), config.load_vae_encoder_config(vae_config_path)
-        dec = OobleckDecoder(precision=precision, max_batch=max_batch, max_latent_len=max_len, device=device, encoder_cfg=ecfg, **dcfg)
+        dec = OobleckDecoder(precision=_vae_precision(precision), max_batch=max_batch, max_latent_len=max_len, device=device, encoder_cfg=ecfg,
+                             **dcfg)
         vshapes = dict(weights.vae_decoder_param_shapes(dcfg))
         vshapes.update(weights.vae_encoder_param_shapes(ecfg))
         vsd = _state_dict(vae_path, vshapes, "state_dict")
@@ -296,7 +306,7 @@ def energy_condition(audio: torch.Tensor, hop_size=240, window_size=1920, paddin
 
 
 class EzAudio_ControlNet(_Base):
-    """api/controlnet.py:31."""
+    """api/controlnet.py:31.  precision as for EzAudio ("fp8" applies to the DiT and the ControlNet)."""
 
     def __init__(self, model_name, ckpt_path=None, controlnet_path=None, vae_path=None, device="cuda", *,
                  text_encoder: Optional[Callable] = None, precision: str = "bf16", max_batch: int = 4, config_path=None,
@@ -315,7 +325,7 @@ class EzAudio_ControlNet(_Base):
         csd = _state_dict(controlnet_path, weights.controlnet_param_shapes(p["model"], p["controlnet"]), "model")
         self.controlnet.load_state_dict(csd, mask_embed=sd["mask_embed"])
         dcfg = config.load_vae_decoder_config(vae_config_path)
-        dec = OobleckDecoder(precision=precision, max_batch=max_batch, max_latent_len=max_len, device=device, **dcfg)
+        dec = OobleckDecoder(precision=_vae_precision(precision), max_batch=max_batch, max_latent_len=max_len, device=device, **dcfg)
         vsd = _state_dict(vae_path, weights.vae_decoder_param_shapes(dcfg), "state_dict")
         vsd = {(k[len("autoencoder."):] if k.startswith("autoencoder.") else k): v for k, v in vsd.items()}
         dec.load_state_dict(vsd)

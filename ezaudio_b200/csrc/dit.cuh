@@ -33,6 +33,9 @@ struct BlockW {
   // per-clip cross-attention K / V^T caches
   float *kc32 = nullptr, *vc32 = nullptr;
   bf16 *kc16 = nullptr, *vtc16 = nullptr;
+  // FP8 mode: e4m3 copies of the packed QKV and GEGLU weights with per-row scales (quantised at finalize)
+  uint8_t *qkv8 = nullptr, *mlp18 = nullptr;
+  float *s_qkv = nullptr, *s_mlp1 = nullptr;
 };
 
 struct WeightSpec {
@@ -98,6 +101,10 @@ struct Dit {
   int geglu_bn = 128;     // N-tile of the GEGLU GEMM: packing group = geglu_bn / 2
   int qkv3_bn = 0;        // >0: self-attention QKV weight packed three heads per N-tile of this width (EpiHeads<DH,3>)
   const int32_t* lens = nullptr;   // forward(): valid frames per sample of the padded batch (device [Be]) or null; read by self-attention and the final conv
+  // FP8 mode (precision 2): norm1 -> QKV and norm3 -> GEGLU run on e4m3 operands (ln8 writes act8 / act8_s), everything else as in bf16 mode
+  bool fp8 = false;
+  uint8_t* act8 = nullptr;
+  float* act8_s = nullptr;
 
   ~Dit() {
     for (void* p : allocs) cudaFree(p);
@@ -156,20 +163,24 @@ struct Dit {
     half = d.depth / 2;
     nblk = d.is_controlnet ? half : d.depth + 1;
     kmul = d.precision == 1 ? 3 : 1;
-    if (d.precision != 0 && d.precision != 1) return fail(EZB_ERR_UNSUPPORTED, "precision %d", d.precision);
+    if (d.precision < 0 || d.precision > 2) return fail(EZB_ERR_UNSUPPORTED, "precision %d", d.precision);
+    fp8 = d.precision == 2;
     pair = opt_pair_gemm() != 0;
     swap_ab = opt_swap_ab() != 0;
     geglu_bn = (pair && inner % 128 == 0) ? 256 : 128;
-    qkv3_bn = (pair && d.precision == 0 && (D / H == 72 || D / H == 64) && H % 2 == 0 && opt_qkv3()) ? (D / H == 72 ? 224 : 192) : 0;
+    qkv3_bn = (pair && d.precision != 1 && (D / H == 72 || D / H == 64) && H % 2 == 0 && opt_qkv3()) ? (D / H == 72 ? 224 : 192) : 0;
     if (dh > 96 || dh % 8 || D % 16 || inner % 64 || d.context_dim % 8 || d.depth % 2)
       return fail(EZB_ERR_UNSUPPORTED, "unsupported dims: D %d dh %d inner %d ctx %d depth %d", D, dh, inner, d.context_dim, d.depth);
+    if (fp8 && (qkv3_bn == 0 || D > 1152))
+      return fail(EZB_ERR_UNSUPPORTED, "fp8: needs the packed QKV (head dim 64 or 72, an even head count, options pair_gemm and qkv3 on) "
+                  "and embed_dim <= 1152 (D %d dh %d H %d)", D, dh, H);
     if (d.max_batch < 1 || d.max_batch > 256 || d.max_len < 1 || d.max_ctx_len < 1 || d.max_timesteps < 1) return fail(EZB_ERR_ARG, "workspace bounds");
     Kp = (2 * C + 1 + KP_PATCH_ALIGN - 1) / KP_PATCH_ALIGN * KP_PATCH_ALIGN;
     // q / k row pitch: dh = 72 rows are 80 elements (160 bytes: 64 columns behind a SWIZZLE_128B box + a 16-column SWIZZLE_32B tail box, TMA only
     // needs 16-byte strides); the round-1 pitch of 128 moved 1.56x the algorithmic bytes (ncu dram__bytes_read 43.2 MB vs 27.6 MB)
     DHP = dh == 72 ? (opt_dhp80() ? 80 : 128) : (dh + 63) / 64 * 64;
     DVP = (dh + 15) / 16 * 16;
-    use_tc_attention = (d.precision == 0);
+    use_tc_attention = (d.precision != 1);
     blk.resize(nblk);
     const std::string pre = d.is_controlnet ? "" : "model.";
     // ---- trunk
@@ -244,6 +255,10 @@ struct Dit {
           EZB_CUDA(cudaGetLastError());
           return EZB_OK;
         });
+      }
+      if (fp8) {
+        EZB_TRY(alloc(&w.qkv8, (size_t)H * qkv3_bn * D)); EZB_TRY(alloc(&w.s_qkv, (size_t)H * qkv3_bn));
+        EZB_TRY(alloc(&w.mlp18, (size_t)2 * inner * D)); EZB_TRY(alloc(&w.s_mlp1, (size_t)2 * inner));
       }
       EZB_TRY(alloc_w(&w.mlp2, D, inner));
       reg_linear(p + ".mlp.net.2.weight", D, inner, w.mlp2, inner, 0);
@@ -326,7 +341,8 @@ struct Dit {
       }
     }
     EZB_TRY(alloc(&grid_bar, (size_t)1));
-    if (d.precision == 0 && (D == 1152 || D == 1024)) {   // precombined LayerNorm affine tables (ln_gc_kernel)
+    if (fp8) { EZB_TRY(alloc(&act8, Mx * D)); EZB_TRY(alloc(&act8_s, Mx)); }
+    if (d.precision != 1 && (D == 1152 || D == 1024)) {   // precombined LayerNorm affine tables (ln_gc_kernel)
       gc_T = d.max_timesteps < 128 ? d.max_timesteps : 128;
       for (int i = 0; i < nblk; ++i) {
         EZB_TRY(alloc(&blk[i].lnG1, (size_t)gc_T * D)); EZB_TRY(alloc(&blk[i].lnC1, (size_t)gc_T * D));
@@ -404,6 +420,13 @@ struct Dit {
       EZB_CUDA(cudaGetLastError());
       EZB_CUDA(cudaDeviceSynchronize());
     }
+    if (fp8) {  // after the packing permutations: a row scale follows its row
+      for (auto& w : blk) {
+        EZB_TRY(quant_rows(w.qkv, H * qkv3_bn, D, w.qkv8, w.s_qkv));
+        EZB_TRY(quant_rows(w.mlp1, 2 * inner, D, w.mlp18, w.s_mlp1));
+      }
+      EZB_CUDA(cudaDeviceSynchronize());
+    }
     if (fold_cfg) {  // static sites: norm2 -> cross-Q and skip_norm -> skip_linear (no modulation: G = weight, C = bias)
       for (int i = 0; i < nblk; ++i) {
         BlockW& w = blk[i];
@@ -413,6 +436,12 @@ struct Dit {
       EZB_CUDA(cudaDeviceSynchronize());
     }
     finalized = true;
+    return EZB_OK;
+  }
+  int quant_rows(const bf16* W, int N, int K, uint8_t* Q, float* S) {
+    ++launch_counter();
+    quant_rows_e4m3_kernel<<<(N + 7) / 8, 256>>>(W, N, K, Q, S);
+    EZB_CUDA(cudaGetLastError());
     return EZB_OK;
   }
   int fold_uv(cudaStream_t st, const bf16* W, int ldw, const float* G, const float* Cc, const float* add_v, float* U, float* V, int N, int K, int R) {
@@ -518,6 +547,16 @@ struct Dit {
     }
     return launch_k(ln_mod_cast_kernel, dim3((M + 7) / 8), dim3(256), 0, st, 1, p);
   }
+  // FP8 mode: LayerNorm (+ modulate) of p.x to e4m3 act8 with row scales act8_s (p.out is not written)
+  int ln8(cudaStream_t st, const LnParams& p) {
+    if (opt_skip() & 1) return EZB_OK;
+    if (p.x2 != nullptr || p.w == nullptr || p.D1 > 1152) return fail(EZB_ERR_UNSUPPORTED, "fp8 LayerNorm: single source of at most 1152 features");
+    const int M = p.M, grid = dev->num_sms * 4 < (M + 3) / 4 ? dev->num_sms * 4 : (M + 3) / 4;
+    const LnFp8Out o{act8, act8_s};
+    if (p.D1 == 1152) return launch_k(ln_fp8_kernel<9, true>, dim3(grid), dim3(128), 0, st, 1, p, o);
+    if (p.D1 == 1024) return launch_k(ln_fp8_kernel<8, true>, dim3(grid), dim3(128), 0, st, 1, p, o);
+    return launch_k(ln_fp8_kernel<9, false>, dim3(grid), dim3(128), 0, st, 1, p, o);
+  }
   int ln(cudaStream_t st, const float* x, int D1, const float* x2, const float* x3, int D2, const float* w, const float* b, const float* shift,
          const float* scale, int mod_bstride, int rows_per_batch, bf16* out, int M) {
     return ln(st, ln_params(x, D1, x2, x3, D2, w, b, shift, scale, mod_bstride, rows_per_batch, out, M));
@@ -588,9 +627,8 @@ struct Dit {
     return EZB_OK;
   }
   // Q/K/V projection with the fused per-head LN + RoPE + attention-layout epilogue (fast mode)
-  int lin_heads(cudaStream_t st, const bf16* A, const bf16* W, int M, int N, const int* kinds, const float (*nq)[96], const float (*nk)[96], bool rope,
-                int L, bf16* qo, bf16* ko, bf16* vto, int Lpad, const FoldIn* fin = nullptr) {
-    if (opt_skip() & 4) return EZB_OK;
+  EpiHeadsParams heads_params(int N, const int* kinds, const float (*nq)[96], const float (*nk)[96], bool rope, int L, bf16* qo, bf16* ko, bf16* vto,
+                              int Lpad, const FoldIn* fin) {
     EpiHeadsParams e;
     memset(&e, 0, sizeof e);
     if (fin) e.fin = *fin;
@@ -605,6 +643,12 @@ struct Dit {
     for (int i = 0; i < dh / 2 && i < 36; ++i) e.inv_freq[i] = h_inv_freq[i];
     e.out[0] = qo; e.out[1] = ko; e.out[2] = vto;
     e.ld_qk = DHP; e.dvp = DVP; e.Lpad = Lpad;
+    return e;
+  }
+  int lin_heads(cudaStream_t st, const bf16* A, const bf16* W, int M, int N, const int* kinds, const float (*nq)[96], const float (*nk)[96], bool rope,
+                int L, bf16* qo, bf16* ko, bf16* vto, int Lpad, const FoldIn* fin = nullptr) {
+    if (opt_skip() & 4) return EZB_OK;
+    EpiHeadsParams e = heads_params(N, kinds, nq, nk, rope, L, qo, ko, vto, Lpad, fin);
     const bool direct = opt_heads_direct() != 0, fo = fin != nullptr;
     int variant;
     if (qkv3_bn > 0 && N == 3 * D) {  // packed self-attention QKV: three heads per tile
@@ -779,18 +823,24 @@ struct Dit {
         if (!entry_ln_done) EZB_TRY(ln(st, x_in, D, skip, cskip, D, w.snw, w.snb, nullptr, nullptr, 0, L, act, M));
         const LnParams p1 = ln_params(x_out, D, nullptr, nullptr, 0, w.n1w, w.n1b, m + 0 * D, m + 1 * D, mbs, L, act, M);
         entry_ln_done = false;   // from here on: "norm1 done?"
-        EZB_TRY(lin(st, act, 2 * D, w.skip, M, D, e, &p1, &entry_ln_done));   // the tail runs behind a grid barrier: nobody reads `act` any more
+        EZB_TRY(lin(st, act, 2 * D, w.skip, M, D, e, fp8 ? nullptr : &p1, &entry_ln_done));   // the tail runs behind a grid barrier: nobody reads `act` any more
         fold1 = false;
       }
       x_in = x_out;
     }
     // --- self-attention (blocks.py:137-141)
-    if (!fold1 && !entry_ln_done) EZB_TRY(ln(st, x_in, D, nullptr, nullptr, 0, w.n1w, w.n1b, m + 0 * D, m + 1 * D, mbs, L, act, M));
+    if (fp8) EZB_TRY(ln8(st, ln_params(x_in, D, nullptr, nullptr, 0, w.n1w, w.n1b, m + 0 * D, m + 1 * D, mbs, L, act, M)));
+    else if (!fold1 && !entry_ln_done) EZB_TRY(ln(st, x_in, D, nullptr, nullptr, 0, w.n1w, w.n1b, m + 0 * D, m + 1 * D, mbs, L, act, M));
     if (fused_heads) {
       const int kinds[3] = {0, 1, 2};
       const int Lp = (L + 7) / 8 * 8;
       FoldIn f1 = fold_in(st1, nullptr, D, w.u1 + (size_t)fc.t * n_qkv, w.v1 + (size_t)fc.t * n_qkv);
-      EZB_TRY(lin_heads(st, act, w.qkv, M, 3 * D, kinds, w.h_nq, w.h_nk, true, L, q16, k16, vt16, Lp, fold1 ? &f1 : nullptr));
+      if (fp8) {
+        if (!(opt_skip() & 4))
+          EZB_TRY(heads_gemm_fp8(*dev, st, act8, act8_s, w.qkv8, w.s_qkv, M, dh, heads_params(3 * D, kinds, w.h_nq, w.h_nk, true, L, q16, k16, vt16, Lp, nullptr)));
+      } else {
+        EZB_TRY(lin_heads(st, act, w.qkv, M, 3 * D, kinds, w.h_nq, w.h_nk, true, L, q16, k16, vt16, Lp, fold1 ? &f1 : nullptr));
+      }
       EZB_TRY(attention(st, q32, k32, v32, q16, k16, vt16, nullptr, Be, L, L, Lp, lens));
     } else {
       EZB_TRY(lin_to_qkv(st, act, D, w.qkv, M, 3 * D));
@@ -828,10 +878,11 @@ struct Dit {
       e.bias = w.b_cproj; e.resid = x_out; e.ldr = D; e.out_f32 = x_out; e.ld32 = D;
       if (fc.on) e.fout = fold_out(w.st_b, act, D, w.g3 + (size_t)fc.t * D);
       const LnParams p3 = ln_params(x_out, D, nullptr, nullptr, 0, w.n3w, w.n3b, m + 3 * D, m + 4 * D, mbs, L, act, M);
-      EZB_TRY(lin(st, attn_out, D, w.cproj, M, D, e, fc.on ? nullptr : &p3, &ln3_done));
+      EZB_TRY(lin(st, attn_out, D, w.cproj, M, D, e, fc.on || fp8 ? nullptr : &p3, &ln3_done));
     }
     // --- GEGLU MLP (blocks.py:155-156; modules.py:263-277,366)
-    if (!fc.on && !ln3_done) EZB_TRY(ln(st, x_out, D, nullptr, nullptr, 0, w.n3w, w.n3b, m + 3 * D, m + 4 * D, mbs, L, act, M));
+    if (fp8) EZB_TRY(ln8(st, ln_params(x_out, D, nullptr, nullptr, 0, w.n3w, w.n3b, m + 3 * D, m + 4 * D, mbs, L, act, M)));
+    else if (!fc.on && !ln3_done) EZB_TRY(ln(st, x_out, D, nullptr, nullptr, 0, w.n3w, w.n3b, m + 3 * D, m + 4 * D, mbs, L, act, M));
     {
       EpiGegluParams g;
       memset(&g, 0, sizeof g);
@@ -840,13 +891,15 @@ struct Dit {
       EpiLinearParams e = epi();
       e.bias = w.b_mlp2; e.resid = x_out; e.ldr = D; e.gate = m + 5 * D; e.gate_bstride = mbs; e.rows_per_batch = L; e.out_f32 = x_out; e.ld32 = D;
       if (fc.on) e.fout = block_output_fold(i, fc.t);
-      if (opt_mlp_fused() && geglu_bn == 256 && kmul == 1 && swap_ab && !(opt_skip() & 24) && L >= 32) {
+      if (!fp8 && opt_mlp_fused() && geglu_bn == 256 && kmul == 1 && swap_ab && !(opt_skip() & 24) && L >= 32) {
         // the whole MLP as one persistent launch (north_star: "MLP GEMM + act + GEMM as one persistent kernel")
         if (fc.on) EZB_TRY((mlp_fused<EpiGeglu<256, true>, EpiLinearTF<256>>(*dev, st, act, w.mlp1, M, 2 * inner, D, g, mid, w.mlp2, D, inner, e, grid_bar)));
         else EZB_TRY((mlp_fused<EpiGeglu<256>, EpiLinearT<256>>(*dev, st, act, w.mlp1, M, 2 * inner, D, g, mid, w.mlp2, D, inner, e, grid_bar)));
         return EZB_OK;
       }
       if (opt_skip() & 16) {}
+      else if (fp8 && geglu_bn == 256) EZB_TRY((gemm2_fp8<256, EpiGeglu<256>>(*dev, st, act8, act8_s, w.mlp18, w.s_mlp1, M, 2 * inner, D, g)));
+      else if (fp8) EZB_TRY((gemm2_fp8<128, EpiGeglu<128>>(*dev, st, act8, act8_s, w.mlp18, w.s_mlp1, M, 2 * inner, D, g)));   // inner % 128 != 0
       else if (geglu_bn == 256 && fc.on) EZB_TRY((gemm2<256, EpiGeglu<256, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       else if (geglu_bn == 256 && (opt_ksub2() & 1) && kmul == 1) EZB_TRY((gemm2<256, EpiGeglu<256>, 2>(*dev, st, act, D, w.mlp1, D, M, 2 * inner, D, g)));   // 128-deep slots
       else if (geglu_bn == 256) EZB_TRY((gemm2<256, EpiGeglu<256>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
@@ -913,14 +966,15 @@ struct Dit {
     };
     bool done = false;
     LnParams nl = entry_ln(0, x0);
-    EZB_TRY(embed(st, x, gt, gt_mask, nullptr, Be, L, fc, &nl, &done));
+    // FP8 mode: a norm1 LayerNorm (in- and mid-blocks) writes e4m3 rows, so it never runs as the bf16 tail of the GEMM before it
+    EZB_TRY(embed(st, x, gt, gt_mask, nullptr, Be, L, fc, fp8 ? nullptr : &nl, &done));
     const float* xc = x0;
     fc.st_x = st_x0;
     for (int i = 0; i < half; ++i) {
       const bool entry = done;
       done = false;
       nl = entry_ln(i + 1, skips[i]);
-      EZB_TRY(block(st, i, xc, skips[i], nullptr, nullptr, modr, mbs, Be, L, fc, entry, &nl, &done));
+      EZB_TRY(block(st, i, xc, skips[i], nullptr, nullptr, modr, mbs, Be, L, fc, entry, fp8 ? nullptr : &nl, &done));
       xc = skips[i];
       fc.st_x = blk[i].st_out;
     }
@@ -999,14 +1053,14 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
   };
   bool done = false;
   LnParams nl = entry_ln(0, x0);
-  EZB_TRY(embed(st, x, gt, gt_mask, cond_emb, Be, L, fc, &nl, &done));                       // x = patch_embed(x) + condition
+  EZB_TRY(embed(st, x, gt, gt_mask, cond_emb, Be, L, fc, fp8 ? nullptr : &nl, &done));       // x = patch_embed(x) + condition
   const float* xc = x0;
   fc.st_x = st_x0;
   for (int i = 0; i < half; ++i) {
     const bool entry = done;
     done = false;
     if (i + 1 < half) nl = entry_ln(i + 1, skips[i]);
-    EZB_TRY(block(st, i, xc, skips[i], nullptr, nullptr, modr, mbs, Be, L, fc, entry, i + 1 < half ? &nl : nullptr, &done));
+    EZB_TRY(block(st, i, xc, skips[i], nullptr, nullptr, modr, mbs, Be, L, fc, entry, i + 1 < half && !fp8 ? &nl : nullptr, &done));
     xc = skips[i];
     fc.st_x = blk[i].st_out;
   }

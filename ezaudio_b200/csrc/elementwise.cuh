@@ -262,6 +262,99 @@ __device__ __forceinline__ void ln_tail(const LnParams& p) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// FP8 mode: e4m3 operands with one fp32 scale per row, s = amax / 448 and q = e4m3(v * (448 / amax)) saturated (amax = 0: q = 0, s = 0).
+__device__ __forceinline__ float e4m3_inv_scale(float amax) { return amax > 0.f ? 448.f / amax : 0.f; }
+__device__ __forceinline__ uint32_t pack_e4m3x2(float lo, float hi) {   // round to nearest even, saturated to +-448; lo -> the low byte
+  unsigned short r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) { return pack_e4m3x2(a, b) | (pack_e4m3x2(c, d) << 16); }
+struct LnFp8Out {
+  uint8_t* q;   // [M, D1] e4m3
+  float* s;     // [M] row scales
+};
+// LayerNorm (+ AdaLN modulate) of x [M, D1] to e4m3 rows: the operand of the FP8 QKV and GEGLU projections.  The row stays in registers
+// (D1 <= 128 NCH; EXACT: D1 == 128 NCH), so its amax costs one warp reduction.  Affine from the precombined per-timestep tables (p.G, p.C,
+// as ln_gc_kernel) when set, else weight, bias and the per-batch shift / scale (as ln_row_generic).  One warp per row, rows in a strided loop.
+template <int NCH, bool EXACT>
+__global__ void __launch_bounds__(128) ln_fp8_kernel(const LnParams p, const LnFp8Out o) {
+  pdl_launch();
+  pdl_wait();
+  const int D = EXACT ? NCH * 128 : p.D1;
+  const int lane = threadIdx.x & 31, gw = blockIdx.x * 4 + (threadIdx.x >> 5), nw = gridDim.x * 4;
+  for (int row = gw; row < p.M; row += nw) {
+    const float* x = p.x + (size_t)row * D;
+    float4 v[NCH];
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int c4 = lane + 32 * i;
+      v[i] = (EXACT || 4 * c4 < D) ? ldcg4(x + 4 * c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+    const float mean = warp_sum(s) / D;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      if (!EXACT && 4 * (lane + 32 * i) >= D) continue;
+      const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+      q += (a * a + b * b) + (c * c + d * d);
+    }
+    const float rstd = rsqrtf(warp_sum(q) / D + 1e-5f);
+    const float *sh = nullptr, *sc = nullptr;
+    if (p.G == nullptr && p.shift != nullptr) {
+      const size_t off = (size_t)(row / p.rows_per_batch) * p.mod_bstride;
+      sh = p.shift + off;
+      sc = p.scale + off;
+    }
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int c4 = lane + 32 * i;
+      if (!EXACT && 4 * c4 >= D) continue;
+      float y[4] = {(v[i].x - mean) * rstd, (v[i].y - mean) * rstd, (v[i].z - mean) * rstd, (v[i].w - mean) * rstd};
+      if (p.G != nullptr) {
+        const float4 g = __ldg(reinterpret_cast<const float4*>(p.G) + c4), c = __ldg(reinterpret_cast<const float4*>(p.C) + c4);
+        y[0] = fmaf(y[0], g.x, c.x); y[1] = fmaf(y[1], g.y, c.y); y[2] = fmaf(y[2], g.z, c.z); y[3] = fmaf(y[3], g.w, c.w);
+      } else {
+        const float4 w = __ldg(reinterpret_cast<const float4*>(p.w) + c4), b = __ldg(reinterpret_cast<const float4*>(p.b) + c4);
+        y[0] = y[0] * w.x + b.x; y[1] = y[1] * w.y + b.y; y[2] = y[2] * w.z + b.z; y[3] = y[3] * w.w + b.w;
+        if (sh) {
+          const float4 a = *reinterpret_cast<const float4*>(sc + 4 * c4), d = *reinterpret_cast<const float4*>(sh + 4 * c4);
+          y[0] = y[0] * (1.f + a.x) + d.x; y[1] = y[1] * (1.f + a.y) + d.y; y[2] = y[2] * (1.f + a.z) + d.z; y[3] = y[3] * (1.f + a.w) + d.w;
+        }
+      }
+      v[i] = make_float4(y[0], y[1], y[2], y[3]);
+      amax = fmaxf(amax, fmaxf(fmaxf(fabsf(y[0]), fabsf(y[1])), fmaxf(fabsf(y[2]), fabsf(y[3]))));
+    }
+    amax = warp_max(amax);
+    const float inv = e4m3_inv_scale(amax);
+    uint32_t* out = reinterpret_cast<uint32_t*>(o.q + (size_t)row * D);
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) {
+      const int c4 = lane + 32 * i;
+      if (!EXACT && 4 * c4 >= D) continue;
+      out[c4] = pack_e4m3x4(v[i].x * inv, v[i].y * inv, v[i].z * inv, v[i].w * inv);
+    }
+    if (lane == 0) o.s[row] = amax / 448.f;
+  }
+}
+// FP8 mode, at finalize: rows of a packed bf16 weight [N, K] -> e4m3 [N, K] with per-row scales (the same rule as ln_fp8_kernel).  One warp per row.
+__global__ void __launch_bounds__(256) quant_rows_e4m3_kernel(const __nv_bfloat16* __restrict__ W, int N, int K, uint8_t* __restrict__ Q, float* __restrict__ S) {
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (row >= N) return;
+  const __nv_bfloat16* w = W + (size_t)row * K;
+  float amax = 0.f;
+  for (int k = lane; k < K; k += 32) amax = fmaxf(amax, fabsf(__bfloat162float(w[k])));
+  amax = warp_max(amax);
+  const float inv = e4m3_inv_scale(amax);
+  for (int k = lane; k < K; k += 32) Q[(size_t)row * K + k] = (uint8_t)pack_e4m3x2(__bfloat162float(w[k]) * inv, 0.f);
+  if (lane == 0) S[row] = amax / 448.f;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Per-head LayerNorm(dh, affine) on q / k (attention.py:63-65,141-142), NeoX rotate-half RoPE with fp32 tables on
 // positions 0..L-1 (rotary.py:6-18,72-84; pairs (i, i+dh/2), freq 1e4^(-2i/dh)), and head-major layout for attention:
 //   section 0 (q), 1 (k): dst[b, h, l, 0..dh)  (row pitch dst_ld, zero padding beyond dh pre-cleared)

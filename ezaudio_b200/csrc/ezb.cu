@@ -223,6 +223,53 @@ __attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* 
 }
 
 namespace {
+// packs W (reference layout fp32) as Dit::init does, quantises it as Dit::finalize does, runs the kernel
+int test_fp8_gemm(Device& dev, cudaStream_t st, const ezb_test_fp8_args* a, __nv_bfloat16* Wp, uint8_t* Wq, float* Ws, float* bp) {
+  const int D = a->D, M = a->M;
+  const uint8_t* A = static_cast<const uint8_t*>(a->q);
+  if (a->kind == 1) {
+    constexpr int half = 128;   // GEGLU packing group of the 256-wide N-tiles
+    const int inner = a->inner, N = 2 * inner;
+    pack_weight_kernel<<<(unsigned)(((size_t)N * D + 255) / 256), 256, 0, st>>>(a->w, N, D, Wp, D, 1, 0, inner, half, 0, 0, 0);
+    pack_geglu_bias_kernel<<<(N + 255) / 256, 256, 0, st>>>(a->b, bp, inner, half);
+    quant_rows_e4m3_kernel<<<(N + 7) / 8, 256, 0, st>>>(Wp, N, D, Wq, Ws);
+    EZB_CUDA(cudaGetLastError());
+    if (a->w_q) EZB_CUDA(cudaMemcpyAsync(a->w_q, Wq, (size_t)N * D, cudaMemcpyDeviceToDevice, st));
+    if (a->w_s) EZB_CUDA(cudaMemcpyAsync(a->w_s, Ws, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    EpiGegluParams g;
+    memset(&g, 0, sizeof g);
+    g.bias = bp; g.out_bf16 = static_cast<__nv_bfloat16*>(a->out); g.ld16 = inner;
+    return gemm2_fp8<256, EpiGeglu<256>>(dev, st, A, a->s, Wq, Ws, M, N, D, g);
+  }
+  const int H = a->H, dh = a->dh, bn3 = dh == 72 ? 224 : 192, rows = H * bn3;
+  const unsigned grid_w = (unsigned)(((size_t)D * D + 255) / 256);
+  for (int s = 0; s < 3; ++s) pack_weight_kernel<<<grid_w, 256, 0, st>>>(a->w + (size_t)s * D * D, D, D, Wp, D, 1, 0, 0, 0, dh, s * H, bn3);
+  quant_rows_e4m3_kernel<<<(rows + 7) / 8, 256, 0, st>>>(Wp, rows, D, Wq, Ws);
+  EZB_CUDA(cudaGetLastError());
+  if (a->w_q) EZB_CUDA(cudaMemcpyAsync(a->w_q, Wq, (size_t)rows * D, cudaMemcpyDeviceToDevice, st));
+  if (a->w_s) EZB_CUDA(cudaMemcpyAsync(a->w_s, Ws, (size_t)rows * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  EpiHeadsParams e;
+  memset(&e, 0, sizeof e);
+  EZB_CUDA(cudaStreamSynchronize(st));   // by-value parameters, as ezb_test_heads
+  EZB_CUDA(cudaMemcpy(e.nw[0], a->norm_q, dh * sizeof(float), cudaMemcpyDeviceToHost)); EZB_CUDA(cudaMemcpy(e.nb[0], a->norm_q + dh, dh * sizeof(float), cudaMemcpyDeviceToHost));
+  EZB_CUDA(cudaMemcpy(e.nw[1], a->norm_k, dh * sizeof(float), cudaMemcpyDeviceToHost)); EZB_CUDA(cudaMemcpy(e.nb[1], a->norm_k + dh, dh * sizeof(float), cudaMemcpyDeviceToHost));
+  if (a->rope) EZB_CUDA(cudaMemcpy(e.inv_freq, a->inv_freq, (dh / 2) * sizeof(float), cudaMemcpyDeviceToHost));
+  e.D = D; e.H = H; e.L = a->L;
+  for (int s = 0; s < 3; ++s) e.kind[s] = s;
+  e.rope_kinds = 3; e.rope_ld = a->L; e.rope_mufu = a->rope == 2;
+  e.out[0] = static_cast<__nv_bfloat16*>(a->q_out); e.out[1] = static_cast<__nv_bfloat16*>(a->k_out); e.out[2] = static_cast<__nv_bfloat16*>(a->vt_out);
+  e.ld_qk = a->ld_qk; e.dvp = a->dvp; e.Lpad = a->Lpad;
+  float2* cs = nullptr;
+  if (a->rope) {
+    EZB_CUDA(cudaMallocAsync(&cs, (size_t)a->L * (dh / 2) * sizeof(float2), st));
+    rope_table_kernel<<<(a->L * (dh / 2) + 255) / 256, 256, 0, st>>>(a->inv_freq, cs, a->L, dh / 2);
+    EZB_CUDA(cudaGetLastError());
+    e.rope = cs;
+  }
+  const int rc = heads_gemm_fp8(dev, st, A, a->s, Wq, Ws, M, dh, e);
+  if (cs) EZB_CUDA(cudaFreeAsync(cs, st));
+  return rc;
+}
 int test_vae_run(Device& dev, cudaStream_t st, const ezb_test_vae_args* a, int kmul, float* scratch, size_t part, __nv_bfloat16** wp) {
   float *norms = scratch, *wfold = scratch + part;
   const VaeSnake sn{scratch + 2 * part, scratch + 3 * part};
@@ -302,6 +349,54 @@ __attribute__((visibility("default"))) int ezb_test_vae(int device, const ezb_te
   return rc;
 }
 
+__attribute__((visibility("default"))) int ezb_test_fp8(int device, const ezb_test_fp8_args* a, void* stream) {
+  if (!a) return fail(EZB_ERR_ARG, "ezb_test_fp8: null arguments");
+  const int kind = a->kind, M = a->M, D = a->D;
+  if (kind < 0 || kind > 2) return fail(EZB_ERR_ARG, "ezb_test_fp8: kind %d", kind);
+  if (M < 1 || M > (1 << 24) || D < 16 || D % 16 || D > 1152) return fail(EZB_ERR_SHAPE, "ezb_test_fp8: M %d D %d (D a multiple of 16, at most 1152)", M, D);
+  if (!a->q || !a->s) return fail(EZB_ERR_ARG, "ezb_test_fp8: null operand q / s");
+  if (kind == 0 && (!a->x || !a->weight || !a->bias || (!a->shift != !a->scale))) return fail(EZB_ERR_ARG, "ezb_test_fp8: LayerNorm needs x, weight, bias");
+  if (kind == 1 && (!a->w || !a->b || !a->out || a->inner < 128 || a->inner % 128))
+    return fail(EZB_ERR_ARG, "ezb_test_fp8: GEGLU needs w, b, out and inner (a multiple of 128), inner %d", a->inner);
+  if (kind == 2) {
+    const int H = a->H, dh = a->dh;
+    if ((dh != 64 && dh != 72) || H < 2 || H % 2 || D != H * dh) return fail(EZB_ERR_SHAPE, "ezb_test_fp8: heads H %d dh %d D %d", H, dh, D);
+    if (a->B < 1 || a->L < 1 || (long long)a->B * a->L != M) return fail(EZB_ERR_SHAPE, "ezb_test_fp8: B %d L %d M %d", a->B, a->L, M);
+    if (!a->w || !a->norm_q || !a->norm_k || !a->q_out || !a->k_out || !a->vt_out) return fail(EZB_ERR_ARG, "ezb_test_fp8: heads needs w, norms and outputs");
+    if (a->ld_qk < dh || a->ld_qk % 8 || a->Lpad < a->L || a->dvp < dh) return fail(EZB_ERR_SHAPE, "ezb_test_fp8: output pitches");
+    if (a->rope < 0 || a->rope > 2 || (a->rope && !a->inv_freq)) return fail(EZB_ERR_ARG, "ezb_test_fp8: rope mode %d", a->rope);
+  }
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  dev.tmaps.trim();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (kind == 0) {
+    LnParams p;
+    memset(&p, 0, sizeof p);
+    p.x = a->x; p.D1 = D; p.w = a->weight; p.b = a->bias; p.shift = a->shift; p.scale = a->scale; p.mod_bstride = 0; p.rows_per_batch = 1;
+    p.kmul = 1; p.M = M;
+    const LnFp8Out o{static_cast<uint8_t*>(a->q), a->s};
+    const int grid = dev.num_sms * 4 < (M + 3) / 4 ? dev.num_sms * 4 : (M + 3) / 4;   // as Dit::ln8
+    if (D == 1152) return launch_k(ln_fp8_kernel<9, true>, dim3(grid), dim3(128), 0, st, 1, p, o);
+    if (D == 1024) return launch_k(ln_fp8_kernel<8, true>, dim3(grid), dim3(128), 0, st, 1, p, o);
+    return launch_k(ln_fp8_kernel<9, false>, dim3(grid), dim3(128), 0, st, 1, p, o);
+  }
+  const size_t rows = kind == 1 ? (size_t)2 * a->inner : (size_t)a->H * (a->dh == 72 ? 224 : 192);
+  __nv_bfloat16* Wp = nullptr;
+  uint8_t* Wq = nullptr;
+  float *Ws = nullptr, *bp = nullptr;
+  EZB_CUDA(cudaMallocAsync(&Wp, rows * D * sizeof(__nv_bfloat16), st));
+  EZB_CUDA(cudaMemsetAsync(Wp, 0, rows * D * sizeof(__nv_bfloat16), st));   // packed-3 pad rows stay 0, as Dit::alloc leaves them
+  EZB_CUDA(cudaMallocAsync(&Wq, rows * D, st));
+  EZB_CUDA(cudaMallocAsync(&Ws, rows * sizeof(float), st));
+  EZB_CUDA(cudaMallocAsync(&bp, rows * sizeof(float), st));
+  const int rc = test_fp8_gemm(dev, st, a, Wp, Wq, Ws, bp);
+  EZB_CUDA(cudaFreeAsync(Wp, st));
+  EZB_CUDA(cudaFreeAsync(Wq, st));
+  EZB_CUDA(cudaFreeAsync(Ws, st));
+  EZB_CUDA(cudaFreeAsync(bp, st));
+  return rc;
+}
 
 #define EZB_API __attribute__((visibility("default")))
 #define ST(s) reinterpret_cast<cudaStream_t>(s)

@@ -607,6 +607,13 @@ struct EpiLinearTF {
   }
 };
 
+// FP8 mode (gemm_fp8_kernel): e4m3 operands with per-row scales; the MMA warpgroups multiply the fp32 accumulator by sa[row] * sw[col] as they
+// park it in shared memory, so the epilogues see the dequantised tile and run unchanged.
+struct Fp8Scales {
+  const float* sa;   // [M] per token row (A operand)
+  const float* sw;   // [N] per output feature (W operand, in its packed row order)
+};
+
 // Shared-memory plan of one CTA: the STAGES-deep operand ring (which also holds the finished fp32 accumulator tile between the
 // mainloop and the epilogue of a tile), the epilogues' per-warp transpose tiles, the barriers.
 // KSUB: 64-wide k-blocks per ring slot.  KSUB = 2 gives 128-deep slots: half as many full / empty barrier round trips (and wgmma
@@ -648,9 +655,12 @@ struct GemmCfg {
 // One consumer warpgroup's share of a tile: all BN accumulator columns of NSUB 64-row halves from 64-row block row64.  Runs the
 // k-loop (slot s is released once wgmma.wait_group shows its MMAs complete, while slot s + 1's are in flight), then, after every warpgroup's
 // MMAs have completed, writes its fragments into the accumulator tile in shared memory.
-template <int BN, class Epi, int MC, int KSUB>
+// FP8: the ring slots hold 128-element e4m3 k-blocks (the same 128-byte rows), issued as four k32 MMAs at the bf16 descriptor steps; the
+// accumulator is dequantised with the scales of global rows m0 + .. (< M) and columns n0 + .. on its way to shared memory.
+template <int BN, class Epi, int MC, int KSUB, bool FP8 = false>
 __device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
-                                              int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane) {
+                                              int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane, const Fp8Scales& fs = Fp8Scales{},
+                                              int m0 = 0, int M = 0, int n0 = 0) {
   using SM = GemmCfg<BN, Epi, KSUB>;
   constexpr int NSUB = SM::NSUB;
   auto release = [&](uint32_t s) {   // one thread per warpgroup, on the slot's barrier in every CTA of the cluster
@@ -679,7 +689,8 @@ __device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, cons
         for (int s = 0; s < NSUB; ++s)
 #pragma unroll
           for (int h = 0; h < NH; ++h)
-            Wgmma<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | sub | k) != 0);
+            if constexpr (FP8) WgmmaE4m3<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | sub | k) != 0);
+            else Wgmma<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | sub | k) != 0);
       }
     }
     wgmma_commit();
@@ -695,6 +706,23 @@ __device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, cons
     for (int h = 0; h < NH; ++h) wgmma_fence_regs(d[s][h]);
   named_bar_sync(1, 32 * SM::EPI_WARPS);   // every MMA of the tile has completed: the ring may now hold the accumulator
   // m64nN fragment: register 4i + {0,1} -> row 16 * (warp % 4) + lane / 4, columns 8i + 2 (lane % 4) + {0,1}; 4i + {2,3} -> row + 8
+  if constexpr (FP8) {
+#pragma unroll
+    for (int s = 0; s < NSUB; ++s) {
+      const int r = m0 + (row64 + s) * 64 + 16 * lg + (lane >> 2);
+      const float sa0 = r < M ? fs.sa[r] : 0.f, sa1 = r + 8 < M ? fs.sa[r + 8] : 0.f;
+#pragma unroll
+      for (int h = 0; h < NH; ++h) {
+        const float2* sw = reinterpret_cast<const float2*>(fs.sw + n0 + h * HN + 2 * (lane & 3));
+#pragma unroll
+        for (int i = 0; i < HN / 8; ++i) {
+          const float2 w = __ldg(sw + 4 * i);
+          d[s][h][4 * i] *= sa0 * w.x; d[s][h][4 * i + 1] *= sa0 * w.y;
+          d[s][h][4 * i + 2] *= sa1 * w.x; d[s][h][4 * i + 3] *= sa1 * w.y;
+        }
+      }
+    }
+  }
 #pragma unroll
   for (int s = 0; s < NSUB; ++s) {
 #pragma unroll
@@ -724,9 +752,11 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, int KSUB = 1>
-__device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw) {
+template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, int KSUB = 1, bool FP8 = false>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw,
+                                          const Fp8Scales& fs = Fp8Scales{}) {
   using SM = GemmCfg<BN, Epi, KSUB>;
+  constexpr int KB_ELEMS = FP8 ? 2 * GEMM_BK : GEMM_BK;   // elements per 128-byte k-block row
   // BN > 256: two TMA boxes and two wgmma halves per warpgroup, single CTA, one 64-row half per MMA warpgroup (the 288-token swap-AB tile)
   static_assert(BN % 16 == 0 && BN >= 64 && (BN <= 256 || (BN <= 512 && BN % 32 == 0 && MC == 1 && SM::MMA_WG == 2)), "BN");
   static_assert(MC >= 1 && MC <= 8 && BN % McSub<BN>::ROWS == 0, "MC");
@@ -791,7 +821,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
           uint8_t* dA = sA + stage * SM::A_BYTES + sub * SM::A_SUB;
           uint8_t* dB = sB + stage * SM::B_BYTES + sub * SM::B_SUB;
           if (g.taps == 0) {
-            tma_load_2d(dA, &tmA, &full[stage], kb * GEMM_BK, mt * GEMM_BM);
+            tma_load_2d(dA, &tmA, &full[stage], kb * KB_ELEMS, mt * GEMM_BM);
           } else {
             const int tap = kb / g.cin_blocks, cb = kb - tap * g.cin_blocks;
             const int bidx = mt / g.tiles_per_batch, t0 = (mt - bidx * g.tiles_per_batch) * GEMM_BM;
@@ -806,11 +836,11 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
           if (MC == 1) {
             constexpr int BOX = gemm_b_box(BN);
 #pragma unroll
-            for (int j = 0; j < BN / BOX; ++j) tma_load_2d(dB + j * BOX * 128, &tmB, &full[stage], kb * GEMM_BK, n0 + j * BOX);
+            for (int j = 0; j < BN / BOX; ++j) tma_load_2d(dB + j * BOX * 128, &tmB, &full[stage], kb * KB_ELEMS, n0 + j * BOX);
           } else {
             constexpr int SR = McSub<BN>::ROWS;
             for (int j = (int)cluster_ctarank(); j < BN / SR; j += MC)
-              tma_load_2d_mc(dB + j * SR * 128, &tmB, &full[stage], kb * GEMM_BK, n0 + j * SR, MC_MASK);
+              tma_load_2d_mc(dB + j * SR * 128, &tmB, &full[stage], kb * KB_ELEMS, n0 + j * SR, MC_MASK);
           }
           }
         }
@@ -827,7 +857,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
       EZB_DBG(const long long tm = clock64();)
-      gemm_mma_part<BN, Epi, MC, KSUB>(wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane);
+      gemm_mma_part<BN, Epi, MC, KSUB, FP8>(wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane, fs, mt * GEMM_BM, g.M, nt * BN);
       EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
       named_bar_sync(1, 32 * EPI_WARPS);     // accumulator tile complete in shared memory
       EZB_DBG(const long long te = clock64(); w1 += te - ta;)
@@ -876,6 +906,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const typename Epi::Params ep) {
   extern __shared__ uint8_t smem_dyn[];
   gemm_body<BN, Epi, MC, false, KSUB>(tmA, tmB, g, ep, smem_dyn);
+}
+// FP8 twin of gemm_wgmma_kernel<BN, Epi, 2> (2-CTA clusters, W tile multicast): A [M, K] and W [N, K] e4m3 through UINT8 tensor maps with
+// 128-element k-blocks (num_k_blocks = K / 128), dequantised by the per-row scales fs (see Fp8Scales).
+template <int BN, class Epi>
+__global__ void __launch_bounds__((GemmCfg<BN, Epi>::THREADS), 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g, const typename Epi::Params ep,
+                const Fp8Scales fs) {
+  extern __shared__ uint8_t smem_dyn[];
+  gemm_body<BN, Epi, 2, false, 1, true>(tmA, tmB, g, ep, smem_dyn, fs);
 }
 
 }  // namespace ezb

@@ -84,9 +84,9 @@ inline PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// bf16 tensor, innermost dim first; 128-byte swizzle, zero fill out of bounds.
+// bf16 (or `dtype`) tensor, innermost dim first; 128-byte swizzle, zero fill out of bounds.
 inline int make_tmap(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes /*rank-1*/,
-                     const uint32_t* box) {
+                     const uint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return fail(EZB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
   cuuint64_t gd[5], gs[5];
@@ -100,7 +100,7 @@ inline int make_tmap(CUtensorMap* out, const void* ptr, int rank, const uint64_t
   if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) return fail(EZB_ERR_ARG, "TMA base %p not 16-byte aligned", ptr);
   for (int i = 0; i + 1 < rank; ++i)
     if (gs[i] % 16) return fail(EZB_ERR_ARG, "TMA stride %llu not a multiple of 16 B", (unsigned long long)gs[i]);
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = enc(out, dtype, rank, const_cast<void*>(ptr), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(EZB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): rank %d dims %llu,%llu box %u,%u", (int)r, rank,
@@ -126,6 +126,20 @@ struct TmapCache {
       uint64_t dims[2] = {inner, outer}, str[1] = {ld * 2};
       uint32_t box[2] = {64, box_outer};
       EZB_TRY(make_tmap(&m, ptr, 2, dims, str, box));
+      it = maps.emplace(k, m).first;
+    }
+    *out = &it->second;
+    return EZB_OK;
+  }
+  // 2-D [outer, inner] row-major e4m3 bytes (ld bytes per row), box {128, box_outer}: the same 128-byte rows as a bf16 box of 64
+  int get2d_u8(const void* ptr, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_outer, const CUtensorMap** out) {
+    Key k(ptr, inner, outer, ld, 0, box_outer, 8);
+    auto it = maps.find(k);
+    if (it == maps.end()) {
+      CUtensorMap m;
+      uint64_t dims[2] = {inner, outer}, str[1] = {ld};
+      uint32_t box[2] = {128, box_outer};
+      EZB_TRY(make_tmap(&m, ptr, 2, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_UINT8));
       it = maps.emplace(k, m).first;
     }
     *out = &it->second;
@@ -477,6 +491,49 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
   return EZB_OK;
 }
 
+// FP8 twin of gemm2 (gemm.cuh gemm_fp8_kernel): A [M, K] and W [N, K] e4m3 (row pitch K bytes), per-row scales sa [M], sw [N].
+template <int BN, class Epi>
+int gemm2_fp8(Device& dev, cudaStream_t st, const uint8_t* A, const float* sa, const uint8_t* W, const float* sw, int M, int N, int K,
+              const typename Epi::Params& ep) {
+  if (M <= 0 || N <= 0 || K <= 0) return fail(EZB_ERR_SHAPE, "gemm2_fp8: empty problem %d %d %d", M, N, K);
+  if ((K % 16) || (N % BN)) return fail(EZB_ERR_SHAPE, "gemm2_fp8: K must be a multiple of 16 and N of %d (M%d N%d K%d)", BN, M, N, K);
+  GemmShape g;
+  memset(&g, 0, sizeof g);
+  g.M = M; g.N = N;
+  g.num_n_tiles = N / BN;
+  g.num_m_tiles = ((M + GEMM_BM - 1) / GEMM_BM + 1) & ~1;   // whole clusters, as gemm2
+  g.num_k_blocks = (K + 2 * GEMM_BK - 1) / (2 * GEMM_BK);    // 128-element k-blocks
+  dev.next_weights(W, (size_t)N * K, &g.pf, &g.pf_bytes);
+  const CUtensorMap *tA, *tB;
+  EZB_TRY(dev.tmaps.get2d_u8(A, (uint64_t)K, (uint64_t)M, (uint64_t)K, GEMM_BM, &tA));
+  EZB_TRY(dev.tmaps.get2d_u8(W, (uint64_t)K, (uint64_t)N, (uint64_t)K, McSub<BN>::ROWS, &tB));
+  auto kern = gemm_fp8_kernel<BN, Epi>;
+  constexpr int smem = GemmCfg<BN, Epi>::BYTES;
+  constexpr int GEMM_THREADS = GemmCfg<BN, Epi>::THREADS;
+  static int clusters[16] = {};
+  if (!clusters[dev.id & 15]) {
+    EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    EZB_TRY(resident_clusters2(dev, kern, smem, GEMM_THREADS, &clusters[dev.id & 15]));
+  }
+  const int tiles = g.num_m_tiles * g.num_n_tiles, max_ctas = 2 * clusters[dev.id & 15];
+  const int ctas = tiles < max_ctas ? tiles : max_ctas;
+  GemmProf& gp = gemm_prof();
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (gp.on) {
+    if (gp.used + 2 > gp.ev.size()) {
+      for (int i = 0; i < 2; ++i) { cudaEvent_t e; EZB_CUDA(cudaEventCreate(&e)); gp.ev.push_back(e); }
+    }
+    e0 = gp.ev[gp.used]; e1 = gp.ev[gp.used + 1];
+    gp.used += 2;
+    gp.flops.push_back(2.0 * (double)M * (double)N * (double)K);
+    EZB_CUDA(cudaEventRecord(e0, st));
+  }
+  const Fp8Scales fs{sa, sw};
+  EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, g, ep, fs));
+  if (gp.on) EZB_CUDA(cudaEventRecord(e1, st));
+  return EZB_OK;
+}
+
 inline int& opt_mlp_fused() {
   static int v = [] { const char* e = getenv("EZB_MLP_FUSED"); return e ? atoi(e) : 0; }();
   return v;
@@ -604,6 +661,15 @@ inline int heads_gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, cons
   }
 #undef EZB_HEADS
   return fail(EZB_ERR_ARG, "heads_gemm: variant %d", variant);
+}
+// FP8 mode's packed self-attention QKV: the one kernel it runs (three heads per N-tile, staged q / k stores, no fold).  A [M, D] e4m3 with row
+// scales sa; W [H * BN, D] e4m3 packed as for HEADS_PACKED3 with row scales sw.
+inline int heads_gemm_fp8(Device& dev, cudaStream_t st, const uint8_t* A, const float* sa, const uint8_t* W, const float* sw, int M, int dh,
+                          const EpiHeadsParams& e) {
+  if (e.fin.u != nullptr || e.dbg) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm_fp8: no fold or profiling epilogue");
+  if (dh == 72) return gemm2_fp8<224, EpiHeads<72, 3>>(dev, st, A, sa, W, sw, M, e.H * 224, e.D, e);
+  if (dh == 64) return gemm2_fp8<192, EpiHeads<64, 3>>(dev, st, A, sa, W, sw, M, e.H * 192, e.D, e);
+  return fail(EZB_ERR_UNSUPPORTED, "heads_gemm_fp8: head dimension %d", dh);
 }
 
 }  // namespace ezb

@@ -14,7 +14,18 @@ import torch
 
 from . import _lib, weights
 
-PRECISIONS = {"bf16": 0, "bf16x3": 1}
+# "fp8": the QKV and GEGLU up-projections of every block on e4m3 operands (per-row scales), the rest as "bf16" (include/ezb200.h)
+PRECISIONS = {"bf16": 0, "bf16x3": 1, "fp8": 2}
+
+
+def check_fp8_config(cfg: dict):
+    """The FP8 mode runs the packed three-heads-per-tile QKV kernel and the 256-wide GEGLU kernel only: configurations those cannot hold
+    are rejected here, before any device work."""
+    D, H = cfg["embed_dim"], cfg["num_heads"]
+    dh = D // H
+    if dh not in (64, 72) or H % 2 or D > 1152:
+        raise ValueError(f"precision 'fp8' needs head dim 64 or 72 with an even head count and embed_dim <= 1152 "
+                         f"(embed_dim {D}, heads {H}); use 'bf16' or 'bf16x3'")
 
 
 def _as_f32c(t: torch.Tensor) -> torch.Tensor:
@@ -30,6 +41,8 @@ class _Handle:
         weights.check_dit_config(cfg)
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be one of {list(PRECISIONS)}")
+        if precision == "fp8":
+            check_fp8_config(cfg)
         self.cfg, self.cn = dict(cfg), (dict(controlnet) if controlnet else None)
         self.device = torch.device(device)
         if self.device.type != "cuda":

@@ -36,7 +36,10 @@ typedef struct {
   int32_t is_controlnet;      /* 1: DiTControlNet (src/models/controlnet.py:87) -- first half + stem + zero linears */
   int32_t cond_c0, cond_c1;   /* controlnet stem widths (cond_blocks, ckpts/controlnet/energy_l.yml:40) */
   int32_t max_batch, max_len, max_ctx_len, max_timesteps; /* workspace bounds (effective batch incl. CFG doubling) */
-  int32_t precision;          /* 0: bf16 operands / fp32 accumulate; 1: bf16x3 split operands (fp32-grade parity mode) */
+  int32_t precision;          /* 0: bf16 operands / fp32 accumulate; 1: bf16x3 split operands (fp32-grade parity mode);
+                                 2: FP8 -- the self-attention QKV and GEGLU up-projections of every block take e4m3 operands (one fp32 scale
+                                 per token row and per weight row, amax / 448) on fp32-accumulating wgmma, everything else as in mode 0.
+                                 Needs head dim 64 or 72 with an even head count and embed_dim <= 1152. */
 } ezb_dit_desc;
 
 int ezb_version(void); /* 2: ezb_dit_forward / ezb_cfg_ddim_step take per-sample lengths */
@@ -229,6 +232,25 @@ typedef struct {
   void* w_packed;
 } ezb_test_vae_args;
 int ezb_test_vae(int device, const ezb_test_vae_args* args, void* stream);
+/* The FP8 mode's kernels (precision 2), launched as the model launches them.  Device pointers.
+   kind 0: LayerNorm (eps 1e-5, weight / bias [D]) + AdaLN modulate (shift / scale [D], one row for all rows; NULL: none) of x [M, D] fp32
+           -> q [M, D] e4m3 and row scales s [M] (s = amax / 448 of the row, q = e4m3(y * 448 / amax)).
+   kind 1: GEGLU projection of A = q [M, D] e4m3 with row scales s: W [2*inner, D], b [2*inner] fp32 in the reference layout ([hidden; gate]
+           rows), packed and quantised by the library; out [M, inner] bf16.
+   kind 2: packed self-attention QKV projection of A = (q, s) with the heads epilogue: W [3D, D] fp32 reference layout ([q; k; v]); outputs and
+           their layout as ezb_test_heads with nsec 3, kinds {0, 1, 2} and the staged packed-3 variant.
+   w_q / w_s (optional, kinds 1 and 2): receive the e4m3 weight and its row scales as the GEMM read them (packed row order). */
+typedef struct {
+  int32_t kind, M, D;
+  const float* x; const float* weight; const float* bias; const float* shift; const float* scale;
+  void* q; float* s;
+  int32_t inner; const float* w; const float* b; void* out;
+  int32_t B, L, H, dh;
+  const float* norm_q; const float* norm_k; const float* inv_freq; int32_t rope;
+  void* q_out; void* k_out; void* vt_out; int32_t ld_qk, dvp, Lpad;
+  void* w_q; float* w_s;
+} ezb_test_fp8_args;
+int ezb_test_fp8(int device, const ezb_test_fp8_args* args, void* stream);
 /* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7: that
    generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
