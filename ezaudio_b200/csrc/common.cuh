@@ -82,6 +82,21 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// Shared -> global box store, tracked by the issuing thread's bulk async-groups.  The generic writes that filled `src` must be made
+// visible to the async proxy first (fence_proxy_async_smem by every writing thread, then a barrier); elements outside the map's bounds
+// are not written.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed groups still read their shared-memory source (the buffer may be rewritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's committed groups are still incomplete (their global writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------------------------ wgmma (warpgroup MMA, operands in shared memory)
 // K-major operand tile in shared memory, rows of 64 bf16 (128 B) with the 128-byte swizzle TMA writes

@@ -902,7 +902,7 @@ struct Dit {
       else if (fp8) EZB_TRY((gemm2_fp8<128, EpiGeglu<128>>(*dev, st, act8, act8_s, w.mlp18, w.s_mlp1, M, 2 * inner, D, g)));   // inner % 128 != 0
       else if (geglu_bn == 256 && fc.on) EZB_TRY((gemm2<256, EpiGeglu<256, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       else if (geglu_bn == 256 && (opt_ksub2() & 1) && kmul == 1) EZB_TRY((gemm2<256, EpiGeglu<256>, 2>(*dev, st, act, D, w.mlp1, D, M, 2 * inner, D, g)));   // 128-deep slots
-      else if (geglu_bn == 256) EZB_TRY((gemm2<256, EpiGeglu<256>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
+      else if (geglu_bn == 256) EZB_TRY(gemm2_geglu(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g));
       else if (fc.on) EZB_TRY((gemm<128, EpiGeglu<128, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       else EZB_TRY((gemm<128, EpiGeglu<128>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       if (opt_mlp2_pair() && pair && kmul == 1 && !fc.on)   // MLP-out on 2-CTA cluster tiles (128 tokens x 128 features, thread = token row) instead of swap-AB

@@ -85,7 +85,7 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
       EpiGegluParams p;
       memset(&p, 0, sizeof p);
       p.bias = e->bias; p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(e->out_bf16); p.ld16 = e->ld16; p.split_stride = e->split_stride;
-      if (bn == 256) return gemm2<256, EpiGeglu<256>>(dev, st, a, lda, w, ldw, M, N, K, p);
+      if (bn == 256) return gemm2_geglu(dev, st, a, lda, w, ldw, M, N, K, p);   // what Dit::block dispatches
     }
     return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm pair: bn=%d", bn);
   }
@@ -214,7 +214,7 @@ __attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* 
   if (variant == 0) {
     rc = mlp_fused<EpiGeglu<256>, EpiLinearT<256>>(dev, st, a16, W1p, M, 2 * inner, D, g, m16, w2, D, inner, p, reinterpret_cast<GridBarrier*>(bar));
   } else {
-    rc = variant == 2 ? gemm2<256, EpiGeglu<256>, 2>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g) : gemm2<256, EpiGeglu<256>>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g);
+    rc = variant == 2 ? gemm2<256, EpiGeglu<256>, 2>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g) : gemm2_geglu(dev, st, a16, D, W1p, D, M, 2 * inner, D, g);
     if (rc == EZB_OK) rc = gemm_swapped<EpiLinearT>(dev, st, m16, inner, w2, inner, M, D, inner, p);
   }
   EZB_CUDA(cudaFreeAsync(W1p, st));

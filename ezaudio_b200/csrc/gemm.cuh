@@ -6,6 +6,8 @@
 //                                      slot once its MMAs have completed, then park the finished 128 x BN fp32 tile in shared memory
 //                                      (over the ring, which is idle then); every consumer warp runs the fused epilogue on 32 rows
 //                                      (thread == row) of it.  The producer refills the ring for the next tile once the epilogue is done.
+//   An epilogue that works on the wgmma fragment itself (FRAG, the plain GEGLU: EpiGegluFrag) keeps the accumulator out of the ring instead:
+//   the producer streams the next tile's k-blocks while the MMA warpgroups run the epilogue from their registers and store through TMA.
 //
 // A can also be addressed as an implicit-GEMM operand of a 1-D convolution over channels-last activations
 // [B, T, C]: k-block kb -> tap = kb / cin_blocks, rows shifted by (tap - center) * dilation with TMA zero fill at
@@ -39,7 +41,8 @@ struct GemmShape {
   int taps, center, dilation, cin_blocks, T, tiles_per_batch;
   int stride, pad;     // stride > 1: strided conv (VAE encoder): A is a 4-D map [B, T/stride, stride, C], tap k reads row q*stride + k - pad
   unsigned long long* dbg;  // optional cycle counters of CTA 0 (builds with -DEZB_GEMM_DEBUG): [0] warpgroup 0 mainloop incl. its full-slot waits,
-                            // [1] consumer wait for the accumulator tile, [2] producer wait for empty slots, [3] unused, [4] warp 0 epilogue, [5] total
+                            // [1] consumer wait for the accumulator tile (FRAG: for the output tile's previous store), [2] producer wait for
+                            // empty slots, [3] unused, [4] warp 0 epilogue, [5] total
   // L2 prefetch of the weights the NEXT GEMM of the step will stream (host.cuh WeightSeq): every layer's weights are read once per step,
   // i.e. from HBM, and a kernel's first k-blocks pay that latency on top of its ramp.
   const char* pf;
@@ -439,6 +442,62 @@ struct EpiGeglu {
   }
 };
 
+// The GEGLU epilogue of the plain bf16 path (no LayerNorm fold, no bf16x3 split) on the wgmma fragment, for gemm_body's overlapped schedule
+// (FRAG): the accumulator stays in the MMA warpgroup's registers, so the ring never holds it and the producer streams the next tile's k-blocks
+// while this runs.  In the m64n256 fragment hidden column j and gate column j + 128 of a row sit in the same thread (registers 4i.. and
+// 4(i + 16)..), so the gate is applied in place with EpiGeglu's float operations in EpiGeglu's order: the output is bit-identical.  Each
+// warpgroup writes its 64 x 128 bf16 result into its own 16 KB smem tile (two 64 x 64 boxes in the TMA 128-byte swizzle, conflict-free for
+// the fragment's 4-byte writes) and stores it with two TMA box stores through `out`, a map of out_bf16 [M, N / 2] (pitch ld16) with
+// {64 features, 64 rows} boxes, built by gemm2: its bounds clip rows >= M and the empty padding tile of an odd M-tile count.
+// Params: bias, out_bf16, ld16 as for EpiGeglu; split_stride must be 0 and fin unset.
+// Barrier of MMA warpgroup wg's 128 threads (ids 2 and 3; id 1 is the parked schedule's consumer barrier).  Constant ids, so that ptxas reserves
+// only the barriers the kernel uses.
+__device__ __forceinline__ void warpgroup_bar_sync(int wg) {
+  if (wg == 0) named_bar_sync(2, 128);
+  else named_bar_sync(3, 128);
+}
+struct EpiGegluFrag {
+  using Params = EpiGegluParams;
+  static constexpr bool FRAG = true;
+  static constexpr int EPI_WARPS = 8;                   // two MMA warpgroups, one 64-row half each
+  static constexpr bool WIDE_REGS = false;
+  static constexpr int STAGE_FLOATS = 32 * 32;          // 8 warps x 4 KB = two 16 KB output tiles
+  static constexpr int HALF = 128;
+  // d: this thread's m64n256 fragment of the warpgroup's rows m0 + 64 wg ..; tile: the warpgroup's 16 KB output tile (1024-byte aligned)
+  static __device__ __forceinline__ void frag(const Params& ep, const CUtensorMap* out, float (&d)[128], uint8_t* tile, int m0, int n0, int wg, int lg,
+                                              int lane) {
+    const int q = lane & 3;
+    const int r0 = 16 * lg + (lane >> 2);   // row of registers 4i, 4i + 1; registers 4i + 2, 4i + 3 hold row r0 + 8 (same swizzle phase)
+    const float2* bh = reinterpret_cast<const float2*>(ep.bias + n0) + q;
+    const float2* bg = reinterpret_cast<const float2*>(ep.bias + n0 + HALF) + q;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {   // output columns 8i + 2q, 8i + 2q + 1: box i / 8, 16-byte chunk i % 8 of the box row
+      const float2 b_h = __ldg(bh + 4 * i), b_g = __ldg(bg + 4 * i);
+      const uint32_t lo = pack_bf16(geglu_fast(d[4 * i] + b_h.x, d[64 + 4 * i] + b_g.x), geglu_fast(d[4 * i + 1] + b_h.y, d[64 + 4 * i + 1] + b_g.y));
+      const uint32_t hi = pack_bf16(geglu_fast(d[4 * i + 2] + b_h.x, d[64 + 4 * i + 2] + b_g.x), geglu_fast(d[4 * i + 3] + b_h.y, d[64 + 4 * i + 3] + b_g.y));
+      uint8_t* p = tile + (i >> 3) * 8192 + r0 * 128 + (((i & 7) ^ (r0 & 7)) << 4) + 4 * q;
+      *reinterpret_cast<uint32_t*>(p) = lo;
+      *reinterpret_cast<uint32_t*>(p + 8 * 128) = hi;
+    }
+    fence_proxy_async_smem();        // the generic writes above, before the TMA engine reads the tile
+    warpgroup_bar_sync(wg);
+    if ((threadIdx.x & 127) == 0) {
+      tma_store_2d(out, tile, n0 / 2, m0 + 64 * wg);
+      tma_store_2d(out, tile + 8192, n0 / 2 + 64, m0 + 64 * wg);
+      bulk_commit_group();
+    }
+  }
+};
+// Epilogues that run on the register fragment declare FRAG = true; the others (no FRAG member) use the parked-tile schedule.  A FRAG epilogue
+// may hand its warpgroup's tile to bulk async stores issued by the warpgroup's thread 0: gemm_body has that thread wait until they have
+// read it before the next frag() call (then a warpgroup barrier), and until they are complete before the CTA exits.
+template <class E>
+constexpr auto epi_frag_impl(int) -> decltype(E::FRAG) { return E::FRAG; }
+template <class E>
+constexpr bool epi_frag_impl(long) { return false; }
+template <class E>
+constexpr bool epi_frag() { return epi_frag_impl<E>(0); }
+
 // ---------------------------------------------------------------------------------------------------------------
 // Transposed ("swap-AB") linear epilogue.  For N_out = 1152-wide layers the natural 128/144-column tiles spend more operand
 // bytes per flop and a 256-column tile does not divide 1152.  Computing C^T = W A^T instead puts the 1152 output features on the
@@ -641,38 +700,38 @@ struct GemmCfg {
   // setmaxnreg.inc waits for free registers: the split must not ask for more than the launch allocated
   static_assert(!PRODUCER_WG || (EPI_WARPS == 8 && 128 * REGS_PRODUCER + 32 * EPI_WARPS * REGS_CONSUMER <= THREADS * REGS_LAUNCH &&
                                  REGS_CONSUMER >= 224), "register split");
+  static constexpr int NH = BN > 256 ? 2 : 1;   // wgmma N stops at 256: a wider tile is issued as two halves, HN columns each
+  static constexpr int HN = BN / NH;
+  // FRAG (epi_frag): the epilogue runs on the accumulator registers, the ring never holds the tile
+  static constexpr bool FRAG = epi_frag<Epi>();
   static constexpr int ACC_PITCH = BN + 4;
-  static constexpr int ACC_BYTES = GEMM_BM * ACC_PITCH * 4;
+  static constexpr int ACC_BYTES = FRAG ? 0 : GEMM_BM * ACC_PITCH * 4;
   static constexpr int STAGE_BYTES = EPI_WARPS * Epi::STAGE_FLOATS * 4;   // one transpose tile per epilogue warp
   static constexpr int FIT = (GEMM_SMEM_BUDGET - STAGE_BYTES) / (A_BYTES + B_BYTES);
   static constexpr int STAGES = FIT > 8 ? 8 : FIT;
   static constexpr int RING = STAGES * (A_BYTES + B_BYTES) > ACC_BYTES ? STAGES * (A_BYTES + B_BYTES) : ACC_BYTES;
+  static_assert(!FRAG || (RING % 1024 == 0 && MMA_WG == 2 && NH == 1), "FRAG: 1024-byte aligned output tiles, one 64-row half per warpgroup");
   static constexpr int BYTES = 1024 /*align slack*/ + RING + STAGE_BYTES + (2 * STAGES + 1) * 8;
   static_assert(STAGES >= 2, "smem budget");
   static_assert(BYTES <= 227 * 1024, "smem budget");
 };
 
-// One consumer warpgroup's share of a tile: all BN accumulator columns of NSUB 64-row halves from 64-row block row64.  Runs the
-// k-loop (slot s is released once wgmma.wait_group shows its MMAs complete, while slot s + 1's are in flight), then, after every warpgroup's
-// MMAs have completed, writes its fragments into the accumulator tile in shared memory.
-// FP8: the ring slots hold 128-element e4m3 k-blocks (the same 128-byte rows), issued as four k32 MMAs at the bf16 descriptor steps; the
-// accumulator is dequantised with the scales of global rows m0 + .. (< M) and columns n0 + .. on its way to shared memory.
+// One consumer warpgroup's k-loop over a tile: all BN accumulator columns of NSUB 64-row halves from 64-row block row64 (slot s is released
+// once wgmma.wait_group shows its MMAs complete, while slot s + 1's are in flight).  Returns with every MMA of this warpgroup complete.
+// FP8: the ring slots hold 128-element e4m3 k-blocks (the same 128-byte rows), issued as four k32 MMAs at the bf16 descriptor steps.
 template <int BN, class Epi, int MC, int KSUB, bool FP8 = false>
-__device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
-                                              int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane, const Fp8Scales& fs = Fp8Scales{},
-                                              int m0 = 0, int M = 0, int n0 = 0) {
+__device__ __forceinline__ void gemm_mainloop(float (&d)[GemmCfg<BN, Epi, KSUB>::NSUB][GemmCfg<BN, Epi, KSUB>::NH][GemmCfg<BN, Epi, KSUB>::HN / 2],
+                                              int row64, const uint8_t* sA, const uint8_t* sB, uint64_t* full, uint64_t* empty, int num_k_blocks,
+                                              uint32_t& stage, uint32_t& phase) {
   using SM = GemmCfg<BN, Epi, KSUB>;
-  constexpr int NSUB = SM::NSUB;
+  constexpr int NSUB = SM::NSUB, NH = SM::NH, HN = SM::HN;
   auto release = [&](uint32_t s) {   // one thread per warpgroup, on the slot's barrier in every CTA of the cluster
     if ((threadIdx.x & 127) == 0) {
       if (MC == 1) mbar_arrive(&empty[s]);
       else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
     }
   };
-  constexpr int NH = BN > 256 ? 2 : 1;   // wgmma N stops at 256: a wider tile is issued as two halves, HN columns each
-  constexpr int HN = BN / NH;
   static_assert(HN <= 256 && HN % 8 == 0, "BN");   // HN % 8: the second half starts on a 1024-byte swizzle atom
-  float d[NSUB][NH][HN / 2];
   uint32_t prev = 0;
   for (int kb = 0; kb < num_k_blocks; kb += KSUB) {
     mbar_wait(&full[stage], phase);
@@ -704,6 +763,19 @@ __device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, cons
   for (int s = 0; s < NSUB; ++s)
 #pragma unroll
     for (int h = 0; h < NH; ++h) wgmma_fence_regs(d[s][h]);
+}
+
+// Parked-tile schedule: the k-loop, then, after every warpgroup's MMAs have completed, the fragments written into the accumulator tile in
+// shared memory (over the ring).  FP8: the accumulator is dequantised with the scales of global rows m0 + .. (< M) and columns n0 + .. on its
+// way to shared memory.
+template <int BN, class Epi, int MC, int KSUB, bool FP8 = false>
+__device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
+                                              int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane, const Fp8Scales& fs = Fp8Scales{},
+                                              int m0 = 0, int M = 0, int n0 = 0) {
+  using SM = GemmCfg<BN, Epi, KSUB>;
+  constexpr int NSUB = SM::NSUB, NH = SM::NH, HN = SM::HN;
+  float d[NSUB][NH][HN / 2];
+  gemm_mainloop<BN, Epi, MC, KSUB, FP8>(d, row64, sA, sB, full, empty, num_k_blocks, stage, phase);
   named_bar_sync(1, 32 * SM::EPI_WARPS);   // every MMA of the tile has completed: the ring may now hold the accumulator
   // m64nN fragment: register 4i + {0,1} -> row 16 * (warp % 4) + lane / 4, columns 8i + 2 (lane % 4) + {0,1}; 4i + {2,3} -> row + 8
   if constexpr (FP8) {
@@ -742,7 +814,8 @@ __device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, cons
 // The N-side operand tile (BN rows x 64 columns) is then fetched ONCE per cluster: tmB is a map with SUBROWS-row boxes, CTA rank r issues
 // the sub-boxes j = r, r + MC, ... with .multicast::cluster, every CTA still expects the full A + B bytes on its own `full` barrier, a
 // stage is free again only when the MMA warpgroups of all MC CTAs have released it (`empty` counts their arrivals), and the ring is
-// refilled for the next tile only when every CTA of the cluster has finished reading its accumulator out of it (`acc_free`).
+// refilled for the next tile only when every CTA of the cluster has finished reading its accumulator out of it (`acc_free`; parked-tile
+// schedule only: a FRAG epilogue never puts the accumulator in the ring).
 // FIRST_PHASE: another GEMM phase follows in the same kernel (mlp_fused_kernel): the barriers are invalidated at the end so that the next
 // phase may lay out its own in the same shared memory.
 template <int BN>
@@ -754,7 +827,7 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, int KSUB = 1, bool FP8 = false>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw,
-                                          const Fp8Scales& fs = Fp8Scales{}) {
+                                          const Fp8Scales& fs = Fp8Scales{}, const CUtensorMap* tmC = nullptr) {
   using SM = GemmCfg<BN, Epi, KSUB>;
   constexpr int KB_ELEMS = FP8 ? 2 * GEMM_BK : GEMM_BK;   // elements per 128-byte k-block row
   // BN > 256: two TMA boxes and two wgmma halves per warpgroup, single CTA, one 64-row half per MMA warpgroup (the 288-token swap-AB tile)
@@ -807,7 +880,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     for (int tile = warp == PRODUCER ? (int)blockIdx.x : num_tiles; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
       const int n0 = nt * BN;
-      if (!first) { mbar_wait(acc_free, af_phase); af_phase ^= 1; }   // the ring held the previous tile's accumulator
+      // parked-tile schedule: the ring held the previous tile's accumulator.  FRAG: the producer runs ahead into the next tile, limited by
+      // `empty` alone (which counts the releases of every MMA warpgroup of the cluster before a slot is multicast into again).
+      if (!SM::FRAG && !first) { mbar_wait(acc_free, af_phase); af_phase ^= 1; }
       first = false;
       for (int kb0 = 0; kb0 < g.num_k_blocks; kb0 += KSUB) {
         EZB_DBG(const long long tq = clock64();)
@@ -854,6 +929,25 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     if constexpr (SM::PRODUCER_WG) setmaxnreg_inc<SM::REGS_CONSUMER>();
     const int wg = warp >> 2, lg = warp & 3;
     uint32_t stage = 0, phase = 0;
+    if constexpr (SM::FRAG) {
+      // Overlapped schedule: mainloop, then the epilogue on this warpgroup's registers, then straight into the next tile, whose first k-blocks
+      // the producer has already loaded.  Counters: [0] mainloop, [1] wait for the output tile's previous store, [4] epilogue.
+      static_assert(!FP8 && !FIRST_PHASE && KSUB == 1, "FRAG: bf16 kernels of one phase (gemm_frag_kernel)");
+      uint8_t* tile_buf = reinterpret_cast<uint8_t*>(sStage) + wg * (SM::STAGE_BYTES / 2);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
+        EZB_DBG(const long long tm = clock64();)
+        float d[NSUB][SM::NH][SM::HN / 2];
+        gemm_mainloop<BN, Epi, MC, KSUB>(d, wg * NSUB, sA, sB, full, empty, g.num_k_blocks, stage, phase);
+        EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
+        if ((threadIdx.x & 127) == 0) bulk_wait_group_read<0>();   // the previous tile's store has left this warpgroup's output tile
+        warpgroup_bar_sync(wg);
+        EZB_DBG(const long long te = clock64(); w1 += te - ta;)
+        Epi::frag(ep, tmC, d[0][0], tile_buf, mt * GEMM_BM, nt * BN, wg, lg, lane);
+        EZB_DBG(w4 += clock64() - te;)
+      }
+      if ((threadIdx.x & 127) == 0) bulk_wait_group<0>();
+    } else
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
       EZB_DBG(const long long tm = clock64();)
@@ -906,6 +1000,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const typename Epi::Params ep) {
   extern __shared__ uint8_t smem_dyn[];
   gemm_body<BN, Epi, MC, false, KSUB>(tmA, tmB, g, ep, smem_dyn);
+}
+// gemm_wgmma_kernel<BN, Epi, 2> for an epilogue on the register fragment (epi_frag): tmC is the map its output stores go through.
+template <int BN, class Epi>
+__global__ void __launch_bounds__((GemmCfg<BN, Epi>::THREADS), 1)
+gemm_frag_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
+                 const GemmShape g, const typename Epi::Params ep) {
+  extern __shared__ uint8_t smem_dyn[];
+  gemm_body<BN, Epi, 2>(tmA, tmB, g, ep, smem_dyn, Fp8Scales{}, &tmC);
 }
 // FP8 twin of gemm_wgmma_kernel<BN, Epi, 2> (2-CTA clusters, W tile multicast): A [M, K] and W [N, K] e4m3 through UINT8 tensor maps with
 // 128-element k-blocks (num_k_blocks = K / 128), dequantised by the per-row scales fs (see Fp8Scales).

@@ -359,9 +359,9 @@ int gemm_swapped_at(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int ld
   return launch_gemm_t<BN, Epi>(dev, st, tA, tB, g, ep);
 }
 
-// Token width of the swap-AB tiles, from the compiled set {256, 288}.  The grid is one persistent CTA per SM and the epilogue does not overlap
-// the next tile, so a launch lasts about ceil(tiles / SMs) tile times, and a tile's time grows with its width: take the width with the smaller
-// ceil(tiles / SMs) x width, 256 on a tie.  On 132 SMs with 1152 features (9 feature tiles): 4000 tokens -> 288 (126 tiles in one wave instead
+// Token width of the swap-AB tiles, from the compiled set {256, 288}.  The grid is one persistent CTA per SM and these tiles keep the parked-tile
+// schedule, whose epilogue does not overlap the next tile, so a launch lasts about ceil(tiles / SMs) tile times, and a tile's time grows with its
+// width: take the width with the smaller ceil(tiles / SMs) x width, 256 on a tie.  On 132 SMs with 1152 features (9 feature tiles): 4000 tokens -> 288 (126 tiles in one wave instead
 // of 144 in two), 8000 -> 288 (252 tiles in two waves instead of 288 in three), 6000 -> 256 (two waves either way); 1024 features at 4000
 // tokens -> 256 (128 tiles, one wave).
 inline int swapped_bn(const Device& dev, int M_tokens, int N_features) {
@@ -465,7 +465,18 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
   const CUtensorMap *tA, *tB;
   EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, GEMM_BM, &tA));
   EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, McSub<BN>::ROWS, &tB));
-  auto kern = gemm_wgmma_kernel<BN, Epi, 2, KSUB>;
+  // An epilogue on the register fragment (EpiGegluFrag, the overlapped schedule) stores bf16 [M, N / 2] through a tensor map of its output
+  constexpr bool FRAG = GemmCfg<BN, Epi, KSUB>::FRAG;
+  const CUtensorMap* tC = nullptr;
+  if constexpr (FRAG) {
+    if (ep.split_stride != 0 || ep.fin.u != nullptr || N % BN)
+      return fail(EZB_ERR_ARG, "gemm2: the fragment GEGLU epilogue writes plain bf16 of whole %d-column tiles (N %d)", BN, N);
+    EZB_TRY(dev.tmaps.get2d(ep.out_bf16, (uint64_t)N / 2, (uint64_t)M, (uint64_t)ep.ld16, 64, &tC));
+  }
+  auto kern = [] {
+    if constexpr (FRAG) return gemm_frag_kernel<BN, Epi>;
+    else return gemm_wgmma_kernel<BN, Epi, 2, KSUB>;
+  }();
   constexpr int smem = GemmCfg<BN, Epi, KSUB>::BYTES;
   constexpr int GEMM_THREADS = GemmCfg<BN, Epi, KSUB>::THREADS;
   static int clusters[16] = {};
@@ -486,9 +497,21 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
     gp.flops.push_back(2.0 * (double)M * (double)N * (double)g.num_k_blocks * GEMM_BK);
     EZB_CUDA(cudaEventRecord(e0, st));
   }
-  EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, g, ep));
+  if constexpr (FRAG) EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, *tC, g, ep));
+  else EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, g, ep));
   if (gp.on) EZB_CUDA(cudaEventRecord(e1, st));
   return EZB_OK;
+}
+
+// The 256-wide cluster GEGLU GEMM without a LayerNorm fold (p.fin unset).  The plain bf16 epilogue runs on the register fragment, so the
+// epilogue of one tile overlaps the TMA loads of the next (EpiGegluFrag).  Its TMA stores need a 16-byte aligned output with a row pitch of a
+// multiple of 8 elements; outputs that only meet the parked epilogue's 8-byte alignment, and the bf16x3 split (p.split_stride > 0), keep the
+// parked tile.
+inline int gemm2_geglu(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
+                       const EpiGegluParams& p) {
+  const bool tma_out = (reinterpret_cast<uintptr_t>(p.out_bf16) & 15) == 0 && p.ld16 % 8 == 0;
+  if (p.split_stride == 0 && N % 256 == 0 && tma_out) return gemm2<256, EpiGegluFrag>(dev, st, A, lda, W, ldw, M, N, K, p);
+  return gemm2<256, EpiGeglu<256>>(dev, st, A, lda, W, ldw, M, N, K, p);
 }
 
 // FP8 twin of gemm2 (gemm.cuh gemm_fp8_kernel): A [M, K] and W [N, K] e4m3 (row pitch K bytes), per-row scales sa [M], sw [N].
