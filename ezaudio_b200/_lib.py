@@ -64,6 +64,17 @@ class TestFp8Args(C.Structure):
                [(n, C.c_void_p) for n in ("w_q", "w_s")]
 
 
+class TestStepArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "variant", "M", "D1", "D2", "kmul", "mod_bstride", "rows_per_batch", "B", "L", "C", "Kp",
+                                         "H", "dh", "nsec", "in_bf16")] + \
+               [("kinds", C.c_int32 * 3), ("col_off", C.c_int32 * 3)] + \
+               [(n, C.c_int32) for n in ("ld_in", "ld_qk", "Lpad", "dv_pad", "R", "N", "K", "ld_add", "ld_out", "act")] + \
+               [("out_scale", C.c_float)] + \
+               [(n, C.c_void_p) for n in ("x", "x2", "x3", "w", "b", "shift", "scale", "G", "Cc", "gt", "gt_mask", "mask_embed", "add", "lens",
+                                          "norm_q", "norm_k", "inv_freq", "out")] + \
+               [("f32_out", C.c_void_p * 3), ("bf_out", C.c_void_p * 3)]
+
+
 _lib = None
 
 _VP, _I, _F = C.c_void_p, C.c_int, C.c_float
@@ -99,6 +110,7 @@ _SIGS = {
     "ezb_debug_read": ([C.POINTER(C.c_ulonglong)], _I),
     "ezb_launch_count": ([], C.c_ulonglong),
     "ezb_launch_count_add": ([C.c_ulonglong], None),
+    "ezb_ln_launch_count": ([_I], C.c_ulonglong),
     "ezb_prof_gemm_begin": ([], _I),
     "ezb_prof_gemm_end": ([C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
     "ezb_prof_gemm_stats": ([C.c_double, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
@@ -109,6 +121,7 @@ _SIGS = {
     "ezb_test_mlp": ([_I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP], _I),
     "ezb_test_vae": ([_I, C.POINTER(TestVaeArgs), _VP], _I),
     "ezb_test_fp8": ([_I, C.POINTER(TestFp8Args), _VP], _I),
+    "ezb_test_step": ([_I, C.POINTER(TestStepArgs), _VP], _I),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -46,6 +46,86 @@ struct WeightSpec {
 
 constexpr int KP_PATCH_ALIGN = 8;
 
+// ---------------------------------------------------------------- launches of the step's bandwidth kernels (elementwise.cuh)
+// Shared by Dit and the kernel-level test hook (ezb_test_step), so that a test runs exactly the launch the model makes.
+// LayerNorm kernel: LN_AUTO = what option "ln_variant" selects for these parameters; the others force one kernel, which the caller has
+// checked can take them.
+enum LnVariant { LN_AUTO = 0, LN_GENERIC = 1, LN_REG1 = 2, LN_REG8 = 3, LN_GC = 4, LN_CAT = 5 };
+inline int ln_select(const LnParams& p) {
+  if (p.kmul == 1 && p.x2 == nullptr && p.w != nullptr && (p.D1 == 1152 || p.D1 == 1024)) {
+    if (opt_ln_variant() == 2 && p.G != nullptr && (p.shift == nullptr || p.mod_bstride == 0)) return LN_GC;
+    return opt_ln_variant() == 1 ? LN_REG8 : LN_REG1;
+  }
+  if (p.kmul == 1 && opt_ln_variant() == 2 && p.x2 != nullptr && p.w != nullptr && p.shift == nullptr && p.D1 == p.D2 && (p.D1 == 1152 || p.D1 == 1024))
+    return LN_CAT;
+  return LN_GENERIC;
+}
+// launches per LayerNorm kernel (indexed by LnVariant) since the library was loaded, process-wide: ezb_ln_launch_count
+inline unsigned long long* ln_launch_counts() {
+  static unsigned long long n[LN_CAT + 1] = {};
+  return n;
+}
+inline int ln_launch(const Device& dev, cudaStream_t st, const LnParams& p, int variant = LN_AUTO) {
+  const int M = p.M;
+  const bool d9 = p.D1 == 1152;
+  if (variant == LN_AUTO) variant = ln_select(p);
+  ++ln_launch_counts()[variant];
+  switch (variant) {
+    case LN_GC: {   // warps walk rows in a strided loop: at most 4 CTAs per SM
+      const int grid = dev.num_sms * 4 < (M + 3) / 4 ? dev.num_sms * 4 : (M + 3) / 4;
+      if (d9) return launch_k(ln_gc_kernel<9>, dim3(grid), dim3(128), 0, st, 1, p);
+      return launch_k(ln_gc_kernel<8>, dim3(grid), dim3(128), 0, st, 1, p);
+    }
+    case LN_REG8:
+      if (d9) return launch_k(ln_mod_cast_reg_kernel<9, 8>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
+      return launch_k(ln_mod_cast_reg_kernel<8, 8>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
+    case LN_REG1:
+      if (d9) return launch_k(ln_mod_cast_reg_kernel<9, 1>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
+      return launch_k(ln_mod_cast_reg_kernel<8, 1>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
+    case LN_CAT:
+      if (d9) return launch_k(ln_cat_reg_kernel<9>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
+      return launch_k(ln_cat_reg_kernel<8>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
+    default:
+      return launch_k(ln_mod_cast_kernel, dim3((M + 7) / 8), dim3(256), 0, st, 1, p);
+  }
+}
+template <typename TIn>
+inline int qk_prep_launch(cudaStream_t st, const QkPrepParams<TIn>& p) {   // one warp per (token, section, head)
+  const int total = p.B * p.L * p.H * p.n_sections;
+  ++launch_counter();
+  qk_prep_kernel<TIn><<<(total + 7) / 8, 256, 0, st>>>(p);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int patch_pack_launch(cudaStream_t st, const float* x, const float* gt, const uint8_t* gt_mask, const float* mask_embed, bf16* out, int B, int C, int L,
+                             int Kp, int kmul) {
+  if ((2 * C) % 32) return fail(EZB_ERR_UNSUPPORTED, "latent_chans must be a multiple of 16");
+  dim3 grid((L + 31) / 32, (2 * C) / 32, B), blockd(32, 8);
+  return launch_k(patch_pack_kernel, grid, blockd, 0, st, 1, x, gt, gt_mask, mask_embed, out, B, C, L, Kp, kmul);
+}
+inline int final_conv_launch(const Device& dev, cudaStream_t st, const float* y, const float* wp, const float* bias, float* out, int B, int C, int L,
+                             const int32_t* lens) {
+  if (C % 4) return fail(EZB_ERR_UNSUPPORTED, "final conv: %d channels (multiple of 4 expected)", C);
+  const size_t smem = ((size_t)36 * C + (size_t)(FC_GROUPS - 1) * 128 * 32) * sizeof(float);
+  static bool fc_attr[16] = {};   // function attributes are per device
+  if (!fc_attr[dev.id & 15]) { EZB_CUDA(cudaFuncSetAttribute(final_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); fc_attr[dev.id & 15] = true; }
+  if (smem > 160 * 1024) return fail(EZB_ERR_UNSUPPORTED, "final conv: %d channels exceed the shared-memory tile", C);
+  return launch_k(final_conv_kernel, dim3((L + 31) / 32, B), dim3(128 * FC_GROUPS), smem, st, 1, y, wp, bias, out, B, C, L, lens);
+}
+inline int small_linear_launch(cudaStream_t st, const float* in, int ld_in, const float* W, const float* bias, const float* add, int ld_add, float* out, int ld_out,
+                               int R, int N, int K, int act, float scale) {   // one warp per output feature
+  ++launch_counter();
+  small_linear_kernel<<<(N + 7) / 8, 256, 0, st>>>(in, ld_in, W, bias, add, ld_add, out, ld_out, R, N, K, act, scale);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int timestep_embed_launch(cudaStream_t st, const float* t, float* out, int n) {
+  ++launch_counter();
+  timestep_embed_kernel<<<(n * 128 + 255) / 256, 256, 0, st>>>(t, out, n);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+
 struct FoldCtx {
   bool on = false;
   int t = 0;                  // timestep index (uniform over the batch)
@@ -527,25 +607,7 @@ struct Dit {
   }
   int ln(cudaStream_t st, const LnParams& p) {
     if (opt_skip() & 1) return EZB_OK;
-    const int M = p.M;
-    if (kmul == 1 && p.x2 == nullptr && p.w != nullptr && (p.D1 == 1152 || p.D1 == 1024)) {
-      if (opt_ln_variant() == 2 && p.G != nullptr && (p.shift == nullptr || p.mod_bstride == 0)) {
-        const int grid = dev->num_sms * 4 < (M + 3) / 4 ? dev->num_sms * 4 : (M + 3) / 4;
-        if (p.D1 == 1152) return launch_k(ln_gc_kernel<9>, dim3(grid), dim3(128), 0, st, 1, p);
-        return launch_k(ln_gc_kernel<8>, dim3(grid), dim3(128), 0, st, 1, p);
-      }
-      if (opt_ln_variant() == 1) {
-        if (p.D1 == 1152) return launch_k(ln_mod_cast_reg_kernel<9, 8>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
-        return launch_k(ln_mod_cast_reg_kernel<8, 8>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
-      }
-      if (p.D1 == 1152) return launch_k(ln_mod_cast_reg_kernel<9, 1>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
-      return launch_k(ln_mod_cast_reg_kernel<8, 1>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
-    }
-    if (kmul == 1 && opt_ln_variant() == 2 && p.x2 != nullptr && p.w != nullptr && p.shift == nullptr && p.D1 == p.D2 && (p.D1 == 1152 || p.D1 == 1024)) {
-      if (p.D1 == 1152) return launch_k(ln_cat_reg_kernel<9>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
-      return launch_k(ln_cat_reg_kernel<8>, dim3((M + 3) / 4), dim3(128), 0, st, 1, p);
-    }
-    return launch_k(ln_mod_cast_kernel, dim3((M + 7) / 8), dim3(256), 0, st, 1, p);
+    return ln_launch(*dev, st, p);   // p.kmul == kmul (ln_params)
   }
   // FP8 mode: LayerNorm (+ modulate) of p.x to e4m3 act8 with row scales act8_s (p.out is not written)
   int ln8(cudaStream_t st, const LnParams& p) {
@@ -599,15 +661,11 @@ struct Dit {
   }
   int small_lin(cudaStream_t st, const float* in, int ld_in, const float* W, const float* bias, const float* add, int ld_add, float* out, int ld_out, int R,
                 int N, int K, int act, float scale) {
-    ++launch_counter();
-    small_linear_kernel<<<(N + 7) / 8, 256, 0, st>>>(in, ld_in, W, bias, add, ld_add, out, ld_out, R, N, K, act, scale);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    return small_linear_launch(st, in, ld_in, W, bias, add, ld_add, out, ld_out, R, N, K, act, scale);
   }
   // head layout for attention from a GEMM output holding `nsec` sections
   int qk_prep(cudaStream_t st, int ld_in, int nsec, const int* col_off, const int* kinds, const float* nqw_, const float* nqb_, const float* nkw_,
               const float* nkb_, const float* inv_freq, int B, int L, float* const* f32o, bf16* const* bfo, int Lpad) {
-    const int total = B * L * H * nsec;
     auto fill = [&](auto& p) {
       p.ld_in = ld_in; p.n_sections = nsec;
       for (int i = 0; i < 3; ++i) { p.col_off[i] = i < nsec ? col_off[i] : 0; p.sec_kind[i] = i < nsec ? kinds[i] : 0; p.f32_out[i] = i < nsec ? f32o[i] : nullptr; p.bf_out[i] = i < nsec ? bfo[i] : nullptr; }
@@ -616,15 +674,10 @@ struct Dit {
     };
     if (kmul == 3) {
       QkPrepParams<float> p; p.in = reinterpret_cast<const float*>(qkv); fill(p);
-      ++launch_counter();
-      qk_prep_kernel<float><<<(total + 7) / 8, 256, 0, st>>>(p);
-    } else {
-      QkPrepParams<bf16> p; p.in = reinterpret_cast<const bf16*>(qkv); fill(p);
-      ++launch_counter();
-      qk_prep_kernel<bf16><<<(total + 7) / 8, 256, 0, st>>>(p);
+      return qk_prep_launch(st, p);
     }
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    QkPrepParams<bf16> p; p.in = reinterpret_cast<const bf16*>(qkv); fill(p);
+    return qk_prep_launch(st, p);
   }
   // Q/K/V projection with the fused per-head LN + RoPE + attention-layout epilogue (fast mode)
   EpiHeadsParams heads_params(int N, const int* kinds, const float (*nq)[96], const float (*nk)[96], bool rope, int L, bf16* qo, bf16* ko, bf16* vto,
@@ -735,8 +788,7 @@ struct Dit {
       ++launch_counter();
       fill_timesteps_kernel<<<1, 256, 0, st>>>(t_vals + i0, c, m);
     }
-    ++launch_counter();
-    timestep_embed_kernel<<<(n * 128 + 255) / 256, 256, 0, st>>>(t_vals, t_emb, n);
+    EZB_TRY(timestep_embed_launch(st, t_vals, t_emb, n));
     EZB_TRY(small_lin(st, t_emb, 256, te_w0, te_b0, nullptr, 0, t_h, D, n, D, 256, 1, 1.f));
     EZB_TRY(small_lin(st, t_h, D, te_w2, te_b2, nullptr, 0, t_tok, D, n, D, D, 1, 1.f));  // time_act SiLU folded (udit.py:313)
     EZB_TRY(small_lin(st, t_tok, D, ta_w, ta_b, nullptr, 0, t_ada, 6 * D, n, 6 * D, D, 0, 1.f));
@@ -915,9 +967,7 @@ struct Dit {
 
   int embed(cudaStream_t st, const float* x, const float* gt, const uint8_t* gt_mask, const float* resid, int Be, int L, const FoldCtx& fc = FoldCtx(),
             const LnParams* next_ln = nullptr, bool* next_done = nullptr) {
-    dim3 grid((L + 31) / 32, (2 * C) / 32, Be), blockd(32, 8);
-    if ((2 * C) % 32) return fail(EZB_ERR_UNSUPPORTED, "latent_chans must be a multiple of 16");
-    EZB_TRY(launch_k(patch_pack_kernel, grid, blockd, 0, st, 1, x, gt, gt_mask, (const float*)mask_embed, a_patch, Be, C, L, Kp, kmul));
+    EZB_TRY(patch_pack_launch(st, x, gt, gt_mask, mask_embed, a_patch, Be, C, L, Kp, kmul));
     EpiLinearParams e = epi();
     e.bias = b_patch; e.out_f32 = x0; e.ld32 = D; e.resid = resid; e.ldr = D;
     if (fc.on) e.fout = fold_out(st_x0, act, D, blk[0].g1 + (size_t)fc.t * D);
@@ -1002,13 +1052,7 @@ struct Dit {
     e.bias = b_final; e.out_f32 = ybuf; e.ld32 = C;
     if (fc.on) e.fin = fold_in(fc.st_x, nullptr, D, uF + (size_t)fc.t * C, vF + (size_t)fc.t * C);
     EZB_TRY(lin(st, act, D, w_final, M, C, e));
-    dim3 grid((L + 31) / 32, Be);
-    if (C % 4) return fail(EZB_ERR_UNSUPPORTED, "final conv: %d channels (multiple of 4 expected)", C);
-    const size_t smem = ((size_t)36 * C + (size_t)(FC_GROUPS - 1) * 128 * 32) * sizeof(float);
-    static bool fc_attr[16] = {};   // function attributes are per device
-    if (!fc_attr[dev->id & 15]) { EZB_CUDA(cudaFuncSetAttribute(final_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); fc_attr[dev->id & 15] = true; }
-    if (smem > 160 * 1024) return fail(EZB_ERR_UNSUPPORTED, "final conv: %d channels exceed the shared-memory tile", C);
-    EZB_TRY(launch_k(final_conv_kernel, grid, dim3(128 * FC_GROUPS), smem, st, 1, (const float*)ybuf, (const float*)fc_w, (const float*)fc_b, out, Be, C, L, lens));
+    EZB_TRY(final_conv_launch(*dev, st, ybuf, fc_w, fc_b, out, Be, C, L, lens));
     ws.ok = true;
     return EZB_OK;
   }

@@ -397,6 +397,133 @@ __attribute__((visibility("default"))) int ezb_test_fp8(int device, const ezb_te
   EZB_CUDA(cudaFreeAsync(bp, st));
   return rc;
 }
+}  // extern "C"
+
+namespace {
+// can LayerNorm kernel `variant` (LnVariant) take these parameters?
+bool ln_variant_fits(const LnParams& p, int variant) {
+  const bool reg_width = p.D1 == 1152 || p.D1 == 1024;
+  switch (variant) {
+    case LN_AUTO: case LN_GENERIC: return true;
+    case LN_REG1: case LN_REG8: return p.kmul == 1 && !p.x2 && p.w && reg_width;
+    case LN_GC: return p.kmul == 1 && !p.x2 && p.G && reg_width;
+    case LN_CAT: return p.kmul == 1 && p.x2 && p.w && !p.shift && p.D2 == p.D1 && reg_width;
+  }
+  return false;
+}
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+int test_step_check(const ezb_test_step_args* a) {
+  const int kind = a->kind;
+  if (kind < 0 || kind > 5) return fail(EZB_ERR_ARG, "ezb_test_step: kind %d", kind);
+  if (!a->x || !a->out) return fail(EZB_ERR_ARG, "ezb_test_step: null input or output");
+  if (kind == 0) {
+    if (a->M < 1 || a->M > (1 << 26)) return fail(EZB_ERR_SHAPE, "ezb_test_step: LayerNorm over %d rows", a->M);
+    if (a->kmul != 1 && a->kmul != 3) return fail(EZB_ERR_ARG, "ezb_test_step: kmul %d (1 or 3)", a->kmul);
+    if (a->D1 < 4 || a->D1 % 4 || a->D2 < 0 || a->D2 % 4) return fail(EZB_ERR_SHAPE, "ezb_test_step: LayerNorm widths %d + %d (multiples of 4)", a->D1, a->D2);
+    if ((a->D2 > 0) != (a->x2 != nullptr) || (a->x3 && !a->x2)) return fail(EZB_ERR_ARG, "ezb_test_step: x2 must come with D2 > 0, x3 with x2");
+    if (!a->w != !a->b || !a->shift != !a->scale || !a->G != !a->Cc) return fail(EZB_ERR_ARG, "ezb_test_step: w / b, shift / scale and G / Cc come in pairs");
+    if (a->shift && (a->x2 || a->rows_per_batch < 1 || a->mod_bstride < 0))
+      return fail(EZB_ERR_ARG, "ezb_test_step: modulation needs one source, rows_per_batch >= 1 and mod_bstride >= 0");
+    if (a->G && (a->x2 || (a->D1 != 1152 && a->D1 != 1024))) return fail(EZB_ERR_ARG, "ezb_test_step: a precombined affine is for one source of 1024 or 1152");
+    if (a->variant < LN_AUTO || a->variant > LN_CAT) return fail(EZB_ERR_ARG, "ezb_test_step: LayerNorm variant %d", a->variant);
+    // the kernels read every input as float4 and the register variants store 8-byte groups of the output
+    const void* ps[] = {a->x, a->x2, a->x3, a->w, a->b, a->shift, a->scale, a->G, a->Cc, a->out};
+    for (const void* q : ps)
+      if (!aligned16(q)) return fail(EZB_ERR_ARG, "ezb_test_step: LayerNorm pointers must be 16-byte aligned");
+    if (a->shift && a->mod_bstride % 4) return fail(EZB_ERR_ARG, "ezb_test_step: mod_bstride %d (a multiple of 4)", a->mod_bstride);
+    return EZB_OK;
+  }
+  if (kind == 1) {
+    const int B = a->B, L = a->L, H = a->H, dh = a->dh, nsec = a->nsec;
+    if (B < 1 || L < 1 || H < 1 || dh < 2 || dh > 96 || dh % 2) return fail(EZB_ERR_SHAPE, "ezb_test_step: qk_prep B %d L %d H %d dh %d (even, <= 96)", B, L, H, dh);
+    if (nsec < 1 || nsec > 3 || (long long)B * L * H * nsec > (1 << 26)) return fail(EZB_ERR_SHAPE, "ezb_test_step: qk_prep %d sections", nsec);
+    if (a->in_bf16 != 0 && a->in_bf16 != 1) return fail(EZB_ERR_ARG, "ezb_test_step: in_bf16 %d", a->in_bf16);
+    for (int s = 0; s < nsec; ++s) {
+      const int kd = a->kinds[s];
+      if (kd < 0 || kd > 2) return fail(EZB_ERR_ARG, "ezb_test_step: section %d kind %d", s, kd);
+      if (a->col_off[s] < 0 || a->col_off[s] + H * dh > a->ld_in) return fail(EZB_ERR_SHAPE, "ezb_test_step: section %d at column %d past the row of %d", s, a->col_off[s], a->ld_in);
+      if ((kd == 0 && !a->norm_q) || (kd == 1 && !a->norm_k)) return fail(EZB_ERR_ARG, "ezb_test_step: section %d without its LayerNorm parameters", s);
+      if (!a->f32_out[s] && !a->bf_out[s]) return fail(EZB_ERR_ARG, "ezb_test_step: section %d has no output", s);
+      if (a->bf_out[s] && kd < 2 && a->ld_qk < dh) return fail(EZB_ERR_SHAPE, "ezb_test_step: q / k pitch %d < dh %d", a->ld_qk, dh);
+      if (a->bf_out[s] && kd == 2 && (a->Lpad < L || a->dv_pad < dh)) return fail(EZB_ERR_SHAPE, "ezb_test_step: V^T %d x %d for dh %d L %d", a->dv_pad, a->Lpad, dh, L);
+    }
+    return EZB_OK;
+  }
+  if (kind == 2) {
+    if (a->B < 1 || a->B > 65535 || a->L < 1 || a->C < 16 || a->C % 16 || a->Kp < 2 * a->C + 1) return fail(EZB_ERR_SHAPE, "ezb_test_step: patch_pack B %d C %d L %d Kp %d", a->B, a->C, a->L, a->Kp);
+    if (a->kmul != 1 && a->kmul != 3) return fail(EZB_ERR_ARG, "ezb_test_step: kmul %d (1 or 3)", a->kmul);
+    if (!a->mask_embed || (a->gt_mask && !a->gt)) return fail(EZB_ERR_ARG, "ezb_test_step: patch_pack needs mask_embed, a gt_mask needs gt");
+    return EZB_OK;
+  }
+  if (kind == 3) {
+    if (a->B < 1 || a->B > 65535 || a->L < 1 || a->C < 4 || a->C % 4 || a->C > 512) return fail(EZB_ERR_SHAPE, "ezb_test_step: final_conv B %d C %d L %d", a->B, a->C, a->L);
+    if (!a->w || !a->b) return fail(EZB_ERR_ARG, "ezb_test_step: final_conv needs w and b");
+    if (!aligned16(a->w) || !aligned16(a->b)) return fail(EZB_ERR_ARG, "ezb_test_step: final_conv reads w and b as float4 (16-byte aligned)");
+    return EZB_OK;
+  }
+  if (kind == 4) {
+    if (a->R < 1 || a->N < 1 || a->K < 1 || a->ld_in < a->K || a->ld_out < a->N || (a->add && a->ld_add < a->N))
+      return fail(EZB_ERR_SHAPE, "ezb_test_step: small_linear R %d N %d K %d pitches %d / %d / %d", a->R, a->N, a->K, a->ld_in, a->ld_add, a->ld_out);
+    if (!a->w || (a->act != 0 && a->act != 1)) return fail(EZB_ERR_ARG, "ezb_test_step: small_linear needs w; act %d (0 or 1)", a->act);
+    return EZB_OK;
+  }
+  if (a->M < 1 || a->M > (1 << 20)) return fail(EZB_ERR_SHAPE, "ezb_test_step: %d timesteps", a->M);
+  return EZB_OK;
+}
+// qk_prep parameters as Dit::qk_prep fills them (p.in set by the caller)
+template <typename Params>
+void test_qk_params(Params& p, const ezb_test_step_args* a) {
+  p.ld_in = a->ld_in; p.n_sections = a->nsec;
+  for (int s = 0; s < 3; ++s) {
+    p.col_off[s] = s < a->nsec ? a->col_off[s] : 0; p.sec_kind[s] = s < a->nsec ? a->kinds[s] : 0;
+    p.f32_out[s] = s < a->nsec ? a->f32_out[s] : nullptr; p.bf_out[s] = s < a->nsec ? static_cast<__nv_bfloat16*>(a->bf_out[s]) : nullptr;
+  }
+  if (a->norm_q) { p.nw[0] = a->norm_q; p.nb[0] = a->norm_q + a->dh; }
+  if (a->norm_k) { p.nw[1] = a->norm_k; p.nb[1] = a->norm_k + a->dh; }
+  p.use_rope = a->inv_freq != nullptr; p.inv_freq = a->inv_freq;
+  p.B = a->B; p.L = a->L; p.H = a->H; p.dh = a->dh; p.ld_qk = a->ld_qk; p.Lpad = a->Lpad; p.dv_pad = a->dv_pad;
+}
+}  // namespace
+
+extern "C" {
+
+__attribute__((visibility("default"))) int ezb_test_step(int device, const ezb_test_step_args* a, void* stream) {
+  if (!a) return fail(EZB_ERR_ARG, "ezb_test_step: null arguments");
+  EZB_TRY(test_step_check(a));
+  LnParams p;
+  memset(&p, 0, sizeof p);
+  if (a->kind == 0) {
+    p.x = static_cast<const float*>(a->x); p.x2 = a->x2; p.x3 = a->x3; p.D1 = a->D1; p.D2 = a->D2; p.w = a->w; p.b = a->b;
+    p.shift = a->shift; p.scale = a->scale; p.mod_bstride = a->mod_bstride; p.rows_per_batch = a->shift ? a->rows_per_batch : 1;
+    p.out = static_cast<__nv_bfloat16*>(a->out); p.kmul = a->kmul; p.M = a->M; p.G = a->G; p.C = a->Cc;
+    if (!ln_variant_fits(p, a->variant)) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_step: LayerNorm variant %d cannot take D1 %d D2 %d kmul %d", a->variant, a->D1, a->D2, a->kmul);
+  }
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const float* x = static_cast<const float*>(a->x);
+  switch (a->kind) {
+    case 0: return ln_launch(dev, st, p, a->variant);
+    case 1: {
+      if (a->in_bf16) {
+        QkPrepParams<__nv_bfloat16> q;
+        memset(&q, 0, sizeof q);
+        q.in = static_cast<const __nv_bfloat16*>(a->x);
+        test_qk_params(q, a);
+        return qk_prep_launch(st, q);
+      }
+      QkPrepParams<float> q;
+      memset(&q, 0, sizeof q);
+      q.in = x;
+      test_qk_params(q, a);
+      return qk_prep_launch(st, q);
+    }
+    case 2: return patch_pack_launch(st, x, a->gt, a->gt_mask, a->mask_embed, static_cast<__nv_bfloat16*>(a->out), a->B, a->C, a->L, a->Kp, a->kmul);
+    case 3: return final_conv_launch(dev, st, x, a->w, a->b, static_cast<float*>(a->out), a->B, a->C, a->L, a->lens);
+    case 4: return small_linear_launch(st, x, a->ld_in, a->w, a->b, a->add, a->ld_add, static_cast<float*>(a->out), a->ld_out, a->R, a->N, a->K, a->act, a->out_scale);
+    default: return timestep_embed_launch(st, x, static_cast<float*>(a->out), a->M);
+  }
+}
 
 #define EZB_API __attribute__((visibility("default")))
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
@@ -637,6 +764,7 @@ EZB_API int ezb_debug_read(unsigned long long* out8) {
 EZB_API unsigned long long ezb_launch_count(void) { return launch_counter(); }
 // kernels replayed through a captured CUDA graph never pass the launch helpers: the host layer reports them here
 EZB_API void ezb_launch_count_add(unsigned long long n) { launch_counter() += n; }
+EZB_API unsigned long long ezb_ln_launch_count(int variant) { return variant >= LN_GENERIC && variant <= LN_CAT ? ln_launch_counts()[variant] : 0; }
 EZB_API int ezb_prof_gemm_begin(void) {
   GemmProf& gp = gemm_prof();
   gp.on = true; gp.used = 0; gp.flops.clear();

@@ -251,6 +251,38 @@ typedef struct {
   void* w_q; float* w_s;
 } ezb_test_fp8_args;
 int ezb_test_fp8(int device, const ezb_test_fp8_args* args, void* stream);
+/* The bandwidth kernels of a DiT step (csrc/elementwise.cuh), launched with the grid and shared memory the model uses (csrc/dit.cuh
+   ln_launch and friends).  Device pointers; those of kind 0 and final_conv's w and b are read as float4 and must be 16-byte aligned
+   (kind 0: mod_bstride a multiple of 4).  Every argument, alignment included, is checked before any device work.
+   kind 0 LayerNorm (eps 1e-5) of the row [x | x2 (+ x3)] (x fp32 [M, D1], x2 / x3 optional fp32 [M, D2]) with affine w / b [D1 + D2]
+          (both NULL: cast only), optional AdaLN modulate y (1 + scale) + shift (shift / scale rows at (row / rows_per_batch) * mod_bstride,
+          single source only), optional precombined affine G / Cc [D1] (the ln_gc kernel: y = (x - mu) rstd G + Cc) -> out bf16
+          [M, kmul (D1 + D2)] ([hi | lo | hi] when kmul is 3).  variant: 0 the kernel Dit::ln selects under the current option "ln_variant";
+          1 generic, 2 / 3 register-resident with 1 / 8 CTAs per SM minimum, 4 precombined affine (G, Cc), 5 register-resident concat
+          (D1 == D2): 2-5 take D1 = 1024 or 1152 and kmul 1 only.
+   kind 1 per-head LayerNorm + RoPE + attention layout (qk_prep) of x [B*L, ld_in] (fp32, or bf16 when in_bf16): nsec sections of kinds
+          kinds[s] (0 q, 1 k, 2 v) at column offsets col_off[s]; norm_q / norm_k [2][dh] weight | bias; inv_freq [dh/2] (NULL: no RoPE);
+          f32_out[s] fp32 [B, H, L, dh] and / or bf_out[s] bf16 (q, k: [B, H, L, ld_qk]; v: V^T [B, H, dv_pad, Lpad], rows dh..dv_pad zeroed).
+   kind 2 patch_pack: x [B, C, L], gt [B, C, L] or NULL, gt_mask [B, L] uint8 or NULL, mask_embed [C] -> out bf16 [B*L, kmul Kp].
+   kind 3 final_conv: x = y fp32 [B*L, C], w [3][C][C] (tap, in, out), b [C], lens [B] or NULL -> out fp32 [B, C, L] (frames < lens[b]).
+   kind 4 small_linear: out[r, n] = act(out_scale (x[r, :] . w[n, :]) + b[n]) + add[r, n], r < R, n < N, over K; act 0 none, 1 SiLU; b and
+          add optional; row pitches ld_in, ld_add, ld_out.
+   kind 5 timestep_embed: x = t fp32 [M] -> out fp32 [M, 256] = [cos | sin]. */
+typedef struct {
+  int32_t kind, variant;
+  int32_t M, D1, D2, kmul, mod_bstride, rows_per_batch;
+  int32_t B, L, C, Kp, H, dh, nsec, in_bf16;
+  int32_t kinds[3], col_off[3];
+  int32_t ld_in, ld_qk, Lpad, dv_pad;
+  int32_t R, N, K, ld_add, ld_out, act;
+  float out_scale;
+  const void* x; const float* x2; const float* x3; const float* w; const float* b;
+  const float* shift; const float* scale; const float* G; const float* Cc;
+  const float* gt; const uint8_t* gt_mask; const float* mask_embed; const float* add; const int32_t* lens;
+  const float* norm_q; const float* norm_k; const float* inv_freq;
+  void* out; float* f32_out[3]; void* bf_out[3];
+} ezb_test_step_args;
+int ezb_test_step(int device, const ezb_test_step_args* args, void* stream);
 /* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7: that
    generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
@@ -271,6 +303,9 @@ int ezb_debug_read(unsigned long long* out8);
 /* accounting: kernels launched by this library so far (process-wide); per-GEMM CUDA-event timing for bench.py's roofline leg */
 unsigned long long ezb_launch_count(void);
 void ezb_launch_count_add(unsigned long long n); /* launches replayed from a captured CUDA graph */
+/* stand-alone LayerNorm launches of one kernel (the variant numbers of ezb_test_step: 1 generic, 2 / 3 register-resident, 4 precombined
+   affine, 5 register-resident concat) so far, process-wide; a captured CUDA graph counts once, at capture */
+unsigned long long ezb_ln_launch_count(int variant);
 int ezb_prof_gemm_begin(void);
 int ezb_prof_gemm_end(int* launches, double* flops, double* ms);
 int ezb_prof_gemm_stats(double min_flops, int* launches, double* flops, double* ms); /* subset of the last profile */
