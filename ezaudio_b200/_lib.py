@@ -31,6 +31,14 @@ class T5Desc(C.Structure):
                [("eps", C.c_float)] + [(n, C.c_int32) for n in ("max_batch", "max_len", "precision")]
 
 
+class DdimSlot(C.Structure):
+    """ezb_ddim_slot: the CFG / DDIM constants of one sample of ezb_cfg_ddim_step_slots."""
+    _fields_ = [("guidance_scale", C.c_float), ("guidance_rescale", C.c_float), ("coef", C.c_float * 5), ("flags", C.c_int32)]
+
+
+SLOT_ACTIVE, SLOT_CFG = 1, 2   # ezb_ddim_slot.flags
+
+
 class TestEpilogue(C.Structure):
     _fields_ = [("bias", C.c_void_p), ("bias_mod", C.c_int32), ("resid", C.c_void_p), ("ldr", C.c_int32),
                 ("gate", C.c_void_p), ("gate_bstride", C.c_int32), ("rows_per_batch", C.c_int32),
@@ -90,6 +98,9 @@ _SIGS = {
     "ezb_dit_forward": ([_VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _I, C.POINTER(_VP), _VP, _I, _I, _VP, _VP], _I),
     "ezb_controlnet_forward": ([_VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _I, _VP, _F, C.POINTER(_VP), _I, _I, _VP], _I),
     "ezb_cfg_ddim_step": ([_I, _VP, _VP, _VP, _I, _I, _I, _F, _F, C.POINTER(C.c_float), _VP, _VP], _I),
+    "ezb_dit_set_context_rows": ([_VP, _VP, _VP, _I, _I, _I, _VP], _I),
+    "ezb_dit_forward_tdev": ([_VP, _VP, _VP, _VP, _VP, C.POINTER(_VP), _VP, _I, _I, _VP, _VP], _I),
+    "ezb_cfg_ddim_step_slots": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP], _I),
     "ezb_option_epoch": ([], C.c_ulonglong),
     "ezb_vae_create": ([C.POINTER(_VP), C.POINTER(VaeDesc), _I], _I),
     "ezb_vae_destroy": ([_VP], _I),

@@ -630,13 +630,15 @@ struct Dit {
   }
   // `tail`: the LayerNorm that reads this GEMM's fp32 output; when the GEMM is a one-wave swap-AB launch it runs as the tail phase of the same
   // kernel (gemm_ln.cuh) and *tail_done is set, otherwise the caller launches it separately.
-  int lin(cudaStream_t st, const bf16* A, int K, const bf16* W, int M, int N, const EpiLinearParams& e, const LnParams* tail = nullptr, bool* tail_done = nullptr) {
+  // `m_select` (0: M): the token count the kernel is chosen for (context_rows: the whole batch, so that a part of it comes out bit-identical).
+  int lin(cudaStream_t st, const bf16* A, int K, const bf16* W, int M, int N, const EpiLinearParams& e, const LnParams* tail = nullptr, bool* tail_done = nullptr,
+          int m_select = 0) {
     if ((opt_skip() & 8) && e.out_f32 != nullptr && e.out_bf16 == nullptr) return EZB_OK;
     // fp32-output layers (residual / gated-residual / plain): swap-AB tiles of 128 features x 256 or 288 tokens (host.cuh swapped_bn)
     const bool folded = e.fin.u != nullptr || e.fout.st != nullptr;   // fold epilogues exist in the swap-AB kernel only
     const bool short_clips = e.gate != nullptr && e.rows_per_batch < 32;  // per-token gate lookup lives in the generic (non swap-AB) epilogue
     if (pair && swap_ab && kmul == 1 && e.out_bf16 == nullptr && e.out_f32 != nullptr && e.out_scale == 0.f && e.bias_mod == 0 && !short_clips &&
-        (M >= 512 || folded)) {
+        ((m_select ? m_select : M) >= 512 || folded)) {
       if (folded) return gemm_swapped<EpiLinearTF>(*dev, st, A, K, W, K, M, N, K, e);
       if (tail != nullptr && tail_done != nullptr && opt_ln_tail() && !(opt_skip() & 9))
         return gemm_swapped_ln<EpiLinearT>(*dev, st, A, K, W, K, M, N, K, e, *tail, grid_bar, tail_done);
@@ -750,30 +752,48 @@ struct Dit {
   int set_context(const float* ctx, const uint8_t* mask, int Be, int Lc, cudaStream_t st) {
     if (!finalized) return fail(EZB_ERR_STATE, "weights not finalized");
     if (Be < 1 || Be > d.max_batch || Lc < 1 || Lc > d.max_ctx_len) return fail(EZB_ERR_SHAPE, "set_context: Be %d Lc %d exceed workspace", Be, Lc);
-    const int Mc = Be * Lc, cd = d.context_dim;
     dev->tmaps.trim();
     ctx_Be = Be; ctx_Lc = Lc; ctx_Lpad = (Lc + 7) / 8 * 8;
-    EZB_CUDA(cudaMemcpyAsync(ctx_mask, mask, (size_t)Mc, cudaMemcpyDeviceToDevice, st));
+    return context_rows(ctx, mask, 0, Be, st);
+  }
+  // rows [row0, row0 + n) of the layout the last set_context established (ezb_dit_set_context_rows)
+  int set_context_rows(const float* ctx, const uint8_t* mask, int row0, int n, int Lc, cudaStream_t st) {
+    if (!finalized) return fail(EZB_ERR_STATE, "weights not finalized");
+    if (ctx_Be < 1) return fail(EZB_ERR_STATE, "set_context_rows: no ezb_dit_set_context call established the context layout");
+    if (Lc != ctx_Lc) return fail(EZB_ERR_STATE, "set_context_rows: Lc %d differs from the context layout (Lc %d)", Lc, ctx_Lc);
+    if (row0 < 0 || n < 1 || row0 + n > ctx_Be) return fail(EZB_ERR_SHAPE, "set_context_rows: rows [%d, %d) outside the batch of %d", row0, row0 + n, ctx_Be);
+    dev->tmaps.trim();
+    return context_rows(ctx, mask, row0, n, st);
+  }
+  // The context path of clips [row0, row0 + n) (ctx, mask: their rows only).  Every kernel works per token or per clip, and the one launch whose
+  // kernel depends on the token count (context_embed's fp32-output linear, Dit::lin) is chosen for the whole batch, so a row comes out as a call
+  // on the whole batch computes it.
+  int context_rows(const float* ctx, const uint8_t* mask, int row0, int n, cudaStream_t st) {
+    const int Lc = ctx_Lc, Mc = n * Lc, cd = d.context_dim;
+    const size_t r0 = (size_t)row0 * Lc, kq = (size_t)row0 * H * Lc * DHP, kv = (size_t)row0 * H * DVP * ctx_Lpad, k32 = (size_t)row0 * H * Lc * dh;
+    EZB_CUDA(cudaMemcpyAsync(ctx_mask + r0, mask, (size_t)Mc, cudaMemcpyDeviceToDevice, st));
     EZB_TRY(ln(st, ctx, cd, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, 0, 1, act, Mc));  // cast only
     EpiLinearParams e = epi();
     e.bias = b_ce0; e.out_bf16 = attn_out; e.ld16 = kmul * D; e.split_stride = kmul == 3 ? D : 0; e.act = ACT_SILU;
     EZB_TRY(lin(st, act, cd, w_ce0, Mc, D, e));
     e = epi();
-    e.bias = b_ce2; e.out_f32 = ctx_emb; e.ld32 = D;
-    EZB_TRY(lin(st, attn_out, D, w_ce2, Mc, D, e));
+    e.bias = b_ce2; e.out_f32 = ctx_emb + r0 * D; e.ld32 = D;
+    EZB_TRY(lin(st, attn_out, D, w_ce2, Mc, D, e, nullptr, nullptr, ctx_Be * Lc));
     for (int i = 0; i < nblk; ++i) {
       BlockW& w = blk[i];
-      EZB_TRY(ln(st, ctx_emb, D, nullptr, nullptr, 0, w.ncw, w.ncb, nullptr, nullptr, 0, 1, act, Mc));
+      bf16* kc16 = w.kc16 ? w.kc16 + kq : nullptr;
+      bf16* vtc16 = w.vtc16 ? w.vtc16 + kv : nullptr;
+      EZB_TRY(ln(st, ctx_emb + r0 * D, D, nullptr, nullptr, 0, w.ncw, w.ncb, nullptr, nullptr, 0, 1, act, Mc));
       const int off[2] = {0, D}, kinds[2] = {1, 2};
       if (fused_heads) {
-        EZB_TRY(lin_heads(st, act, w.ckv, Mc, 2 * D, kinds, nullptr, w.h_cnk, false, Lc, nullptr, w.kc16, w.vtc16, ctx_Lpad));
+        EZB_TRY(lin_heads(st, act, w.ckv, Mc, 2 * D, kinds, nullptr, w.h_cnk, false, Lc, nullptr, kc16, vtc16, ctx_Lpad));
         continue;
       }
       EZB_TRY(lin_to_qkv(st, act, D, w.ckv, Mc, 2 * D));
-      float* f32o[2] = {w.kc32, w.vc32};
-      bf16* bfo[2] = {w.kc16, w.vtc16};
-      if (use_tc_attention) EZB_CUDA(cudaMemsetAsync(w.vtc16, 0, (size_t)Be * H * DVP * ctx_Lpad * sizeof(bf16), st));
-      EZB_TRY(qk_prep(st, 2 * D, 2, off, kinds, nullptr, nullptr, w.cnkw, w.cnkb, nullptr, Be, Lc, f32o, bfo, ctx_Lpad));
+      float* f32o[2] = {w.kc32 ? w.kc32 + k32 : nullptr, w.vc32 ? w.vc32 + k32 : nullptr};
+      bf16* bfo[2] = {kc16, vtc16};
+      if (use_tc_attention) EZB_CUDA(cudaMemsetAsync(vtc16, 0, (size_t)n * H * DVP * ctx_Lpad * sizeof(bf16), st));
+      EZB_TRY(qk_prep(st, 2 * D, 2, off, kinds, nullptr, nullptr, w.cnkw, w.cnkb, nullptr, n, Lc, f32o, bfo, ctx_Lpad));
     }
     return EZB_OK;
   }
@@ -806,9 +826,19 @@ struct Dit {
     return build_fold_tables(n, st);
   }
 
-  // modulation rows for this call: uniform timestep -> point into the table (batch stride 0); else gather per sample
-  int select_mod(cudaStream_t st, const int32_t* tidx, int tall, int Be, const float** mod_rows, const float** modf_rows, int* bstride, int* bstride_f) {
+  // modulation rows for this call: uniform timestep -> point into the table (batch stride 0); else gather per sample.  Device indices (tdev)
+  // are always gathered, by a kernel, into the same per-sample rows the host-index gather fills.
+  int select_mod(cudaStream_t st, const int32_t* tidx, int tall, const int32_t* tdev, int Be, const float** mod_rows, const float** modf_rows, int* bstride,
+                 int* bstride_f) {
     const int ldm = nblk * 6 * D;
+    if (tdev) {
+      if (n_timesteps < 1) return fail(EZB_ERR_STATE, "device t_index without a timestep table; call ezb_dit_set_timesteps first");
+      const int n4 = (ldm + (mod_final ? 2 * D : 0)) / 4, gx = (n4 + 255) / 256 < 64 ? (n4 + 255) / 256 : 64;
+      EZB_TRY(launch_k(gather_mod_kernel, dim3(gx, Be), dim3(256), 0, st, 1, tdev, n_timesteps, reinterpret_cast<const float4*>(mod), ldm / 4,
+                       reinterpret_cast<const float4*>(mod_final), 2 * D / 4, reinterpret_cast<float4*>(mod_b), reinterpret_cast<float4*>(modf_b)));
+      *mod_rows = mod_b; *bstride = ldm; *modf_rows = mod_final ? modf_b : nullptr; *bstride_f = 2 * D;
+      return EZB_OK;
+    }
     bool uniform = true;
     int t0 = tidx ? tidx[0] : tall;
     for (int i = 0; tidx && i < Be; ++i) {
@@ -993,8 +1023,9 @@ struct Dit {
   // lens_ (device [Be] or null): sample b is a clip of lens_[b] <= L frames padded to L.  Only self-attention and the final conv mix
   // frames; both stop at the clip end, so its frames come out as a solo forward at that length computes them.  Every other kernel works
   // per token.
+  // tdev (device [Be] or null): per-sample timestep indices read on the device, in place of tidx / tall.
   int forward(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const float* const* cskips, float* out, int Be, int L,
-              const int32_t* lens_, cudaStream_t st) {
+              const int32_t* lens_, cudaStream_t st, const int32_t* tdev = nullptr) {
     if (d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_dit_forward called on a controlnet handle");
     EZB_TRY(check_call(Be, L));
     lens = lens_;
@@ -1002,7 +1033,7 @@ struct Dit {
     WeightSeqScope ws(dev, this, cskips ? 1 : 0, ((long long)Be << 32) | (unsigned)L);   // L2 prefetch of the next GEMM's weights (host.cuh)
     const float *modr, *modf;
     int mbs, mbsf;
-    EZB_TRY(select_mod(st, tidx, tall, Be, &modr, &modf, &mbs, &mbsf));
+    EZB_TRY(select_mod(st, tidx, tall, tdev, Be, &modr, &modf, &mbs, &mbsf));
     FoldCtx fc = fold_ctx(mbs, modr, L);
     const int M = Be * L;
     // the LayerNorm that opens block i, as parameters for the tail phase of the GEMM that produces its input x (gemm_ln.cuh)
@@ -1075,7 +1106,7 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
   WeightSeqScope ws(dev, this, 2, ((long long)Be << 32) | (unsigned)L);
   const float *modr, *modf;
   int mbs, mbsf;
-  EZB_TRY(select_mod(st, tidx, tall, Be, &modr, &modf, &mbs, &mbsf));
+  EZB_TRY(select_mod(st, tidx, tall, nullptr, Be, &modr, &modf, &mbs, &mbsf));
   const int c0 = d.cond_c0, c1 = d.cond_c1, T = 2 * L;
   auto conv = [&](const float* in, const float* w, const float* b, float* out, int Cin, int cin_real, int Tin, int Cout, int Tout, int K, int stride, int pad,
                   int act, int tr) -> int {

@@ -3,6 +3,7 @@
 // All fp32 math; bf16 only where a tensor feeds a tensor-core operand.
 #pragma once
 #include "common.cuh"
+#include "../../include/ezb200.h"
 
 namespace ezb {
 
@@ -689,15 +690,14 @@ __device__ __forceinline__ double ld_dsmem_f64(const double* local, uint32_t ran
   asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(mapa_u32(smem_u32(local), rank)));
   return v;
 }
-__global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
-                                                        const float* __restrict__ noise, const int32_t* __restrict__ lens, int C, int L, float gs, float gr,
-                                                        float c0, float c1, float c2, float c3, float c4) {
+// The update of one sample by its cluster (after pdl_wait): shared by cfg_ddim_kernel (scalars of the call) and cfg_ddim_slots_kernel
+// (scalars of the sample's slot).  out_uncond null: no guidance; noise null: sigma == 0.
+__device__ __forceinline__ void cfg_ddim_sample(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
+                                                const float* __restrict__ noise, const int32_t* __restrict__ lens, int sample, int C, int L, float gs,
+                                                float gr, float c0, float c1, float c2, float c3, float c4) {
   __shared__ double red[4][32];
   __shared__ double part[4];
-  pdl_launch();
-  pdl_wait();
   const uint32_t rank = cluster_ctarank();
-  const int sample = blockIdx.x / CFG_CLUSTER;
   const size_t base = (size_t)sample * C * L;
   const int len = lens != nullptr ? min(max(lens[sample], 1), L) : L;
   const int n = C * len;
@@ -751,6 +751,43 @@ __global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict_
     float prev = c2 * x0 + c3 * eps;
     if (z) prev += c4 * z[j];
     x[j] = prev;
+  }
+}
+__global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
+                                                        const float* __restrict__ noise, const int32_t* __restrict__ lens, int C, int L, float gs, float gr,
+                                                        float c0, float c1, float c2, float c3, float c4) {
+  pdl_launch();
+  pdl_wait();
+  cfg_ddim_sample(out_text, out_uncond, latents, noise, lens, blockIdx.x / CFG_CLUSTER, C, L, gs, gr, c0, c1, c2, c3, c4);
+}
+// The same update with the constants of each sample read from its slot (ezb_ddim_slot, device memory), so that one captured launch serves
+// samples at different points of different schedules.  out_uncond = the B uncond rows, used by slots with EZB_SLOT_CFG; a slot without
+// EZB_SLOT_ACTIVE leaves its latents untouched; noise is read only by slots with sigma != 0.
+__global__ void __launch_bounds__(1024) cfg_ddim_slots_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond,
+                                                              float* __restrict__ latents, const float* __restrict__ noise,
+                                                              const int32_t* __restrict__ lens, const ezb_ddim_slot* __restrict__ slots, int C, int L) {
+  pdl_launch();
+  pdl_wait();
+  const int sample = blockIdx.x / CFG_CLUSTER;
+  const ezb_ddim_slot s = slots[sample];
+  if (!(s.flags & EZB_SLOT_ACTIVE)) return;   // every CTA of the cluster reads the same slot: the cluster leaves whole, before any cluster barrier
+  cfg_ddim_sample(out_text, (s.flags & EZB_SLOT_CFG) ? out_uncond : nullptr, latents, s.coef[4] != 0.f ? noise : nullptr, lens, sample, C, L,
+                  s.guidance_scale, s.guidance_rescale, s.coef[0], s.coef[1], s.coef[2], s.coef[3], s.coef[4]);
+}
+
+// Per-sample modulation rows from DEVICE timestep indices (Dit::select_mod): sample b gets row t_index[b] (clamped to [0, n_t)) of the AdaLN
+// table mod [n_t, ldm4 float4] and of the FinalBlock table modf [n_t, ldf4 float4] (null: none) in mod_b / modf_b.  The indices are read when
+// the kernel runs, so a replayed graph follows later copies into them.
+__global__ void __launch_bounds__(256) gather_mod_kernel(const int32_t* __restrict__ t_index, int n_t, const float4* __restrict__ mod, int ldm4,
+                                                         const float4* __restrict__ modf, int ldf4, float4* __restrict__ mod_b, float4* __restrict__ modf_b) {
+  pdl_launch();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const int t = min(max(t_index[b], 0), n_t - 1);
+  const int n = ldm4 + (modf ? ldf4 : 0);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (i < ldm4) mod_b[(size_t)b * ldm4 + i] = mod[(size_t)t * ldm4 + i];
+    else modf_b[(size_t)b * ldf4 + (i - ldm4)] = modf[(size_t)t * ldf4 + (i - ldm4)];
   }
 }
 

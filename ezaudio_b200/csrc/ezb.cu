@@ -577,6 +577,22 @@ EZB_API int ezb_cfg_ddim_step(int device, const float* model_out, float* latents
   return launch_k(cfg_ddim_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, uncond, latents,
                   coef[4] != 0.f ? noise : (const float*)nullptr, lens, C, L, gs, gr, coef[0], coef[1], coef[2], coef[3], coef[4]);
 }
+EZB_API int ezb_dit_set_context_rows(ezb_dit* h, const float* ctx, const uint8_t* ctx_mask, int row0, int n, int Lc, void* stream) {
+  if (!h || !ctx || !ctx_mask) return fail(EZB_ERR_ARG, "ezb_dit_set_context_rows: null argument");
+  return reinterpret_cast<Dit*>(h)->set_context_rows(ctx, ctx_mask, row0, n, Lc, ST(stream));
+}
+EZB_API int ezb_dit_forward_tdev(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_dev,
+                                 const float* const* cskips, float* out, int Be, int L, void* stream, const int32_t* lens) {
+  if (!h || !x || !out || !t_index_dev) return fail(EZB_ERR_ARG, "ezb_dit_forward_tdev: null argument");
+  return reinterpret_cast<Dit*>(h)->forward(x, gt, gt_mask, nullptr, 0, cskips, out, Be, L, lens, ST(stream), t_index_dev);
+}
+EZB_API int ezb_cfg_ddim_step_slots(int device, const float* model_out, float* latents, const float* noise, const ezb_ddim_slot* slots, int B, int C,
+                                    int L, void* stream, const int32_t* lens) {
+  if (!model_out || !latents || !slots || B < 1 || C < 1 || L < 1) return fail(EZB_ERR_ARG, "ezb_cfg_ddim_step_slots: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  return launch_k(cfg_ddim_slots_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, model_out + (size_t)B * C * L,
+                  latents, noise, lens, slots, C, L);
+}
 EZB_API int ezb_vae_create(ezb_vae** out, const ezb_vae_desc* desc, int device) {
   if (!out || !desc) return fail(EZB_ERR_ARG, "ezb_vae_create: null argument");
   EZB_CUDA(cudaSetDevice(device));

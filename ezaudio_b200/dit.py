@@ -67,6 +67,7 @@ class _Handle:
             _lib.check(_lib.lib().ezb_dit_create(C.byref(self.h), C.byref(d), self.dev_index))
         self.loaded = False
         self._ctx_key = None
+        self.ctx_epoch = 0
         self._ts: List[int] = []
         _Handle._serial += 1
         self.serial = _Handle._serial   # identifies this handle in graph-cache keys (id() values are recycled)
@@ -107,6 +108,18 @@ class _Handle:
             _lib.check(_lib.lib().ezb_dit_set_context(self.h, _lib.ptr(ctx), _lib.ptr(m), B, Lc, _lib.stream_ptr()))
         self._keep = (ctx, m)
         self._ctx_key = None   # a direct set_context invalidates whatever ensure_context cached
+        self.ctx_epoch += 1    # lets a holder of context rows (engine.ContinuousEngine) see that the layout was replaced
+
+    def set_context_rows(self, context: torch.Tensor, context_mask: Optional[torch.Tensor], row0: int):
+        n, Lc, _ = context.shape
+        ctx = _as_f32c(context).to(self.device)
+        if context_mask is None:
+            context_mask = torch.ones(n, Lc, dtype=torch.bool, device=self.device)
+        m = context_mask.to(self.device).to(torch.uint8).contiguous()
+        with torch.cuda.device(self.dev_index):
+            _lib.check(_lib.lib().ezb_dit_set_context_rows(self.h, _lib.ptr(ctx), _lib.ptr(m), int(row0), n, Lc, _lib.stream_ptr()))
+        self._keep_rows = (ctx, m)
+        self._ctx_key = None
 
     def set_timesteps(self, ts: Sequence[int]):
         ts = [int(t) for t in ts]
@@ -188,24 +201,38 @@ class MaskDiT:
     def set_timesteps(self, ts):
         self._h.set_timesteps(ts)
 
-    def forward_step(self, x, step_index: int, gt=None, gt_mask_u8=None, controlnet_skips=None, out=None, lengths=None):
+    def set_context_rows(self, context, context_mask, row0: int):
+        """Replaces the text context of samples [row0, row0 + n) (context (n,Lc,ctx), context_mask (n,Lc)) in the layout of the last
+        set_context, without recomputing the other rows; Lc must be that call's.  The rows come out as set_context of the whole updated
+        batch computes them."""
+        self._h.set_context_rows(context, context_mask, row0)
+
+    def forward_step(self, x, step_index: int, gt=None, gt_mask_u8=None, controlnet_skips=None, out=None, lengths=None, t_index=None):
         """One denoiser forward at table row `step_index` (all samples share it).  x (Be,C,L) fp32 cuda.
         `lengths`: None, or a cuda int32 tensor (Be,) of clip lengths in 1..L (padded batch): frames < lengths[b] of sample b come out as a
         forward of that clip alone computes them; frames past it are not written.  The values are read on the device when the kernels run
-        (so a captured graph follows later copies into the tensor) and are not checked here: the caller validates them."""
+        (so a captured graph follows later copies into the tensor) and are not checked here: the caller validates them.
+        `t_index`: None, or a cuda int32 tensor (Be,) of per-sample table rows used instead of `step_index`; read on the device like
+        `lengths` (out-of-range rows are clamped, the caller validates them)."""
         Be, Cc, L = x.shape
         if lengths is not None:
             if gt is not None or controlnet_skips is not None:
                 raise NotImplementedError("per-sample lengths with inpainting (gt) or ControlNet skips")
             if lengths.dtype != torch.int32 or not lengths.is_cuda or tuple(lengths.shape) != (Be,) or not lengths.is_contiguous():
                 raise ValueError(f"lengths must be a contiguous cuda int32 tensor of shape ({Be},)")
+        if t_index is not None and (t_index.dtype != torch.int32 or not t_index.is_cuda or tuple(t_index.shape) != (Be,) or not t_index.is_contiguous()):
+            raise ValueError(f"t_index must be a contiguous cuda int32 tensor of shape ({Be},)")
         out = torch.empty_like(x) if out is None else out
         sk = None
         if controlnet_skips is not None:
             sk = (C.c_void_p * len(controlnet_skips))(*[s.data_ptr() for s in controlnet_skips])
         with torch.cuda.device(self._h.dev_index):
-            _lib.check(_lib.lib().ezb_dit_forward(self._h.h, _lib.ptr(x), _lib.ptr(gt), _lib.ptr(gt_mask_u8), None, int(step_index),
-                                                  sk, _lib.ptr(out), Be, L, _lib.stream_ptr(), _lib.ptr(lengths)))
+            if t_index is not None:
+                _lib.check(_lib.lib().ezb_dit_forward_tdev(self._h.h, _lib.ptr(x), _lib.ptr(gt), _lib.ptr(gt_mask_u8), _lib.ptr(t_index), sk,
+                                                           _lib.ptr(out), Be, L, _lib.stream_ptr(), _lib.ptr(lengths)))
+            else:
+                _lib.check(_lib.lib().ezb_dit_forward(self._h.h, _lib.ptr(x), _lib.ptr(gt), _lib.ptr(gt_mask_u8), None, int(step_index),
+                                                      sk, _lib.ptr(out), Be, L, _lib.stream_ptr(), _lib.ptr(lengths)))
         return out
 
     def _forward_raw(self, x, gt, gt_mask, timesteps, context, context_mask, controlnet_skips, gt_is_final=False):

@@ -1,0 +1,316 @@
+"""Continuous batching for text-to-audio: requests join a running batch at step boundaries.
+
+`ContinuousEngine` keeps `slots` requests in flight in one padded, CFG-doubled batch (effective batch 2 * slots, clips padded to
+`max_length_s`).  Each denoising step is one replay of one captured CUDA graph: the CFG-doubling copy, the DiT forward with per-sample
+timestep rows read from device memory (`MaskDiT.forward_step(t_index=)`) and the fused CFG + rescale + DDIM update with per-sample
+constants (ezb_cfg_ddim_step_slots).  Between steps the host admits queued requests into free slots, first come first served -- it
+encodes the prompt, replaces that slot's text context row (`MaskDiT.set_context_rows`), seeds its generator and draws its initial noise
+-- and decodes each request that finished its schedule alone at its own length.
+
+Every request keeps its own step count (one of `ddim_steps`), guidance scale, rescale, eta, length and seed: the denoiser's timestep table
+holds the sorted union of the allowed schedules (with trailing spacing the 25- and 50-step schedules are subsets of the 100-step one).  A
+request's audio does not depend on what it shares the batch with.  Requests have the semantics of `EzAudio.generate_audio` for one prompt
+(`frontend.Request`); the empty prompt "" runs without guidance, as it does there.  Inpainting, ControlNet and the FP8 mode are not served.
+
+The host logic (admission, schedules, DDIM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots`, which tests replace
+with a stub."""
+from __future__ import annotations
+
+import collections
+import dataclasses
+import math
+import numbers
+from typing import Iterable, Iterator, List, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import _lib
+from .frontend import Request
+from .inference import scale_shift_re
+from .scheduler import DDIMScheduler
+
+MAX_TABLE = 128   # rows of the denoiser's per-timestep LayerNorm tables (csrc/dit.cuh gc_T / fold_T)
+
+
+@dataclasses.dataclass
+class SlotStep:
+    """What one active slot does in one step."""
+    t_index: int              # row of the timestep table
+    frames: int
+    guidance_scale: float     # 0 without guidance
+    guidance_rescale: float
+    coef: List[float]         # DDIMScheduler.step_coefficients
+    cfg: bool
+    draw_noise: bool          # eta > 0: the slot's generator draws this step's (1, C, frames) noise
+
+
+@dataclasses.dataclass
+class _Active:
+    ticket: int
+    req: Request
+    frames: int
+    timesteps: List[int]
+    sched: DDIMScheduler
+    step: int = 0
+
+
+class ContinuousEngine:
+    """Continuous-batching server for `ez` (an `api.EzAudio`): `submit` requests, then `step` / `stream` / `run` them (see the module docstring).
+
+    slots: requests in flight (the denoiser runs 2 * slots samples; ez must have been built with max_batch >= slots).
+    max_length_s: the padded clip length (at most ez.max_length_s); longer requests are rejected.
+    ddim_steps: the step counts requests may ask for; the union of their schedules must fit the timestep table."""
+
+    def __init__(self, ez, slots: int = 4, max_length_s: float = 10.0, ddim_steps: Sequence[int] = (25, 50, 100), *, backend=None):
+        self.slots = int(slots)
+        if self.slots < 1:
+            raise ValueError("slots must be >= 1")
+        if any(isinstance(n, bool) or int(n) != n for n in ddim_steps):
+            raise ValueError(f"ddim_steps must list positive step counts, got {list(ddim_steps)}")
+        allowed = sorted({int(n) for n in ddim_steps})
+        if not allowed or allowed[0] < 1:
+            raise ValueError(f"ddim_steps must list positive step counts, got {list(ddim_steps)}")
+        make = backend.make_scheduler if backend is not None else (lambda: DDIMScheduler(**ez.params["diff"]))
+        self._scheds = {}
+        for n in allowed:
+            s = make()
+            s.set_timesteps(n)
+            self._scheds[n] = s
+        self._timesteps = {n: [int(t) for t in s.timesteps] for n, s in self._scheds.items()}
+        table = sorted({t for ts in self._timesteps.values() for t in ts})
+        max_t = backend.max_timesteps if backend is not None else ez.unet._h.desc.max_timesteps
+        if len(table) > min(max_t, MAX_TABLE):
+            raise ValueError(f"the schedules of ddim_steps {allowed} hold {len(table)} distinct timesteps; the table holds at most "
+                             f"{min(max_t, MAX_TABLE)}")
+        self.ddim_steps = tuple(allowed)
+        self.table = table
+        self._row = {t: i for i, t in enumerate(table)}
+        self.backend = backend if backend is not None else CudaSlots(ez, self.slots, max_length_s, table)
+        self._queue: collections.deque = collections.deque()
+        self._active: List[Optional[_Active]] = [None] * self.slots
+        self._tickets = 0
+
+    # ---- requests
+    def _frames(self, r: Request) -> int:
+        if not isinstance(r.ddim_steps, numbers.Integral) or isinstance(r.ddim_steps, bool) or int(r.ddim_steps) not in self._scheds:
+            raise ValueError(f"ddim_steps {r.ddim_steps} is not one of this engine's step counts {list(self.ddim_steps)}")
+        if not isinstance(r.length, numbers.Real) or isinstance(r.length, bool) or not math.isfinite(r.length) or r.length <= 0:
+            raise ValueError(f"length must be a positive number of seconds, got {r.length!r}")
+        frames = int(r.length * self.backend.latent_sr)
+        if not 1 <= frames <= self.backend.max_frames:
+            raise ValueError(f"length {r.length} s is {frames} frames; this engine serves 1..{self.backend.max_frames}")
+        s = r.random_seed
+        if s is not None and (not isinstance(s, numbers.Integral) or isinstance(s, bool) or not 0 <= int(s) < 2 ** 63):
+            raise ValueError(f"random_seed must be None or an integer in [0, 2**63), got {s!r}")
+        for name in ("guidance_scale", "guidance_rescale", "eta"):
+            v = getattr(r, name)
+            if v is not None and (not isinstance(v, numbers.Real) or isinstance(v, bool) or not math.isfinite(v)):
+                raise ValueError(f"{name} must be a finite number or None, got {v!r}")
+        if (r.eta or 0) < 0:
+            raise ValueError(f"eta must be >= 0, got {r.eta}")
+        return frames
+
+    def submit(self, prompt: str, **kw) -> int:
+        """Queues a request (the keyword arguments of `frontend.Request`); returns its ticket.  Invalid requests raise ValueError here,
+        before any device work."""
+        r = Request(prompt, **kw)
+        frames = self._frames(r)
+        t = self._tickets
+        self._tickets += 1
+        self._queue.append((t, r, frames))
+        return t
+
+    def pending(self) -> int:
+        """Requests queued or in flight."""
+        return len(self._queue) + sum(a is not None for a in self._active)
+
+    # ---- scheduling
+    def _admit(self):
+        for k in range(self.slots):
+            if self._active[k] is None and self._queue:
+                t, r, frames = self._queue.popleft()
+                self.backend.admit(k, r.prompt, None if r.random_seed is None else int(r.random_seed), frames)
+                n = int(r.ddim_steps)
+                self._active[k] = _Active(t, r, frames, self._timesteps[n], self._scheds[n])
+
+    def step(self) -> List[Tuple[int, int, object]]:
+        """Admits queued requests into free slots, runs one denoising step of every request in flight and returns (ticket, sample_rate,
+        waveform) of those that finished their schedule with it."""
+        self._admit()
+        if not any(a is not None for a in self._active):
+            return []
+        plan: List[Optional[SlotStep]] = []
+        for a in self._active:
+            if a is None:
+                plan.append(None)
+                continue
+            r, t = a.req, a.timesteps[a.step]
+            eta = float(r.eta or 0.0)
+            cfg = bool(r.guidance_scale) and r.prompt != ""   # "" switches guidance off (api/ezaudio.py:109-111)
+            plan.append(SlotStep(self._row[t], a.frames, float(r.guidance_scale) if cfg else 0.0, float(r.guidance_rescale or 0.0),
+                                 a.sched.step_coefficients(t, eta), cfg, eta > 0))
+        self.backend.step(plan)
+        done = []
+        for k, a in enumerate(self._active):
+            if a is None:
+                continue
+            a.step += 1
+            if a.step == len(a.timesteps):
+                wav = self.backend.finish(k, a.frames)
+                self._active[k] = None
+                done.append((a.ticket, self.backend.sr, wav))
+        return done
+
+    def stream(self, requests: Optional[Iterable[Request]] = None) -> Iterator[Tuple[int, int, object]]:
+        """Submits `requests` (if given) and yields (ticket, sample_rate, waveform) in completion order until nothing is queued or in flight."""
+        if requests is not None:
+            for r in requests:
+                self.submit(**dataclasses.asdict(r))
+        while self.pending():
+            yield from self.step()
+
+    def run(self, requests: Optional[Iterable[Request]] = None) -> List[Tuple[int, object]]:
+        """`requests` (default: the queued ones), in request order: result[i] = (sample_rate, waveform)."""
+        if requests is not None:
+            tickets = [self.submit(**dataclasses.asdict(r)) for r in requests]
+        else:
+            tickets = [t for t, _, _ in self._queue]
+        pos = {t: i for i, t in enumerate(tickets)}
+        out: List[Optional[Tuple[int, object]]] = [None] * len(tickets)
+        for t, sr, w in self.stream():
+            if t in pos:
+                out[pos[t]] = (sr, w)
+        return out
+
+
+class CudaSlots:
+    """Device side of ContinuousEngine: the slot buffers, the captured step graph and the per-slot generators of one `api.EzAudio`.
+
+    Between steps the engine owns the denoiser's context and timestep table: a generate_audio call on the same EzAudio replaces them, and the
+    next step restores them (set_context of the whole batch, set_timesteps of the table)."""
+
+    def __init__(self, ez, slots: int, max_length_s: float, table: Sequence[int]):
+        p = ez.params["autoencoder"]
+        self.ez, self.unet, self.S, self.table = ez, ez.unet, int(slots), [int(t) for t in table]
+        self.sr, self.latent_sr = int(p["sr"]), int(p["latent_sr"])
+        self.max_frames = int(round(max_length_s * self.latent_sr))
+        desc = self.unet._h.desc
+        self.max_timesteps = int(desc.max_timesteps)
+        if getattr(self.unet, "precision", "bf16") == "fp8":
+            raise NotImplementedError("the continuous engine serves the bf16 and bf16x3 precisions")
+        if 2 * self.S > desc.max_batch:
+            raise ValueError(f"{self.S} slots need a denoiser batch of {2 * self.S}; this EzAudio holds {desc.max_batch} (max_batch {desc.max_batch // 2})")
+        if max_length_s > ez.max_length_s or self.max_frames > desc.max_len or self.max_frames < 1:
+            raise ValueError(f"max_length_s {max_length_s} must lie in (0, {ez.max_length_s}] (the EzAudio's max_length_s)")
+        if ez.encode_text is None:
+            raise RuntimeError("no text encoder available: pass text_encoder=<callable> to EzAudio")
+        self.C = int(self.unet.cfg["out_chans"])
+        S, Be, C, L = self.S, 2 * self.S, self.C, self.max_frames
+        self.device = torch.device("cuda", self.unet._h.dev_index)
+        with torch.cuda.device(self.device):
+            d = dict(device=self.device, dtype=torch.float32)
+            self.lat, self.noise = torch.zeros(S, C, L, **d), torch.zeros(S, C, L, **d)   # padded frames stay zero
+            self.x_in, self.out = torch.zeros(Be, C, L, **d), torch.zeros(Be, C, L, **d)
+            # per-step inputs as one int32 block, staged through pinned memory: t_index [Be] | lens [Be] | ezb_ddim_slot [S] (8 words each)
+            words = 2 * Be + 8 * S
+            self._h = torch.zeros(words, dtype=torch.int32, pin_memory=True)
+            self._d = torch.zeros(words, dtype=torch.int32, device=self.device)
+            self._copied = None
+            self.t_index, self.lens, self.slots_dev = self._d[:Be], self._d[Be:2 * Be], self._d[2 * Be:]
+            uemb, umask = ez.encode_text([""])   # the uncond rows: the "" embedding, once
+            self.Lc = int(uemb.shape[1])
+            self.ctx = uemb.to(**d).expand(Be, -1, -1).contiguous()
+            self.cmask = umask.to(self.device).bool().expand(Be, -1).contiguous()
+        self.gens: List[Optional[torch.Generator]] = [None] * S
+        self.graph, self._key, self._launches = None, None, 0
+        self.captures = 0   # step graphs captured so far
+        self._ctx_epoch = None
+
+    def _own_denoiser(self):
+        """Puts the engine's timestep table and context back if something else replaced them since the last step."""
+        self.unet.set_timesteps(self.table)   # no device work when the table is already loaded
+        h = self.unet._h
+        if self._ctx_epoch != h.ctx_epoch:
+            self.unet.set_context(self.ctx, self.cmask)
+            self._ctx_epoch = h.ctx_epoch
+
+    def admit(self, k: int, prompt: str, seed: Optional[int], frames: int):
+        with torch.cuda.device(self.device):
+            self._own_denoiser()
+            emb, mask = self.ez.encode_text([prompt])
+            if tuple(emb.shape[1:]) != tuple(self.ctx.shape[1:]):
+                raise ValueError(f"the text encoder returned {tuple(emb.shape)}, the engine's context rows are {tuple(self.ctx.shape[1:])}")
+            self.ctx[k:k + 1].copy_(emb)
+            self.cmask[k:k + 1].copy_(mask)
+            self.unet.set_context_rows(self.ctx[k:k + 1], self.cmask[k:k + 1], k)
+            g = torch.Generator(device=self.device)
+            if seed is None:
+                g.seed()
+            else:
+                g.manual_seed(seed)
+            self.gens[k] = g
+            self.lat[k].zero_()
+            self.lat[k, :, :frames] = torch.randn((1, self.C, frames), generator=g, device=self.device)[0]   # the draw of a solo run
+
+    def _launch_step(self):
+        S = self.S
+        self.x_in[:S].copy_(self.lat)
+        self.x_in[S:].copy_(self.lat)
+        self.unet.forward_step(self.x_in, 0, out=self.out, lengths=self.lens, t_index=self.t_index)
+        _lib.check(_lib.lib().ezb_cfg_ddim_step_slots(self.device.index, _lib.ptr(self.out), _lib.ptr(self.lat), _lib.ptr(self.noise),
+                                                      _lib.ptr(self.slots_dev), S, self.C, self.max_frames, _lib.stream_ptr(),
+                                                      _lib.ptr(self.lens[:S])))
+
+    def step(self, plan: Sequence[Optional[SlotStep]]):
+        S, Be = self.S, 2 * self.S
+        with torch.cuda.device(self.device):
+            self._own_denoiser()
+            if self._copied is not None:
+                self._copied.synchronize()   # the previous step's copy has read the pinned block
+            h = self._h.numpy()
+            tix, lens = h[:Be], h[Be:2 * Be]
+            words = h[2 * Be:].reshape(S, 8)
+            fl = words.view(np.float32)
+            for k, e in enumerate(plan):
+                if e is None:   # inactive: one frame, no update
+                    tix[k] = tix[S + k] = 0
+                    lens[k] = lens[S + k] = 1
+                    words[k] = 0
+                    continue
+                tix[k] = tix[S + k] = e.t_index
+                lens[k] = lens[S + k] = e.frames
+                fl[k, 0], fl[k, 1] = e.guidance_scale, e.guidance_rescale
+                fl[k, 2:7] = e.coef
+                words[k, 7] = _lib.SLOT_ACTIVE | (_lib.SLOT_CFG if e.cfg else 0)
+                if e.draw_noise:   # the draw a solo run makes at this step: a contiguous (1, C, frames) tensor from the slot's generator
+                    self.noise[k, :, :e.frames] = torch.empty((1, self.C, e.frames), device=self.device).normal_(generator=self.gens[k])[0]
+            self._d.copy_(self._h, non_blocking=True)
+            self._copied = torch.cuda.Event()
+            self._copied.record()
+            key = (S, self.max_frames, self.Lc, int(_lib.lib().ezb_option_epoch()))
+            L_ = _lib.lib()
+            if self.graph is not None and key == self._key:
+                self.graph.replay()
+                L_.ezb_launch_count_add(self._launches)
+                return
+            self._launch_step()   # eager pass: this step's result, and warm caches for the capture
+            snap = self.lat.clone()
+            g = torch.cuda.CUDAGraph()
+            n0 = L_.ezb_launch_count()
+            with torch.cuda.graph(g):
+                self._launch_step()
+            self._launches = int(L_.ezb_launch_count() - n0)
+            self.graph, self._key = g, key
+            self.captures += 1
+            self.lat.copy_(snap)   # capture does not execute; keep the eager result
+
+    def finish(self, k: int, frames: int):
+        """Decodes slot k alone at its own length (as inference() does) and frees it; returns the float32 waveform (hop * frames,)."""
+        with torch.cuda.device(self.device):
+            p = self.ez.params["autoencoder"]
+            pred = scale_shift_re(self.lat[k:k + 1, :, :frames], p["scale"], p["shift"]).contiguous()
+            wav = self.ez.autoencoder(embedding=pred)
+            self.lat[k].zero_()
+            self.gens[k] = None
+            return wav[0, 0].cpu().numpy()

@@ -7,8 +7,8 @@
  *
  * Conventions: plain pointers and sizes, no torch types.  Every device pointer is owned by the caller (PyTorch) and
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
- * `stream` (void*).  The per-step entry points (set_context, set_timesteps, forward, controlnet_forward, cfg_ddim_step, decode,
- * encode, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
+ * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
+ * cfg_ddim_step, cfg_ddim_step_slots, decode, encode, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
  */
@@ -81,6 +81,20 @@ int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, const ui
                            int t_index_all, const float* condition, float conditioning_scale, float* const* skips_out, int Be,
                            int L, void* stream);
 
+/* --- step-level scheduling: samples of one batch at different points of different schedules (continuous batching).
+ * ezb_dit_set_context_rows: the context path of ezb_dit_set_context for rows [row0, row0 + n) of the batch only -- context_embed,
+ * norm_context, and per block the cross-attention K / V^T caches and the key-mask bytes of those rows; the other rows keep what they hold.
+ * ctx (n,Lc,context_dim) fp32 and ctx_mask (n,Lc) uint8 are DEVICE pointers to the new rows.  It writes into the layout (Be, Lc) of the last
+ * ezb_dit_set_context call and fails with EZB_ERR_STATE when there was none or when Lc differs from it; the rows come out bit-identical to a
+ * ezb_dit_set_context of the whole updated batch (the kernels are chosen for the whole batch).  Graph-safe, no synchronisation. */
+int ezb_dit_set_context_rows(ezb_dit* h, const float* ctx, const uint8_t* ctx_mask, int row0, int n, int Lc, void* stream);
+/* ezb_dit_forward with the per-sample timestep indices in DEVICE memory: t_index_dev int32 [Be], indices into the table of
+ * ezb_dit_set_timesteps.  The indices are read when the kernels run (a captured graph replays with new indices); out-of-range values are
+ * clamped to the table, validating them is the caller's job.  The output is bit-identical to ezb_dit_forward with the same indices in
+ * t_index_host when they are not all equal (a batch that shares one timestep may take other kernels there). */
+int ezb_dit_forward_tdev(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_dev,
+                         const float* const* controlnet_skips, float* out, int Be, int L, void* stream, const int32_t* lens);
+
 /* --- fused classifier-free guidance + rescale + DDIM update (src/inference.py:12-23,88-100; diffusers DDIMScheduler.step
  * restated, SURVEY Appendix B).  model_out holds B text rows followed by B uncond rows when guidance_scale != 0, else B
  * rows.  coef = {sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-sigma^2), sigma}; noise (B,C,L) may be NULL when
@@ -90,6 +104,20 @@ int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, const ui
  * frames of latents are left untouched. */
 int ezb_cfg_ddim_step(int device, const float* model_out, float* latents, const float* noise, int B, int C, int L, float guidance_scale,
                       float guidance_rescale, const float* coef5_host, void* stream, const int32_t* lens);
+/* ezb_cfg_ddim_step with the constants of each sample in a DEVICE array slots_dev[B], read when the kernel runs (a captured graph replays
+ * with new slots).  model_out always holds B text rows followed by B uncond rows.  Sample b with flags & EZB_SLOT_ACTIVE is updated as
+ * ezb_cfg_ddim_step on that sample alone with its slot's guidance_scale (when flags & EZB_SLOT_CFG; without it only the text row is used,
+ * as with guidance_scale 0), guidance_rescale and coef computes it, bit for bit; an inactive sample's latents are not touched.  noise
+ * (B,C,L) is read only by samples whose sigma (coef[4]) is non-zero; it may be NULL when no active slot has one -- checking that is the
+ * caller's job, as is validating lens (clamped to [1, L] as in ezb_cfg_ddim_step). */
+typedef struct {
+  float guidance_scale, guidance_rescale;
+  float coef[5];   /* as coef5_host of ezb_cfg_ddim_step */
+  int32_t flags;   /* EZB_SLOT_ACTIVE | EZB_SLOT_CFG */
+} ezb_ddim_slot;
+enum { EZB_SLOT_ACTIVE = 1, EZB_SLOT_CFG = 2 };
+int ezb_cfg_ddim_step_slots(int device, const float* model_out, float* latents, const float* noise, const ezb_ddim_slot* slots_dev, int B,
+                            int C, int L, void* stream, const int32_t* lens);
 
 /* --- VAE decoder: OobleckDecoder.forward (stable_vae/models/autoencoders.py:149-190) behind
  * Autoencoder(embedding=z) (src/modules/autoencoder_wrapper.py:74-77). */
