@@ -1,7 +1,8 @@
 """Public API -- same classes, method signatures, defaults and return types as the reference
 (api/ezaudio.py:31-207 `EzAudio`, api/controlnet.py:31-161 `EzAudio_ControlNet`), hosted on the CUDA library.
 
-Extensions (all optional, keyword-only): `text` may be a list of prompts (batched; returns a list of waveforms);
+Extensions (all optional, keyword-only): `text` may be a list of prompts (batched; returns a list of waveforms; for `editing_audio`
+the clip, mask, boundary and seed arguments then list one value per prompt and the edits, whatever their crop lengths, run as one batch);
 `text_encoder=` injects a callable `(list[str]) -> (emb (B,Lc,ctx) , mask (B,Lc))` standing in for flan-T5 (the image has no
 network, so T5 weights cannot be fetched -- BASELINE configs use cached embeddings); `ckpt_path="synthetic:<seed>"` builds
 the deterministic random checkpoint of `weights.synthetic_state_dict` instead of reading a file.
@@ -161,6 +162,41 @@ class _Base:
         return NativeTextEncoder(tok, enc, ml, device)
 
 
+def edit_plan(n_samples: int, sr: int, latent_sr: int, hop: int, boundary, mask_start, mask_length) -> dict:
+    """The index arithmetic of one edit (api/ezaudio.py:140-203), on the host: a clip of n_samples samples, the mask [mask_start,
+    mask_start + mask_length) seconds regenerated with `boundary` seconds of context on either side.
+    n_total: samples of the output clip (the input zero-padded to the mask's end when outpainting); [s0, s1): samples of the crop that is
+    encoded; frames: its latent frames (whole hops, the last one zero-padded); [m0, m1): latent frames regenerated; n_paste: samples of the
+    decoded crop pasted back at s0."""
+    mask_end = mask_start + mask_length
+    audio_length = n_samples / sr
+    mask_start = min(mask_start, audio_length)
+    n_total = n_samples
+    if mask_end > audio_length:
+        n_total += round((mask_end - audio_length) * sr)
+        audio_length = n_total / sr
+    boundary = min((mask_end - mask_start) / 2, boundary)
+    start_idx = max(mask_start - boundary, 0)
+    end_idx = min(mask_end + boundary, audio_length)
+    mask_start -= start_idx
+    mask_end -= start_idx
+    s0, s1 = round(start_idx * sr), round(end_idx * sr)
+    frames = -(-(s1 - s0) // hop)
+    m0, m1 = min(round(mask_start * latent_sr), frames), min(round(mask_end * latent_sr), frames)
+    n_paste = min(round((end_idx - start_idx) * sr), frames * hop, n_total - s0)
+    return dict(n_total=n_total, s0=s0, s1=s1, frames=frames, m0=m0, m1=m1, n_paste=n_paste)
+
+
+def _per_clip(name: str, value, n: int, scalar_types) -> list:
+    """One value per clip: a scalar is repeated, a list must hold n."""
+    if isinstance(value, scalar_types):
+        return [value] * n
+    value = list(value)
+    if len(value) != n:
+        raise ValueError(f"{name} lists one value per prompt: got {len(value)} for {n} prompts")
+    return value
+
+
 def _vae_precision(precision: str) -> str:
     """The VAE (and T5) have no FP8 mode: precision="fp8" builds them in "bf16"."""
     return "bf16" if precision == "fp8" else precision
@@ -249,8 +285,18 @@ class EzAudio(_Base):
         return (sr, out) if batched else (sr, out[0])
 
     def editing_audio(self, text, boundary, gt_file, mask_start, mask_length, guidance_scale=3.5, guidance_rescale=0, ddim_steps=100,
-                      eta=1, random_seed=None, randomize_seed=False):
-        """api/ezaudio.py:132-207 (crop -> VAE encode -> masked sampling -> paste -> decode -> splice)."""
+                      eta=1, random_seed=None, randomize_seed=False, *, pad_length=None):
+        """api/ezaudio.py:132-207 (crop -> VAE encode -> masked sampling -> paste -> decode -> splice).
+        With a list of prompts, `gt_file` (paths or waveforms), `mask_start`, `mask_length`, `boundary` and `random_seed` list one value per
+        prompt (a scalar applies to all) and the call returns (sr, [waveforms]).  The edits run as one batch -- one VAE encode, one sampling
+        loop, one decode -- padded to the longest crop, or to `pad_length` seconds (at most max_length_s) so that batches of different crops
+        reuse one captured graph.  Each waveform equals the scalar call of that edit with its seed, the calls made in list order (they
+        draw the bottleneck noise from the global RNG in that order)."""
+        if isinstance(text, (list, tuple)):
+            return self._editing_batch(list(text), boundary, gt_file, mask_start, mask_length, guidance_scale, guidance_rescale, ddim_steps, eta,
+                                       random_seed, randomize_seed, pad_length)
+        if pad_length is not None:
+            raise ValueError("pad_length applies to a list of edits")
         sr = self.params["autoencoder"]["sr"]
         if text == "":
             guidance_scale = None
@@ -287,6 +333,62 @@ class EzAudio(_Base):
         n = min(round((end_idx - start_idx) * sr), pred.shape[-1], n_total - s0)
         post.splice_wave(output_audio, pred[0, 0], s0, n)
         return sr, output_audio.cpu().numpy()
+
+    def _editing_batch(self, prompts, boundary, gt_file, mask_start, mask_length, guidance_scale, guidance_rescale, ddim_steps, eta, random_seed,
+                       randomize_seed, pad_length):
+        sr, latent_sr = self.params["autoencoder"]["sr"], self.params["autoencoder"]["latent_sr"]
+        dec = self.autoencoder.decoder
+        B, hop = len(prompts), dec.hop
+        # ---- everything is checked on the host before any device work
+        if B < 1 or B > dec.max_batch:
+            raise ValueError(f"{B} edits in one call: 1..{dec.max_batch} (max_batch) fit the workspace")
+        num = (int, float, np.integer, np.floating)
+        files = _per_clip("gt_file", gt_file, B, (str, np.ndarray))
+        starts, lengths_s = _per_clip("mask_start", mask_start, B, num), _per_clip("mask_length", mask_length, B, num)
+        bounds = _per_clip("boundary", boundary, B, num)
+        if randomize_seed:
+            seeds = [random.randint(0, MAX_SEED) for _ in range(B)]
+        elif random_seed is None:
+            seeds = None
+        else:
+            seeds = [int(v) for v in _per_clip("random_seed", random_seed, B, num)]
+        empty = [t == "" for t in prompts]
+        if any(empty) and not all(empty):
+            raise ValueError("empty prompts run without guidance: they cannot share a batch with non-empty ones")
+        if all(empty):
+            guidance_scale = None
+            print("empyt input")
+        if any(v < 0 for v in starts) or any(v <= 0 for v in lengths_s) or any(v < 0 for v in bounds):
+            raise ValueError("mask_start and boundary must be >= 0 and mask_length > 0 for every edit")
+        raws = [_load_audio(f, sr) if isinstance(f, str) else np.asarray(f, dtype=np.float32) for f in files]
+        if any(r.ndim != 1 or len(r) < 1 for r in raws):
+            raise ValueError("every gt_file must be a non-empty mono waveform")
+        plans = [edit_plan(len(r), sr, latent_sr, hop, bd, ms, ml) for r, bd, ms, ml in zip(raws, bounds, starts, lengths_s)]
+        frames = [p["frames"] for p in plans]
+        max_frames = int(round(self.max_length_s * latent_sr))
+        if pad_length is not None and pad_length > self.max_length_s:
+            raise ValueError(f"pad_length {pad_length} s exceeds max_length_s {self.max_length_s} s")
+        L = max(frames) if pad_length is None else int(pad_length * latent_sr)
+        if min(frames) < 1 or max(frames) > L or L > max_frames:
+            raise ValueError(f"crops of {frames} latent frames must be non-empty and fit the padded length ({L} frames, at most {max_frames}: "
+                             f"max_length_s {self.max_length_s} s)")
+        # ---- per clip: normalise + pad on the device, crop into the padded batch
+        outs, crops = [], torch.zeros(B, 1, L * hop, device=self.device)
+        for b, (r, p) in enumerate(zip(raws, plans)):
+            o = post.prepare_wave(torch.from_numpy(r).to(self.device).unsqueeze(0), p["n_total"], normalize=True)[0]
+            crops[b, 0, :p["s1"] - p["s0"]] = o[p["s0"]:p["s1"]]
+            outs.append(o)
+        gt_latent = self.autoencoder(audio=crops, lengths=frames)   # clip b's bottleneck noise: (1, C, frames[b]) from the global RNG, in order
+        gt_mask = torch.zeros(B, gt_latent.shape[1], L, device=self.device)
+        for b, p in enumerate(plans):
+            gt_mask[b, :, p["m0"]:p["m1"]] = 1
+            gt_mask[b, :, frames[b]:] = 1
+        embeds = self._text_embeds(prompts, [""])
+        wavs = inference(self.autoencoder, self.unet, gt_latent, gt_mask.bool(), None, None, self.params, self.noise_scheduler, prompts, None, L,
+                         guidance_scale, guidance_rescale, ddim_steps, eta, seeds, self.device, text_embeds=embeds, lengths=frames, padded_gt=True)
+        for o, w, p in zip(outs, wavs, plans):
+            post.splice_wave(o, w[0], p["s0"], p["n_paste"])
+        return sr, [o.cpu().numpy() for o in outs]
 
 
 def energy_condition(audio: torch.Tensor, hop_size=240, window_size=1920, padding="reflect", min_db=-60, norm=True, quantize_levels=None,

@@ -689,6 +689,14 @@ EZB_API int ezb_vae_decode(ezb_vae* h, const float* z, float* wav, int B, int L,
   if (!h || !z || !wav) return fail(EZB_ERR_ARG, "ezb_vae_decode: null argument");
   return reinterpret_cast<Vae*>(h)->decode(z, wav, B, L, ST(stream));
 }
+EZB_API int ezb_vae_decode_lens(ezb_vae* h, const float* z, float* wav, int B, int L, const int32_t* lens, void* stream) {
+  if (!h || !z || !wav || !lens) return fail(EZB_ERR_ARG, "ezb_vae_decode_lens: null argument");
+  return reinterpret_cast<Vae*>(h)->decode(z, wav, B, L, ST(stream), lens);
+}
+EZB_API int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noise, float* z, int B, int T, const int32_t* lens, void* stream) {
+  if (!h || !audio || !z || !lens) return fail(EZB_ERR_ARG, "ezb_vae_encode_lens: null argument");
+  return reinterpret_cast<Vae*>(h)->encode(audio, noise, z, B, T, ST(stream), lens);
+}
 }  // extern "C"
 
 namespace {

@@ -323,6 +323,44 @@ struct EpiLinear {
   }
 };
 
+// EpiLinear for the convs of a padded batch of clips of different lengths (conv addressing only: rows are (clip, t), rows_per_clip per
+// clip, and a tile never straddles clips).  Clip b ends at row end = clamp(lens[b], 1, max_len) * frame_rows of this layer.  Rows below it
+// go through EpiLinear with the row count a run of that clip alone at its own length has (nvalid = end - t0), so they are the same bits;
+// rows at or past it are stored as zeros to out_bf16 ([hi | lo | hi] included) -- the operand the next conv reads is then the zero halo
+// the TMA fill gives the solo run -- and out_f32 is not written there.  lens is read when the kernel runs.
+struct EpiLinearLensParams {
+  EpiLinearParams lin;
+  const int32_t* lens;     // [B] device, latent frames per clip
+  int rows_per_clip;       // GEMM rows per clip (ConvAddr::T)
+  int max_len;             // padded length in latent frames
+  int frame_rows;          // GEMM rows of this layer per latent frame
+};
+template <int BN>
+struct EpiLinearLens {
+  using Params = EpiLinearLensParams;
+  static constexpr int EPI_WARPS = EpiLinear<BN>::EPI_WARPS;
+  static constexpr bool WIDE_REGS = false;
+  static constexpr int STAGE_FLOATS = EPI_STAGE_FLOATS;
+  template <class Wait>
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+                                             int c_end, Wait wait) {
+    if (nvalid <= 0) { wait(); return; }   // this warp's rows lie past the padded length (row0 may belong to the next clip)
+    const int b = row0 / ep.rows_per_clip, t0 = row0 - b * ep.rows_per_clip;
+    const int end = min(max(ep.lens[b], 1), ep.max_len) * ep.frame_rows;
+    const int live = min(nvalid, end - t0);
+    EpiLinear<BN>::run(ep.lin, st, ar, row0, live, n0, N, lane, c_begin, c_end, wait);
+    const EpiLinearParams& e = ep.lin;
+    const int nv = nvalid < 32 ? nvalid : 32;
+    if (e.out_bf16 == nullptr || live >= nv) return;
+    for (int c = c_begin; c < c_end; c += 64) {
+      const int col = n0 + c + 2 * lane;
+      if (c + 2 * lane >= c_end || col >= N) continue;
+      const int c16 = e.phase_cols > 0 ? (col / e.phase_cols) * e.phase_ld16 + col % e.phase_cols : col;
+      for (int rr = live > 0 ? live : 0; rr < nv; ++rr) store_bf16x2(e.out_bf16 + (size_t)(row0 + rr) * e.ld16 + c16, e.split_stride, 0.f, 0.f);
+    }
+  }
+};
+
 // GEGLU (src/models/utils/modules.py:274-277): W rows are packed so that an N-tile of BN columns holds BN/2 hidden
 // features followed by the BN/2 matching gate features; out[row, n0/2 + j] = (h_j + bh_j) * gelu_erf(g_j + bg_j).
 struct EpiGegluParams {

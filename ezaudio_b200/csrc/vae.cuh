@@ -61,6 +61,11 @@ __global__ void snake_prep_kernel(const float* __restrict__ alpha, const float* 
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < C) { a[i] = expf(alpha[i]); binv[i] = 1.0f / (expf(beta[i]) + 1e-9f); }
 }
+// Per-sample clip ends (padded batch, lens [B] device int32 in latent frames, read when the kernel runs and clamped to [1, L]): the
+// length-aware kernels below treat everything at or past a clip's end as the zero padding a run of that clip alone sees, and write zeros
+// there.
+__device__ __forceinline__ int clip_frames(const int32_t* lens, int b, int L) { return min(max(lens[b], 1), L); }
+
 // z (B, C, L) fp32 -> channels-last bf16 [B, L, kmul*C]
 __global__ void latent_pack_kernel(const float* __restrict__ z, __nv_bfloat16* __restrict__ out, int C, int L, int kmul) {
   __shared__ float tile[32][33];
@@ -68,6 +73,21 @@ __global__ void latent_pack_kernel(const float* __restrict__ z, __nv_bfloat16* _
   for (int i = threadIdx.y; i < 32; i += 8) {
     const int c = c0 + i, l = l0 + threadIdx.x;
     tile[i][threadIdx.x] = (c < C && l < L) ? z[((size_t)b * C + c) * L + l] : 0.f;
+  }
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += 8) {
+    const int l = l0 + i, c = c0 + threadIdx.x;
+    if (l < L && c < C) store_act(out + ((size_t)b * L + l) * kmul * C, c, C, kmul, tile[threadIdx.x][i]);
+  }
+}
+// latent_pack_kernel for a padded batch: frames at or past the clip's end are written as zeros and never read (they may hold NaN)
+__global__ void latent_pack_lens_kernel(const float* __restrict__ z, __nv_bfloat16* __restrict__ out, int C, int L, int kmul, const int32_t* __restrict__ lens) {
+  __shared__ float tile[32][33];
+  const int b = blockIdx.z, l0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const int Lv = clip_frames(lens, b, L);
+  for (int i = threadIdx.y; i < 32; i += 8) {
+    const int c = c0 + i, l = l0 + threadIdx.x;
+    tile[i][threadIdx.x] = (c < C && l < Lv) ? z[((size_t)b * C + c) * L + l] : 0.f;
   }
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += 8) {
@@ -148,6 +168,14 @@ __global__ void __launch_bounds__(128, 3) wave_out_kernel(const __nv_bfloat16* _
   }
   if (t0 + lane < T) wav[(size_t)b * T + t0 + lane] = acc[0];
 }
+// Padded batch: wave_out_kernel runs as it is -- the activated rows at or past a clip's end are zeros already (EpiLinearLens), which is
+// the zero padding the clip alone sees, so the samples before the end need nothing new -- and this kernel then zeroes the samples of wav
+// [B, T] at or past it (hop samples per latent frame; the few just past the end hold the conv's reach into the clip).
+__global__ void wave_tail_zero_kernel(float* __restrict__ wav, int T, const int32_t* __restrict__ lens, int hop) {
+  const int b = blockIdx.y;
+  const int t = clip_frames(lens, b, T / hop) * hop + blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < T) wav[(size_t)b * T + t] = 0.f;
+}
 __global__ void fold_wave_w_kernel(const float* __restrict__ v, const float* __restrict__ g, const float* __restrict__ norms, float* __restrict__ w, int C) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // v [1, C, 7] -> w [7][C]
   if (i < 7 * C) { const int k = i / C, c = i - k * C; w[i] = g[0] * v[c * 7 + k] / norms[0]; }
@@ -155,38 +183,67 @@ __global__ void fold_wave_w_kernel(const float* __restrict__ v, const float* __r
 
 // encoder stem: Conv1d(1 -> C0, k=7, pad 3) on the raw waveform (autoencoders.py:133) -> channels-last fp32 residual stream
 // + bf16 SnakeBeta(next) operand.  w folded fp32 [7][C0].
-__global__ void enc_conv_in_kernel(const float* __restrict__ audio, const float* __restrict__ w, const float* __restrict__ bias, const float* __restrict__ sa,
-                                   const float* __restrict__ sb, float* __restrict__ raw, __nv_bfloat16* __restrict__ act, int C, int T, int kmul) {
+// LENS: samples at or past the clip's end (hop per latent frame) read as zero, whatever the buffer holds there, and rows at or past it get
+// a zero activation (they would be snake(bias)); raw is not written there.
+template <bool LENS>
+__device__ __forceinline__ void enc_conv_in_body(const float* __restrict__ audio, const float* __restrict__ w, const float* __restrict__ bias,
+                                                 const float* __restrict__ sa, const float* __restrict__ sb, float* __restrict__ raw,
+                                                 __nv_bfloat16* __restrict__ act, int C, int T, int kmul, const int32_t* lens, int hop) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (i >= (size_t)T * C) return;
   const int t = i / C, c = i - (size_t)t * C;
+  const int end = LENS ? clip_frames(lens, b, T / hop) * hop : T;
+  if (LENS && t >= end) {
+    store_act(act + ((size_t)b * T + t) * kmul * C, c, C, kmul, 0.f);
+    return;
+  }
   const float* a = audio + (size_t)b * T;
   float v = bias[c];
 #pragma unroll
   for (int k = 0; k < 7; ++k) {
     const int tt = t + k - 3;
-    if (tt >= 0 && tt < T) v = fmaf(w[k * C + c], a[tt], v);
+    if (tt >= 0 && tt < end) v = fmaf(w[k * C + c], a[tt], v);
   }
   raw[((size_t)b * T + t) * C + c] = v;
   const float sn = sinf(v * sa[c]);
   store_act(act + ((size_t)b * T + t) * kmul * C, c, C, kmul, v + sb[c] * sn * sn);
+}
+__global__ void enc_conv_in_kernel(const float* __restrict__ audio, const float* __restrict__ w, const float* __restrict__ bias, const float* __restrict__ sa,
+                                   const float* __restrict__ sb, float* __restrict__ raw, __nv_bfloat16* __restrict__ act, int C, int T, int kmul) {
+  enc_conv_in_body<false>(audio, w, bias, sa, sb, raw, act, C, T, kmul, nullptr, 1);
+}
+__global__ void enc_conv_in_lens_kernel(const float* __restrict__ audio, const float* __restrict__ w, const float* __restrict__ bias,
+                                        const float* __restrict__ sa, const float* __restrict__ sb, float* __restrict__ raw, __nv_bfloat16* __restrict__ act,
+                                        int C, int T, int kmul, const int32_t* __restrict__ lens, int hop) {
+  enc_conv_in_body<true>(audio, w, bias, sa, sb, raw, act, C, T, kmul, lens, hop);
 }
 __global__ void fold_conv_in_w_kernel(const float* __restrict__ v, const float* __restrict__ g, const float* __restrict__ norms, float* __restrict__ w, int C) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // v [C, 1, 7] -> w [7][C]
   if (i < 7 * C) { const int k = i / C, c = i - k * C; w[i] = g[c] * v[c * 7 + k] / norms[c]; }
 }
 // VAEBottleneck.encode (bottleneck.py:66-70,77-87): enc [B*L, 2*Cz] channels-last (mean | scale) -> z (B, Cz, L)
-__global__ void vae_sample_kernel(const float* __restrict__ enc, const float* __restrict__ noise, float* __restrict__ z, int Cz, int L) {
+// LENS: z frames at or past the clip's end are zeros (enc rows there are not read: the encoder's last conv leaves them unwritten)
+template <bool LENS>
+__device__ __forceinline__ void vae_sample_body(const float* __restrict__ enc, const float* __restrict__ noise, float* __restrict__ z, int Cz, int L,
+                                                const int32_t* lens) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (i >= (size_t)Cz * L) return;
   const int c = i / L, l = i - (size_t)c * L;
+  if (LENS && l >= clip_frames(lens, b, L)) { z[((size_t)b * Cz + c) * L + l] = 0.f; return; }
   const float* row = enc + ((size_t)b * L + l) * 2 * Cz;
   const float mean = row[c], sc = row[Cz + c];
   const float sp = sc > 20.f ? sc : log1pf(expf(sc));  // F.softplus (threshold 20)
   const float nz = noise ? noise[((size_t)b * Cz + c) * L + l] : 0.f;
   z[((size_t)b * Cz + c) * L + l] = nz * (sp + 1e-4f) + mean;
+}
+__global__ void vae_sample_kernel(const float* __restrict__ enc, const float* __restrict__ noise, float* __restrict__ z, int Cz, int L) {
+  vae_sample_body<false>(enc, noise, z, Cz, L, nullptr);
+}
+__global__ void vae_sample_lens_kernel(const float* __restrict__ enc, const float* __restrict__ noise, float* __restrict__ z, int Cz, int L,
+                                       const int32_t* __restrict__ lens) {
+  vae_sample_body<true>(enc, noise, z, Cz, L, lens);
 }
 
 struct VaeConv {  // one packed conv / conv-transpose
@@ -269,8 +326,10 @@ inline int vae_fold_conv_in_w(cudaStream_t st, const float* v, const float* g, f
 // One implicit-GEMM conv: A [B, T_in, kmul*cin] -> raw_out fp32 [B*T, N] (pre-activation, + resid_in when given) and act_out bf16
 // [B, T * phases, kmul*cout] (SnakeBeta(snake) of it, [hi | lo | hi] in bf16x3).  T: input rows, except for a strided conv (output rows,
 // the input has T * stride).  resid_in may alias raw_out.
+// lens (device [B], or null): clips of lens[b] <= max_len latent frames, frame_rows = T / max_len GEMM rows each, in a batch padded to T
+// rows: the EpiLinearLens kernel, which zeroes act_out past each clip's end and leaves raw_out unwritten there.
 inline int vae_conv(Device& dev, cudaStream_t st, const VaeConv& c, int kmul, const __nv_bfloat16* A, int B, int T, const float* resid_in,
-                    float* raw_out, __nv_bfloat16* act_out, const VaeSnake* snake) {
+                    float* raw_out, __nv_bfloat16* act_out, const VaeSnake* snake, const int32_t* lens = nullptr, int max_len = 0) {
   EpiLinearParams e;
   memset(&e, 0, sizeof e);
   e.bias = c.bias;
@@ -288,41 +347,55 @@ inline int vae_conv(Device& dev, cudaStream_t st, const VaeConv& c, int kmul, co
   ca.taps = c.taps; ca.center = c.center; ca.dilation = c.dil; ca.cin_pad = c.cin_pad; ca.T = T; ca.B = B;
   if (c.stride > 1 && c.N == c.cout) { ca.stride = c.stride; ca.pad = c.center; }  // strided conv (T = output length); conv-transpose has N = s*cout
   const int ld = c.taps * c.cin_pad;
+  if (lens != nullptr) {
+    if (max_len < 1 || T % max_len) return fail(EZB_ERR_SHAPE, "vae_conv: %d rows per clip are not a multiple of the %d padded frames", T, max_len);
+    const EpiLinearLensParams el{e, lens, T, max_len, T / max_len};
+    return gemm<128, EpiLinearLens<128>>(dev, st, A, kmul * c.cin, c.w, ld, B * T, c.N, kmul * c.cin, el, &ca);
+  }
   return gemm<128, EpiLinear<128>>(dev, st, A, kmul * c.cin, c.w, ld, B * T, c.N, kmul * c.cin, e, &ca);
 }
 
 // z (B, C, L) fp32 -> act [B, L, kmul*C]
-inline int vae_latent_pack(cudaStream_t st, const float* z, __nv_bfloat16* act, int B, int C, int L, int kmul) {
+inline int vae_latent_pack(cudaStream_t st, const float* z, __nv_bfloat16* act, int B, int C, int L, int kmul, const int32_t* lens = nullptr) {
   dim3 grid((L + 31) / 32, (C + 31) / 32, B), blk(32, 8);
   ++launch_counter();
-  latent_pack_kernel<<<grid, blk, 0, st>>>(z, act, C, L, kmul);
+  if (lens != nullptr) latent_pack_lens_kernel<<<grid, blk, 0, st>>>(z, act, C, L, kmul, lens);
+  else latent_pack_kernel<<<grid, blk, 0, st>>>(z, act, C, L, kmul);
   EZB_CUDA(cudaGetLastError());
   return EZB_OK;
 }
 // act [B, T, kmul*C] -> wav [B, T], w folded [7][C]
-inline int vae_wave_out(cudaStream_t st, const __nv_bfloat16* act, const float* w, float* wav, int B, int C, int T, int kmul) {
+// lens (device [B] latent frames of `hop` samples, or null): samples at or past a clip's end are zeroed by a second launch
+inline int vae_wave_out(cudaStream_t st, const __nv_bfloat16* act, const float* w, float* wav, int B, int C, int T, int kmul,
+                        const int32_t* lens = nullptr, int hop = 1) {
   if (C % 4) return fail(EZB_ERR_UNSUPPORTED, "wave_out: %d channels in the last stage (multiple of 4 expected)", C);
   dim3 g2((T + 127) / 128, B);
   ++launch_counter();
   if (kmul == 3) wave_out_kernel<3><<<g2, 128, 0, st>>>(act, w, wav, C, T);
   else wave_out_kernel<1><<<g2, 128, 0, st>>>(act, w, wav, C, T);
+  if (lens != nullptr) {
+    ++launch_counter();
+    wave_tail_zero_kernel<<<dim3((T - hop + 255) / 256 + 1, B), 256, 0, st>>>(wav, T, lens, hop);
+  }
   EZB_CUDA(cudaGetLastError());
   return EZB_OK;
 }
 // audio [B, T] -> raw [B, T, C] fp32 and act = SnakeBeta(snake) [B, T, kmul*C], w folded [7][C]
 inline int vae_enc_conv_in(cudaStream_t st, const float* audio, const float* w, const float* bias, const VaeSnake& snake, float* raw,
-                           __nv_bfloat16* act, int B, int C, int T, int kmul) {
+                           __nv_bfloat16* act, int B, int C, int T, int kmul, const int32_t* lens = nullptr, int hop = 1) {
   dim3 grid((unsigned)(((size_t)T * C + 255) / 256), B);
   ++launch_counter();
-  enc_conv_in_kernel<<<grid, 256, 0, st>>>(audio, w, bias, snake.a, snake.binv, raw, act, C, T, kmul);
+  if (lens != nullptr) enc_conv_in_lens_kernel<<<grid, 256, 0, st>>>(audio, w, bias, snake.a, snake.binv, raw, act, C, T, kmul, lens, hop);
+  else enc_conv_in_kernel<<<grid, 256, 0, st>>>(audio, w, bias, snake.a, snake.binv, raw, act, C, T, kmul);
   EZB_CUDA(cudaGetLastError());
   return EZB_OK;
 }
 // enc [B*L, 2*Cz] (mean | scale) -> z (B, Cz, L)
-inline int vae_sample(cudaStream_t st, const float* enc, const float* noise, float* z, int B, int Cz, int L) {
+inline int vae_sample(cudaStream_t st, const float* enc, const float* noise, float* z, int B, int Cz, int L, const int32_t* lens = nullptr) {
   dim3 g2((unsigned)(((size_t)Cz * L + 255) / 256), B);
   ++launch_counter();
-  vae_sample_kernel<<<g2, 256, 0, st>>>(enc, noise, z, Cz, L);
+  if (lens != nullptr) vae_sample_lens_kernel<<<g2, 256, 0, st>>>(enc, noise, z, Cz, L, lens);
+  else vae_sample_kernel<<<g2, 256, 0, st>>>(enc, noise, z, Cz, L);
   EZB_CUDA(cudaGetLastError());
   return EZB_OK;
 }
@@ -531,13 +604,18 @@ struct Vae {
     return EZB_OK;
   }
 
+  // lens / lens_max: the per-clip lengths of the encode / decode in flight (null: every clip fills the batch's length)
+  const int32_t* lens = nullptr;
+  int lens_max = 0;
   int run_conv(cudaStream_t st, const VaeConv& c, const __nv_bfloat16* A, int B, int T, const float* resid_in, float* raw_out, __nv_bfloat16* act_out,
                const VaeSnake* snake) {
-    return vae_conv(*dev, st, c, kmul, A, B, T, resid_in, raw_out, act_out, snake);
+    return vae_conv(*dev, st, c, kmul, A, B, T, resid_in, raw_out, act_out, snake, lens, lens_max);
   }
 
-  // audio (B, 1, T) fp32, T = hop * L; noise (B, latent, L) fp32 or null (-> mean); z (B, latent, L) fp32
-  int encode(const float* audio, const float* noise, float* z, int B, int T, cudaStream_t st) {
+  // audio (B, 1, T) fp32, T = hop * L; noise (B, latent, L) fp32 or null (-> mean); z (B, latent, L) fp32.
+  // lens_ (device [B] latent frames, or null): clip b is its first hop * lens_[b] samples; its z frames come out as an encode of the
+  // clip alone at that length, the frames past it as zeros, whatever audio and noise hold past the end.
+  int encode(const float* audio, const float* noise, float* z, int B, int T, cudaStream_t st, const int32_t* lens_ = nullptr) {
     if (!finalized || !d.with_encoder) return fail(EZB_ERR_STATE, "VAE encoder weights not loaded");
     int hop = 1;
     for (int j = 0; j < nst; ++j) hop *= e_stride[j];
@@ -546,7 +624,8 @@ struct Vae {
     if (B < 1 || B > d.max_batch || L < 1 || L > d.max_latent_len) return fail(EZB_ERR_SHAPE, "vae_encode: B %d L %d exceed workspace", B, L);
     const int C0 = e_cin[0];
     __nv_bfloat16 *cur = actA, *oth = actB;
-    EZB_TRY(vae_enc_conv_in(st, audio, e_in_w, e_in_b, e_res_s0[0], resid, cur, B, C0, T, kmul));
+    lens = lens_; lens_max = L;
+    EZB_TRY(vae_enc_conv_in(st, audio, e_in_w, e_in_b, e_res_s0[0], resid, cur, B, C0, T, kmul, lens, hop));
     int Tc = T;
     for (int j = 0; j < nst; ++j) {
       for (int u = 0; u < 3; ++u) {
@@ -562,13 +641,16 @@ struct Vae {
       std::swap(cur, oth);
     }
     EZB_TRY(run_conv(st, e_out, cur, B, Tc, nullptr, resid, nullptr, nullptr));  // (mean | scale), channels-last fp32
-    return vae_sample(st, resid, noise, z, B, d.latent_dim, L);
+    return vae_sample(st, resid, noise, z, B, d.latent_dim, L, lens);
   }
 
-  int decode(const float* z, float* wav, int B, int L, cudaStream_t st) {
+  // lens_ (device [B] latent frames, or null): clip b is its first lens_[b] frames; its hop * lens_[b] samples come out as a decode of the
+  // clip alone at that length, the samples past them as zeros, whatever z holds past the end (NaN included).
+  int decode(const float* z, float* wav, int B, int L, cudaStream_t st, const int32_t* lens_ = nullptr) {
     if (!finalized) return fail(EZB_ERR_STATE, "VAE weights not finalized");
     if (B < 1 || B > d.max_batch || L < 1 || L > d.max_latent_len) return fail(EZB_ERR_SHAPE, "vae_decode: B %d L %d exceed workspace", B, L);
-    EZB_TRY(vae_latent_pack(st, z, actA, B, d.latent_dim, L, kmul));
+    lens = lens_; lens_max = L;
+    EZB_TRY(vae_latent_pack(st, z, actA, B, d.latent_dim, L, kmul, lens));
     __nv_bfloat16 *cur = actA, *oth = actB;
     int T = L;
     EZB_TRY(run_conv(st, conv_in, cur, B, T, nullptr, nullptr, oth, &up_snake[0]));
@@ -585,7 +667,7 @@ struct Vae {
         EZB_TRY(run_conv(st, res1[3 * j + u], oth, B, T, resid, last ? nullptr : resid, cur, nxt));
       }
     }
-    return vae_wave_out(st, cur, out_w, wav, B, cout_s[nst - 1], T, kmul);
+    return vae_wave_out(st, cur, out_w, wav, B, cout_s[nst - 1], T, kmul, lens, T / L);
   }
 };
 

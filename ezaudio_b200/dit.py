@@ -216,8 +216,10 @@ class MaskDiT:
         `lengths` (out-of-range rows are clamped, the caller validates them)."""
         Be, Cc, L = x.shape
         if lengths is not None:
-            if gt is not None or controlnet_skips is not None:
-                raise NotImplementedError("per-sample lengths with inpainting (gt) or ControlNet skips")
+            if controlnet_skips is not None:
+                raise NotImplementedError("per-sample lengths with ControlNet skips")
+            if gt is not None and gt_mask_u8 is None:   # the padded frames of gt must be marked as regenerated, which takes a mask
+                raise NotImplementedError("per-sample lengths with inpainting (gt) need gt_mask_u8, set past each clip's end")
             if lengths.dtype != torch.int32 or not lengths.is_cuda or tuple(lengths.shape) != (Be,) or not lengths.is_contiguous():
                 raise ValueError(f"lengths must be a contiguous cuda int32 tensor of shape ({Be},)")
         if t_index is not None and (t_index.dtype != torch.int32 or not t_index.is_cuda or tuple(t_index.shape) != (Be,) or not t_index.is_contiguous()):

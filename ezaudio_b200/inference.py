@@ -6,7 +6,8 @@ Differences from the reference loop, all additive:
   * step-invariant work (context embedding, cross-attention K/V, timestep/AdaLN tables) is computed once per clip;
   * CFG + rescale + DDIM update is one fused kernel (ezb_cfg_ddim_step);
   * clips of different lengths in one batch (`lengths=`): the batch is padded to `audio_frames` and every prompt's frames come out as
-    that prompt run alone at its own length computes them (same seed, same bits).
+    that prompt run alone at its own length computes them (same seed, same bits); one length-aware VAE decode turns the padded batch into
+    waveforms.  Inpainting joins in with `padded_gt=True`: gt / gt_mask padded like the batch, ignored past each clip's end.
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -43,10 +44,13 @@ def _ddim_step(model_out, latents, noise, B, Cc, L, gs, gr, coef, lens=None):
                                             arr, _lib.stream_ptr(), _lib.ptr(lens)))
 
 
-def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None):
-    """Validates per-prompt clip lengths (frames) against the batch size and the padded length L, on the host, before any device work."""
-    if gt is not None:
-        raise NotImplementedError("per-prompt lengths with inpainting (gt) are not supported")
+def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None, padded_gt=False):
+    """Validates per-prompt clip lengths (frames) against the batch size and the padded length L, on the host, before any device work.
+    Inpainting goes with lengths only when the caller states, with `padded_gt=True`, that `gt` (and its mask) is the padded (B,C,L) batch
+    whose frames past each clip's end are to be ignored; a ControlNet never does."""
+    if gt is not None and not padded_gt:
+        raise NotImplementedError("per-prompt lengths with inpainting (gt) need padded_gt=True: gt / gt_mask padded to the batch's length, "
+                                  "ignored past each clip's end")
     if controlnet is not None:
         raise NotImplementedError("per-prompt lengths with a ControlNet are not supported: its stem convolutions cross the clip ends")
     lens = [int(v) for v in lengths]
@@ -56,6 +60,8 @@ def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None):
         raise ValueError(f"lengths lists one length per prompt: got {len(lens)} for {B} prompts")
     if any(v < 1 or v > L for v in lens):
         raise ValueError(f"every length must lie in 1..{L} (the padded length), got {lens}")
+    if gt is not None and (tuple(gt.shape[:1]) + tuple(gt.shape[2:])) != (B, L):
+        raise ValueError(f"gt must be the padded batch ({B}, C, {L}), got {tuple(gt.shape)}")
     return lens
 
 
@@ -63,7 +69,7 @@ def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None):
 def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, gt=None, gt_mask=None,
                    audio_frames=500, guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024,
                    controlnet=None, condition=None, conditioning_scale=1.0, init_noise=None, step_noise=None, device=None,
-                   use_graphs=True, paste_gt=True, lengths=None):
+                   use_graphs=True, paste_gt=True, lengths=None, padded_gt=False):
     """Denoising loop on cached text embeddings.  text (B,Lc,ctx) / text_mask (B,Lc); uncond_* (1 or B rows) when
     guidance_scale is truthy.  gt / gt_mask (B,C,L) for inpainting.  Returns the final latents (B,C,L) fp32 on device.
     `init_noise` / `step_noise` inject the RNG draws (parity tests); otherwise per-prompt generators are used.
@@ -72,9 +78,12 @@ def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, unc
     `lengths`: one clip length (frames, 1..audio_frames) per prompt, or None.  The batch is padded to `audio_frames`; prompt b's initial
     noise and per-step draws are made at its own shape (1, C, lengths[b]), so its frames < lengths[b] of the result equal a run of that
     prompt alone at audio_frames = lengths[b] with the same seed (random_seed must then be per-prompt or None; injected noise is not
-    accepted).  Frames past a prompt's length are zero.  One captured graph serves every mix of lengths at the same padded length."""
+    accepted).  Frames past a prompt's length are zero.  One captured graph serves every mix of lengths at the same padded length.
+    gt / gt_mask go with lengths under `padded_gt=True` (refused without it): both are padded to audio_frames like the batch, the solo run
+    is the one with gt[b:b+1, :, :lengths[b]] and the same slice of
+    the mask; what gt and gt_mask hold past a clip's end is ignored."""
     if lengths is not None:
-        lengths = check_lengths(lengths, text.shape[0], int(audio_frames), gt, controlnet)
+        lengths = check_lengths(lengths, text.shape[0], int(audio_frames), gt, controlnet, padded_gt)
         if init_noise is not None or step_noise is not None:
             raise ValueError("lengths draws the noise per prompt: init_noise / step_noise cannot be injected")
     dev_index = unet._h.dev_index   # the loop runs where the denoiser's weights live
@@ -83,6 +92,11 @@ def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, unc
         if d.type != "cuda" or (d.index is not None and d.index != dev_index):
             raise ValueError(f"sample_latents(device={d}) but the denoiser lives on cuda:{dev_index}")
     device = torch.device("cuda", dev_index)
+    if lengths is not None and gt is not None:   # past a clip's end nothing of gt is used: those frames count as regenerated
+        gt, gt_mask = gt.to(device=device, dtype=torch.float32).clone(), gt_mask.to(device).bool().clone()
+        for b, n in enumerate(lengths):
+            gt[b, :, n:] = 0
+            gt_mask[b, ..., n:] = True
     # every launch below (noise draws, the C-ABI calls, graph capture and replay) targets `device`, whatever the caller's current device is
     with torch.cuda.device(device):
         lat = _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
@@ -244,13 +258,14 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
 @torch.no_grad()
 def inference(autoencoder, unet, gt, gt_mask, tokenizer, text_encoder, params, noise_scheduler, text_raw, neg_text=None,
               audio_frames=500, guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device="cuda",
-              text_embeds=None, controlnet=None, condition=None, conditioning_scale=1.0, lengths=None):
+              text_embeds=None, controlnet=None, condition=None, conditioning_scale=1.0, lengths=None, padded_gt=False):
     """Signature of src/inference.py:26-37 (+ keyword-only extensions).  Returns the waveform tensor (B,1,480*L).
     With `lengths` (one clip length in frames per prompt, batch padded to audio_frames; see sample_latents) it returns a list of B
-    waveforms (1, 480*lengths[b]): the VAE decodes each group of equal lengths at that length, because its receptive field crosses the
-    clip end."""
+    waveforms (1, 480*lengths[b]) from one length-aware VAE decode of the padded batch (each equal to the decode of that clip alone).
+    gt / gt_mask go with lengths under `padded_gt=True`, as in sample_latents: padded to audio_frames, ignored past each clip's end."""
     if lengths is not None:
-        lengths = check_lengths(lengths, len(text_raw) if text_embeds is None else text_embeds[0].shape[0], int(audio_frames), gt, controlnet)
+        lengths = check_lengths(lengths, len(text_raw) if text_embeds is None else text_embeds[0].shape[0], int(audio_frames), gt, controlnet,
+                                padded_gt)
     if neg_text is None:
         neg_text = [""]
     if text_embeds is not None:
@@ -261,16 +276,12 @@ def inference(autoencoder, unet, gt, gt_mask, tokenizer, text_encoder, params, n
         raise ValueError("either tokenizer/text_encoder or text_embeds is required (the denoiser is text-conditioned)")
     latents = sample_latents(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
                              guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, device=device, paste_gt=False,
-                             lengths=lengths)
+                             lengths=lengths, padded_gt=padded_gt)
     pred = scale_shift_re(latents, params["autoencoder"]["scale"], params["autoencoder"]["shift"])
-    if lengths is not None:
-        wavs = [None] * len(lengths)
-        for n in sorted(set(lengths)):
-            idx = [b for b, v in enumerate(lengths) if v == n]
-            w = autoencoder(embedding=pred[idx, :, :n].contiguous())
-            for j, b in enumerate(idx):
-                wavs[b] = w[j]
-        return wavs
     if gt is not None:  # src/inference.py:104-105: pred[~gt_mask] = gt[~gt_mask], with the raw gt, after the rescale
         pred = torch.where(gt_mask.to(pred.device).bool().expand_as(pred), pred, gt.to(device=pred.device, dtype=pred.dtype))
+    if lengths is not None:   # what the paste put past a clip's end is never read by the decode
+        w = autoencoder(embedding=pred, lengths=lengths)
+        hop = w.shape[-1] // pred.shape[-1]
+        return [w[b, :, :hop * n] for b, n in enumerate(lengths)]
     return autoencoder(embedding=pred)

@@ -70,21 +70,45 @@ class OobleckDecoder:
             _lib.check(L.ezb_vae_finalize_weights(self.h, st))
         return self
 
-    def __call__(self, z: torch.Tensor) -> torch.Tensor:
+    def _lens(self, lengths, B: int, L: int):
+        """lengths (list of ints, or a cuda int32 tensor read on the device when the kernels run) -> (device int32 [B], host list or None).
+        A list is validated here, before any device work; a tensor's values are the caller's to validate (the kernels clamp to 1..L)."""
+        if isinstance(lengths, torch.Tensor):
+            if lengths.dtype != torch.int32 or not lengths.is_cuda or tuple(lengths.shape) != (B,) or not lengths.is_contiguous():
+                raise ValueError(f"lengths must be a contiguous cuda int32 tensor of shape ({B},)")
+            return lengths, None
+        host = [int(v) for v in lengths]
+        if len(host) != B or any(v != w for v, w in zip(host, lengths)) or any(v < 1 or v > L for v in host):
+            raise ValueError(f"lengths lists one whole frame count in 1..{L} per clip ({B} clips), got {list(lengths)}")
+        return torch.tensor(host, dtype=torch.int32).to(self.device), host
+
+    def __call__(self, z: torch.Tensor, lengths=None) -> torch.Tensor:
+        """z (B,latent,L) -> (B,1,hop*L).  `lengths` (latent frames per clip, a list or a cuda int32 tensor): z is a padded batch; clip b's
+        hop * lengths[b] samples equal the decode of z[b:b+1, :, :lengths[b]] alone, bit for bit, whatever the padded frames hold, and the
+        samples past them are zeros."""
         z = _as_f32c(z).to(self.device)
         B, Cz, L = z.shape
+        lens = None if lengths is None else self._lens(lengths, B, L)[0]
         wav = torch.empty(B, 1, L * self.hop, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.dev_index):
             for b0 in range(0, B, self.max_batch):
                 nb = min(self.max_batch, B - b0)
-                _lib.check(_lib.lib().ezb_vae_decode(self.h, _lib.ptr(z[b0:b0 + nb]), C.c_void_p(wav[b0:b0 + nb].data_ptr()), nb, L, _lib.stream_ptr()))
+                zs, ws = _lib.ptr(z[b0:b0 + nb]), C.c_void_p(wav[b0:b0 + nb].data_ptr())
+                if lens is None:
+                    _lib.check(_lib.lib().ezb_vae_decode(self.h, zs, ws, nb, L, _lib.stream_ptr()))
+                else:
+                    _lib.check(_lib.lib().ezb_vae_decode_lens(self.h, zs, ws, nb, L, _lib.ptr(lens[b0:b0 + nb]), _lib.stream_ptr()))
         return wav
 
     forward = __call__
 
-    def encode(self, audio: torch.Tensor, noise=None) -> torch.Tensor:
+    def encode(self, audio: torch.Tensor, noise=None, lengths=None) -> torch.Tensor:
         """audio (B,1,T) -> latents (B,latent,T/hop): encoder + z = mean + (softplus(scale)+1e-4) * noise
-        (`noise=None` draws torch.randn from the global RNG like the reference's vae_sample; pass False for the mean)."""
+        (`noise=None` draws torch.randn from the global RNG like the reference's vae_sample; pass False for the mean).
+        `lengths` (latent frames per clip, a list or a cuda int32 tensor): audio is a padded batch, clip b being its first hop * lengths[b]
+        samples; frames < lengths[b] of the result equal the encode of that clip alone, bit for bit, and the frames past them are zeros.
+        With `noise=None` the bottleneck noise of clip b is drawn as (1, latent, lengths[b]) from the global RNG, in clip order -- the draws
+        consecutive solo calls make -- which needs the lengths on the host (a list)."""
         if self.encoder_cfg is None:
             raise _lib.EzbError("this handle was created without encoder_cfg")
         a = _as_f32c(audio).to(self.device)
@@ -97,15 +121,28 @@ class OobleckDecoder:
             T += pad
         L = T // self.hop
         Cz = self.cfg["latent_dim"]
-        if noise is None:
+        lens = host = None
+        if lengths is not None:
+            lens, host = self._lens(lengths, B, L)
+        if noise is None and lens is not None:
+            if host is None:
+                raise ValueError("encode(lengths=<tensor>) cannot size the per-clip noise draws: pass the lengths as a list, or the noise")
+            noise = torch.zeros(B, Cz, L, device=self.device, dtype=torch.float32)
+            for b, n in enumerate(host):
+                noise[b, :, :n] = torch.randn(1, Cz, n, device=self.device, dtype=torch.float32)[0]
+        elif noise is None:
             noise = torch.randn(B, Cz, L, device=self.device, dtype=torch.float32)
         nz = None if noise is False else _as_f32c(noise).to(self.device)
         z = torch.empty(B, Cz, L, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.dev_index):
             for b0 in range(0, B, self.max_batch):
                 nb = min(self.max_batch, B - b0)
-                _lib.check(_lib.lib().ezb_vae_encode(self.h, _lib.ptr(a[b0:b0 + nb]), None if nz is None else C.c_void_p(nz[b0:b0 + nb].data_ptr()),
-                                                     C.c_void_p(z[b0:b0 + nb].data_ptr()), nb, T, _lib.stream_ptr()))
+                args = (self.h, _lib.ptr(a[b0:b0 + nb]), None if nz is None else C.c_void_p(nz[b0:b0 + nb].data_ptr()),
+                        C.c_void_p(z[b0:b0 + nb].data_ptr()), nb, T)
+                if lens is None:
+                    _lib.check(_lib.lib().ezb_vae_encode(*args, _lib.stream_ptr()))
+                else:
+                    _lib.check(_lib.lib().ezb_vae_encode_lens(*args, _lib.ptr(lens[b0:b0 + nb]), _lib.stream_ptr()))
         return z
 
 
@@ -122,11 +159,12 @@ class Autoencoder:
     def to(self, *a, **k):
         return self
 
-    def __call__(self, audio=None, embedding=None):
+    def __call__(self, audio=None, embedding=None, lengths=None):
+        """`lengths`: latent frames per clip of a padded batch (OobleckDecoder.__call__ / .encode)."""
         if embedding is not None:
-            return self.decoder(embedding)
+            return self.decoder(embedding, lengths=lengths)
         if audio is not None:
-            return self.decoder.encode(audio)
+            return self.decoder.encode(audio, lengths=lengths)
         raise ValueError("Either audio or embedding must be provided.")
 
     forward = __call__

@@ -71,7 +71,8 @@ int ezb_dit_set_timesteps(ezb_dit* h, const int64_t* timesteps_host, int n, void
  * lens: NULL (every sample is L frames long) or a DEVICE int32 [Be]: sample b is a clip of lens[b] frames padded to L.  Its frames
  * < lens[b] come out as a forward of that clip alone at L = lens[b] computes them, whatever the padded frames hold (NaN included); its
  * frames >= lens[b] of `out` are not written.  Kernels read the lengths when they run (a captured graph replays with new lengths) and
- * clamp them to [1, L]; validating them is the caller's job.  Not combined with gt / gt_mask or ControlNet skips by the Python layer. */
+ * clamp them to [1, L]; validating them is the caller's job.  gt / gt_mask are padded like x (the Python layer marks the
+ * padded frames as regenerated); not combined with ControlNet skips by the Python layer. */
 int ezb_dit_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_host,
                     int t_index_all, const float* const* controlnet_skips, float* out, int Be, int L, void* stream,
                     const int32_t* lens);
@@ -143,6 +144,15 @@ int ezb_vae_decode(ezb_vae* h, const float* z /*(B,latent,L)*/, float* wav /*(B,
  * VAEBottleneck.encode (bottleneck.py:66-87): z = mean + (softplus(scale) + 1e-4) * noise.  audio (B,1,T) fp32, T a multiple of the
  * hop (480); noise (B,latent,L) fp32 drawn by the caller (the reference uses torch.randn_like), NULL -> z = mean. */
 int ezb_vae_encode(ezb_vae* h, const float* audio, const float* noise, float* z, int B, int T, void* stream);
+/* Decode / encode of a padded batch of clips of different lengths.  lens: DEVICE int32 [B], latent frames per clip, read when the kernels
+ * run (a captured graph replays with new lengths) and clamped to [1, L]; validating them is the caller's job.
+ * ezb_vae_decode_lens: samples < hop * lens[b] of clip b come out bit-identical to ezb_vae_decode of z[b, :, :lens[b]] alone, the samples
+ *   past them as zeros, whatever the padded frames of z hold (NaN included).
+ * ezb_vae_encode_lens: clip b is the first hop * lens[b] samples of audio[b] (T = hop * L); frames < lens[b] of z[b] come out bit-identical
+ *   to ezb_vae_encode of that clip alone with noise[b, :, :lens[b]], the frames past them as zeros, whatever audio and noise hold past
+ *   the clip's end. */
+int ezb_vae_decode_lens(ezb_vae* h, const float* z, float* wav, int B, int L, const int32_t* lens, void* stream);
+int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noise, float* z, int B, int T, const int32_t* lens, void* stream);
 
 /* EnergyExtractor.forward (src/models/conditions/energy.py:19-56) as wrapped by Conditioner (condition_wrapper.py:26-42): audio (B,T) fp32
  * -> (B, T/hop) fp32 frame energies in dB, normalised per clip when norm != 0; quantize_levels <= 1 disables quantisation. Only the shipped
