@@ -124,6 +124,7 @@ _SIGS = {
     "ezb_launch_count": ([], C.c_ulonglong),
     "ezb_launch_count_add": ([C.c_ulonglong], None),
     "ezb_ln_launch_count": ([_I], C.c_ulonglong),
+    "ezb_attn_launch_count": ([_I], C.c_ulonglong),
     "ezb_prof_gemm_begin": ([], _I),
     "ezb_prof_gemm_end": ([C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),
     "ezb_prof_gemm_stats": ([C.c_double, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double)], _I),

@@ -11,6 +11,7 @@
 //     + RES                 one CTA per (b, h): all key blocks of the head (Lk <= 512) are loaded once and stay resident while the CTA
 //                           walks every query tile of that head (K / V^T read from L2 once per head instead of once per query tile)
 //   generation 7            4 warps, 128-key blocks (half as many block barriers and rescales per key)
+//   generation 8 (default for dh 64 / 72)  TMA-fed, warp-specialised wgmma kernel of attention_wgmma.cuh; other head dims run generation 6
 // Layouts as produced by the QKV GEMM epilogue: Q, K [B*H, L, DHP] bf16; V^T [B*H, DVP, Lkpad] bf16.  Output [B, Lq, H*dh] bf16
 // token-major.
 // Padded batches (self-attention of clips of different lengths, p.lens): sample b holds len = lens[b] valid tokens.  Keys at or past len are
@@ -18,6 +19,7 @@
 // in the padded tokens (not even NaN) reaches them; query rows at or past len are written as zeros.  Those kernels are the VARLEN = true
 // instantiations; without lens the VARLEN = false ones run, compiled without any of this.
 #pragma once
+#include "attention_wgmma.cuh"
 #include "host.cuh"
 
 namespace ezb {
@@ -259,8 +261,9 @@ __global__ void __launch_bounds__(WARPS * 32) attn_mma_kernel(const AttnMmaParam
 // generation-6 CTA take one exp2 in four on the FMA pipe while the even warps stay on the MUFU (the two warp halves share the SM's MUFU);
 // bit 2 = generation 6 issues the P V MMAs after each half of a key block instead of after each 16-key slice.  opt_attn_pp: bit 1's
 // split for generation 4.
+constexpr int ATTN6_DEFAULT = 5;
 inline int& opt_attn6() {
-  static int v = [] { const char* e = getenv("EZB_ATTN6"); return e ? atoi(e) : 5; }();
+  static int v = [] { const char* e = getenv("EZB_ATTN6"); return e ? atoi(e) : ATTN6_DEFAULT; }();
   return v;
 }
 inline int& opt_attn7() {
@@ -283,7 +286,17 @@ inline int& opt_attn_pp() {
   static int v = [] { const char* e = getenv("EZB_ATTN_PP"); return e ? atoi(e) : 0; }();
   return v;
 }
-inline int attention_variant() { return opt_attn7() ? 7 : (opt_attn6() & 1) ? 6 : 4; }
+// generation 8 (attention_wgmma.cuh); it runs only while attn6 and attn7 are at their defaults, so that a non-default value of either still
+// selects its generation
+inline int& opt_attn8() {
+  static int v = [] { const char* e = getenv("EZB_ATTN8"); return e ? atoi(e) : 1; }();
+  return v;
+}
+inline int attention_variant() {
+  if (opt_attn7()) return 7;
+  if (opt_attn8() && opt_attn6() == ATTN6_DEFAULT) return 8;
+  return (opt_attn6() & 1) ? 6 : 4;
+}
 
 template <int DK, int WARPS, int KB, bool RES>
 int attn_mma_launch(cudaStream_t st, const AttnMmaParams& p, int B, int H) {
@@ -298,6 +311,7 @@ int attn_mma_launch(cudaStream_t st, const AttnMmaParams& p, int B, int H) {
   }
   const dim3 grid(RES ? 1 : (p.Lq + 16 * WARPS - 1) / (16 * WARPS), B * H);
   ++launch_counter();
+  ++attn_launch_counts()[KB == 128 ? 7 : WARPS == 8 ? 4 : 6];
   kern<<<grid, WARPS * 32, smem, st>>>(p);
   EZB_CUDA(cudaGetLastError());
   return EZB_OK;
@@ -312,12 +326,12 @@ int attn_mma_dispatch(cudaStream_t st, const AttnMmaParams& p, int B, int H, int
   return attn_mma_launch<DK, 4, 64, false>(st, p, B, H);
 }
 
-// variant: 4, 6 or 7 (see the file comment); 0 = the one the options select
+// variant: 4, 6, 7 or 8 (see the file comment); 0 = the one the options select (generation 8 falls back to 6 for a head dimension other
+// than 64 or 72)
 // lens: [B] valid tokens per sample (device) or null, see the file comment
 inline int attention_mma(Device& dev, cudaStream_t st, const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* vt, const uint8_t* key_mask,
                          __nv_bfloat16* out, int B, int H, int Lq, int Lk, int Lkpad, int dh, int dhp, int dvp, float scale, int variant = 0,
                          const int32_t* lens = nullptr) {
-  (void)dev;
   if (dh % 8 || dh > 80) return fail(EZB_ERR_UNSUPPORTED, "attention: head dimension %d (multiples of 8 up to 80)", dh);
   if (dhp < dh || dhp % 8 || dvp < dh || Lkpad < Lk || Lkpad % 8) return fail(EZB_ERR_SHAPE, "attention: pitches dhp %d dvp %d Lkpad %d", dhp, dvp, Lkpad);
   if (B < 1 || H < 1 || Lq < 1 || Lk < 1) return fail(EZB_ERR_SHAPE, "attention: empty problem");
@@ -325,7 +339,12 @@ inline int attention_mma(Device& dev, cudaStream_t st, const __nv_bfloat16* q, c
   p.q = q; p.k = k; p.vt = vt; p.key_mask = key_mask; p.lens = lens; p.out = out;
   p.H = H; p.Lq = Lq; p.Lk = Lk; p.Lkpad = Lkpad; p.dh = dh; p.dhp = dhp; p.dvp = dvp;
   p.scale_log2 = scale * 1.4426950408889634f;
+  const bool forced = variant != 0;
   if (variant == 0) variant = attention_variant();
+  if (variant == 8) {
+    if (dh == 64 || dh == 72 || forced) return attention_wgmma(dev, st, q, k, vt, key_mask, out, B, H, Lq, Lk, Lkpad, dh, dhp, dvp, scale, lens);
+    variant = 6;
+  }
   const bool split = (variant == 6 && (opt_attn6() & 2)) || (variant == 4 && opt_attn_pp());
   p.poly = opt_attn_poly() ? 1 : split ? 2 : 0;
   p.halves = variant == 6 && (opt_attn6() & 4);

@@ -110,6 +110,16 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;                       // layout type: SWIZZLE_128B
   return d;
 }
+// K-major operand tile with rows of 16 bf16 (32 B) and the 32-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_32B): 8-row groups are
+// 256 B apart (SBO), LBO unused.  A row is exactly one K step of 16 bf16.
+__device__ __forceinline__ uint64_t wgmma_desc_sw32(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address, 16 B units
+  d |= (uint64_t)1 << 16;                       // leading byte offset (ignored for swizzled K-major)
+  d |= (uint64_t)(256 >> 4) << 32;              // stride byte offset: 8 rows * 32 B
+  d |= (uint64_t)3 << 62;                       // layout type: SWIZZLE_32B
+  return d;
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -700,7 +700,7 @@ EZB_API int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noi
 }  // extern "C"
 
 namespace {
-// impl 0: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]); impl 1/4/6/7 (+100): tensor-core kernel (q,k bf16 [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad])
+// impl 0: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]); impl 1/4/6/7/8 (+100): tensor-core kernel (q,k bf16 [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad])
 int test_attention(int device, const void* q, const void* k, const void* v, const uint8_t* key_mask, const int32_t* lens, void* out, int B, int H,
                    int Lq, int Lk, int dh, int impl, void* stream) {
   if (!q || !k || !v || !out) return fail(EZB_ERR_ARG, "ezb_test_attention: null pointer");
@@ -718,12 +718,13 @@ int test_attention(int device, const void* q, const void* k, const void* v, cons
     EZB_CUDA(cudaGetLastError());
     return EZB_OK;
   }
-  // impl 1: the variant the options select; 4 / 6 / 7: that generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's
+  // impl 1: the variant the options select; 4 / 6 / 7 / 8: that generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's
   // layout) instead of a 64-multiple
   const int variant = impl % 100, row80 = impl >= 100;
-  if (variant != 1 && variant != 4 && variant != 6 && variant != 7) return fail(EZB_ERR_ARG, "ezb_test_attention: impl %d", impl);
+  if (variant != 1 && variant != 4 && variant != 6 && variant != 7 && variant != 8) return fail(EZB_ERR_ARG, "ezb_test_attention: impl %d", impl);
   const int dhp = (row80 && dh == 72) ? 80 : (dh + 63) / 64 * 64;
   const int dvp = (dh + 15) / 16 * 16, lkpad = (Lk + 7) / 8 * 8;
+  device_ctx(device).tmaps.trim();
   return attention_mma(device_ctx(device), ST(stream), reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
                        reinterpret_cast<const __nv_bfloat16*>(v), key_mask, reinterpret_cast<__nv_bfloat16*>(out), B, H, Lq, Lk, lkpad, dh, dhp, dvp, scale, variant == 1 ? 0 : variant,
                        lens);
@@ -757,6 +758,7 @@ EZB_API int ezb_set_option(const char* name, int value) {
   if (name && !strcmp(name, "ksub2")) { opt_ksub2() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn6")) { opt_attn6() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn7")) { opt_attn7() = value; return EZB_OK; }
+  if (name && !strcmp(name, "attn8")) { opt_attn8() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn_res")) { opt_attn_res() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn_pp")) { opt_attn_pp() = value; return EZB_OK; }
   if (name && !strcmp(name, "gemm_debug")) {  // cycle counters of CTA 0 of every 2-CTA cluster GEMM launch (accumulated; needs -DEZB_GEMM_DEBUG)
@@ -788,6 +790,7 @@ EZB_API int ezb_debug_read(unsigned long long* out8) {
 EZB_API unsigned long long ezb_launch_count(void) { return launch_counter(); }
 // kernels replayed through a captured CUDA graph never pass the launch helpers: the host layer reports them here
 EZB_API void ezb_launch_count_add(unsigned long long n) { launch_counter() += n; }
+EZB_API unsigned long long ezb_attn_launch_count(int generation) { return generation >= 0 && generation <= 8 ? attn_launch_counts()[generation] : 0; }
 EZB_API unsigned long long ezb_ln_launch_count(int variant) { return variant >= LN_GENERIC && variant <= LN_CAT ? ln_launch_counts()[variant] : 0; }
 EZB_API int ezb_prof_gemm_begin(void) {
   GemmProf& gp = gemm_prof();

@@ -84,9 +84,10 @@ inline PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// bf16 (or `dtype`) tensor, innermost dim first; 128-byte swizzle, zero fill out of bounds.
+// bf16 (or `dtype`) tensor, innermost dim first; 128-byte swizzle unless `swizzle` says otherwise, zero fill out of bounds.
 inline int make_tmap(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes /*rank-1*/,
-                     const uint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
+                     const uint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return fail(EZB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
   cuuint64_t gd[5], gs[5];
@@ -101,7 +102,7 @@ inline int make_tmap(CUtensorMap* out, const void* ptr, int rank, const uint64_t
   for (int i = 0; i + 1 < rank; ++i)
     if (gs[i] % 16) return fail(EZB_ERR_ARG, "TMA stride %llu not a multiple of 16 B", (unsigned long long)gs[i]);
   CUresult r = enc(out, dtype, rank, const_cast<void*>(ptr), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(EZB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d): rank %d dims %llu,%llu box %u,%u", (int)r, rank,
                                      (unsigned long long)gd[0], (unsigned long long)gd[1], bx[0], bx[1]);
@@ -155,6 +156,22 @@ struct TmapCache {
       uint64_t dims[3] = {inner, rows, batch}, str[2] = {ld_row * 2, ld_batch * 2};
       uint32_t box[3] = {64, box_rows, 1};
       EZB_TRY(make_tmap(&m, ptr, 3, dims, str, box));
+      it = maps.emplace(k, m).first;
+    }
+    *out = &it->second;
+    return EZB_OK;
+  }
+  // 3-D [batch, rows, inner] bf16, box {box_inner, box_rows, 1} with a 128- or 32-byte swizzle (box_inner 64 or 16)
+  int get3d_box(const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld_row, uint64_t ld_batch, uint32_t box_inner,
+                uint32_t box_rows, const CUtensorMap** out) {
+    Key k(ptr, inner, rows, batch, ld_row * 1000003ull + ld_batch, box_inner << 16 | box_rows, 4);
+    auto it = maps.find(k);
+    if (it == maps.end()) {
+      CUtensorMap m;
+      uint64_t dims[3] = {inner, rows, batch}, str[2] = {ld_row * 2, ld_batch * 2};
+      uint32_t box[3] = {box_inner, box_rows, 1};
+      EZB_TRY(make_tmap(&m, ptr, 3, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                        box_inner == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B));
       it = maps.emplace(k, m).first;
     }
     *out = &it->second;

@@ -321,8 +321,8 @@ typedef struct {
   void* out; float* f32_out[3]; void* bf_out[3];
 } ezb_test_step_args;
 int ezb_test_step(int device, const ezb_test_step_args* args, void* stream);
-/* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7: that
-   generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
+/* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7 / 8: that
+   generation forced (8 takes dh 64 or 72 only); +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
                        int B, int H, int Lq, int Lk, int dh, int impl, void* stream);
 /* Self-attention (Lq = Lk = L, no key mask) of a padded batch, as ezb_test_attention with the same impl codes: lens DEVICE int32 [B],
@@ -331,7 +331,7 @@ int ezb_test_attention_lens(int device, const void* q, const void* k, const void
                             int L, int dh, int impl, void* stream);
 
 /* runtime switches for A/B measurements and profiling (csrc/host.cuh, csrc/ezb.cu list them): e.g. "pair_gemm" (1 = 2-CTA cluster tiles
-   sharing the weight tile, default), "attn6" / "attn7" / "attn_res" (attention variant), "ksub2", "ln_variant", "skip" (profiling: kernel classes not launched).  Products never need to call this. */
+   sharing the weight tile, default), "attn6" / "attn7" / "attn8" / "attn_res" (attention variant), "ksub2", "ln_variant", "skip" (profiling: kernel classes not launched).  Products never need to call this. */
 int ezb_set_option(const char* name, int value);
 /* incremented by every ezb_set_option call: hosts that cache captured CUDA graphs key them on it (options change kernel selection) */
 unsigned long long ezb_option_epoch(void);
@@ -344,6 +344,8 @@ void ezb_launch_count_add(unsigned long long n); /* launches replayed from a cap
 /* stand-alone LayerNorm launches of one kernel (the variant numbers of ezb_test_step: 1 generic, 2 / 3 register-resident, 4 precombined
    affine, 5 register-resident concat) so far, process-wide; a captured CUDA graph counts once, at capture */
 unsigned long long ezb_ln_launch_count(int variant);
+/* tensor-core attention launches of one generation (4, 6, 7 or 8) so far, process-wide; a captured CUDA graph counts once, at capture */
+unsigned long long ezb_attn_launch_count(int generation);
 int ezb_prof_gemm_begin(void);
 int ezb_prof_gemm_end(int* launches, double* flops, double* ms);
 int ezb_prof_gemm_stats(double min_flops, int* launches, double* flops, double* ms); /* subset of the last profile */
