@@ -417,6 +417,7 @@ class EzAudio_ControlNet(_Base):
         self.params = params if params is not None else config.load_params(model_name, config_path, config.BUILTIN_CONTROLNET)
         p = self.params
         max_len = 10 * p["autoencoder"]["latent_sr"]  # the reference ControlNet API is hard-wired to 10 s (api/controlnet.py:131-138)
+        self.max_length_s = 10.0
         self.noise_scheduler = DDIMScheduler(**p["diff"])
         kw = dict(precision=precision, max_batch=2 * max_batch, max_len=max_len, max_ctx_len=p["text_encoder"]["max_length"], max_timesteps=1000,
                   device=device)
@@ -438,7 +439,13 @@ class EzAudio_ControlNet(_Base):
 
     def generate_audio(self, text, audio_path, surpass_noise=0, guidance_scale=3.5, guidance_rescale=0, ddim_steps=50, eta=1,
                        conditioning_scale=1, random_seed=None, randomize_seed=False):
-        """api/controlnet.py:113-161.  `audio_path` may also be a float32 numpy waveform at the model sample rate."""
+        """api/controlnet.py:113-161.  `audio_path` may also be a float32 numpy waveform at the model sample rate.
+        With a list of prompts, `audio_path` may list one reference clip per prompt (and `surpass_noise` one gate per prompt, or one for
+        all): each clip is prepared on its own, the batch runs once and waveform b is trimmed to clip b's length.  Pass one seed per prompt
+        in `random_seed` to make the batch reproduce the scalar calls."""
+        if isinstance(audio_path, (list, tuple)):
+            return self._generate_per_clip(text, list(audio_path), surpass_noise, guidance_scale, guidance_rescale, ddim_steps, eta,
+                                           conditioning_scale, random_seed, randomize_seed)
         sr = self.params["autoencoder"]["sr"]
         gt = _load_audio(audio_path, sr) if isinstance(audio_path, str) else np.asarray(audio_path, dtype=np.float32)
         original_length = len(gt)
@@ -462,3 +469,35 @@ class EzAudio_ControlNet(_Base):
         if batched:
             return sr, [pred[i, 0][:original_length] for i in range(pred.shape[0])]
         return sr, pred.squeeze(0).squeeze(0)[:original_length]
+
+    def _generate_per_clip(self, text, audio_paths, surpass_noise, guidance_scale, guidance_rescale, ddim_steps, eta, conditioning_scale,
+                           random_seed, randomize_seed):
+        sr = self.params["autoencoder"]["sr"]
+        # ---- everything is checked on the host before any device work
+        if isinstance(text, str):
+            raise ValueError("a list of reference clips takes a list of prompts (one clip per prompt)")
+        prompts = list(text)
+        B = len(prompts)
+        if len(audio_paths) != B:
+            raise ValueError(f"audio_path lists one clip per prompt: got {len(audio_paths)} for {B} prompts")
+        num = (int, float, np.integer, np.floating)
+        gates = [float(g or 0) for g in _per_clip("surpass_noise", surpass_noise, B, num)]
+        if isinstance(random_seed, (list, tuple)) and len(random_seed) != B:
+            raise ValueError(f"random_seed lists one seed per prompt: got {len(random_seed)} for {B} prompts")
+        raws = [_load_audio(a, sr) if isinstance(a, str) else np.asarray(a, dtype=np.float32) for a in audio_paths]
+        if any(r.ndim != 1 or len(r) < 1 for r in raws):
+            raise ValueError("every reference clip must be a non-empty mono waveform")
+        num_samples = int(10 * sr)
+        audio_frames = round(num_samples / sr * self.params["autoencoder"]["latent_sr"])
+        cond_kw = {k: v for k, v in self.params["conditioner"].items() if k != "condition_type"}
+        # ---- per clip: normalise, noise-gate, pad / crop to 10 s and the energy condition, as the scalar call does; stacked (B, 1, 2L)
+        condition = torch.cat([energy_condition(post.prepare_wave(torch.from_numpy(r).to(self.device).unsqueeze(0), num_samples, normalize=True,
+                                                                  gate=g), **cond_kw) for r, g in zip(raws, gates)], 0)
+        if randomize_seed:
+            random_seed = random.randint(0, MAX_SEED)
+        embeds = self._text_embeds(prompts, [""])
+        pred = inference(self.autoencoder, self.unet, None, None, None, None, self.params, self.noise_scheduler, prompts, None, audio_frames,
+                         guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, self.device, text_embeds=embeds,
+                         controlnet=self.controlnet, condition=condition, conditioning_scale=conditioning_scale)
+        pred = pred.cpu().numpy()
+        return sr, [pred[b, 0][:len(r)] for b, r in enumerate(raws)]

@@ -161,6 +161,10 @@ struct Dit {
   float *t_vals = nullptr, *t_emb = nullptr, *t_h = nullptr, *t_tok = nullptr, *t_ada = nullptr, *t_lora = nullptr, *mod = nullptr, *mod_final = nullptr,
         *mod_b = nullptr, *modf_b = nullptr;
   int n_timesteps = 0, ctx_Be = 0, ctx_Lc = 0, ctx_Lpad = 0;
+  // ControlNet condition cache (ezb_controlnet_set_condition): the stem's output [cond_Be, cond_L, D], apart from the cond_emb scratch that
+  // ezb_controlnet_forward writes on every call
+  float* cond_cache = nullptr;
+  int cond_Be = 0, cond_L = 0;
   float2* rope_cs = nullptr;
   float h_inv_freq[48] = {};
   bool fused_heads = false;
@@ -464,6 +468,7 @@ struct Dit {
       EZB_TRY(alloc(&ybuf, Mx * C));
     } else {
       EZB_TRY(alloc(&cond_emb, Mx * D));
+      EZB_TRY(alloc(&cond_cache, Mx * D));
       EZB_TRY(alloc(&cs_t0, (size_t)d.max_batch * (d.cond_c0 + 1) * 2 * d.max_len));
       EZB_TRY(alloc(&cs_t1, (size_t)d.max_batch * (d.cond_c0 + 1) * 2 * d.max_len));
       EZB_TRY(alloc(&cs_t2, (size_t)d.max_batch * d.cond_c1 * d.max_len));
@@ -1090,6 +1095,12 @@ struct Dit {
 
   int controlnet_forward(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const float* cond, float cscale,
                          float* const* skips_out, int Be, int L, cudaStream_t st);
+  int controlnet_forward_tdev(const float* x, const int32_t* tdev, const float* scale_dev, float* const* skips_out, int Be, int L, cudaStream_t st);
+  int set_condition(const float* cond, int Be, int L, cudaStream_t st);
+  int set_condition_rows(const float* cond, int row0, int n, int L, cudaStream_t st);
+  int controlnet_stem(const float* cond, float* out, int Be, int L, cudaStream_t st);
+  int controlnet_trunk(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const int32_t* tdev, const float* cond,
+                       float cscale, const float* scale_dev, float* const* skips_out, int Be, int L, cudaStream_t st);
 };
 
 }  // namespace ezb
@@ -1101,25 +1112,72 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
                                    float* const* skips_out, int Be, int L, cudaStream_t st) {
   if (!d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_controlnet_forward called on a DiT handle");
   EZB_TRY(check_call(Be, L));
-  lens = nullptr;   // the stem convs cross clip ends: ControlNet batches are uniform in length
-  dev->tmaps.trim();
-  WeightSeqScope ws(dev, this, 2, ((long long)Be << 32) | (unsigned)L);
-  const float *modr, *modf;
-  int mbs, mbsf;
-  EZB_TRY(select_mod(st, tidx, tall, nullptr, Be, &modr, &modf, &mbs, &mbsf));
+  return controlnet_trunk(x, gt, gt_mask, tidx, tall, nullptr, cond, cscale, nullptr, skips_out, Be, L, st);
+}
+
+// The stem (controlnet_pre, controlnet.py:65-84) of Be conditions (Be,1,2L) into out (Be,L,D).  It depends on the condition only, and every
+// kernel computes each output element on its own, so a clip's rows do not depend on the batch.
+inline int Dit::controlnet_stem(const float* cond, float* out, int Be, int L, cudaStream_t st) {
   const int c0 = d.cond_c0, c1 = d.cond_c1, T = 2 * L;
-  auto conv = [&](const float* in, const float* w, const float* b, float* out, int Cin, int cin_real, int Tin, int Cout, int Tout, int K, int stride, int pad,
+  auto conv = [&](const float* in, const float* w, const float* b, float* o, int Cin, int cin_real, int Tin, int Cout, int Tout, int K, int stride, int pad,
                   int act, int tr) -> int {
     const size_t n = (size_t)Be * Cout * Tout;
     ++launch_counter();
-    conv1d_direct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, w, b, out, Be, Cin, cin_real, Tin, Cout, Tout, K, stride, pad, act, tr);
+    conv1d_direct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, w, b, o, Be, Cin, cin_real, Tin, Cout, Tout, K, stride, pad, act, tr);
     EZB_CUDA(cudaGetLastError());
     return EZB_OK;
   };
   EZB_TRY(conv(cond, cs_in_w, cs_in_b, cs_t0, 1, 1, T, c0, T, 1, 1, 0, 0, 0));              // conv_in
   EZB_TRY(conv(cs_t0, cs_c0_w, cs_c0_b, cs_t1, c0 + 1, c0, T, c0 + 1, T, 3, 1, 1, 1, 0));    // conv3 + SiLU (mask channel == 0)
   EZB_TRY(conv(cs_t1, cs_c1_w, cs_c1_b, cs_t2, c0 + 1, c0 + 1, T, c1, L, 3, 2, 1, 1, 0));    // conv3 stride 2 + SiLU
-  EZB_TRY(conv(cs_t2, cs_out_w, cs_out_b, cond_emb, c1, c1, L, D, L, 1, 1, 0, 0, 1));        // conv_out -> (B,L,D)
+  EZB_TRY(conv(cs_t2, cs_out_w, cs_out_b, out, c1, c1, L, D, L, 1, 1, 0, 0, 1));             // conv_out -> (B,L,D)
+  return EZB_OK;
+}
+
+inline int Dit::set_condition(const float* cond, int Be, int L, cudaStream_t st) {
+  if (!d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_controlnet_set_condition called on a DiT handle");
+  if (!finalized) return fail(EZB_ERR_STATE, "weights not finalized");
+  if (Be < 1 || Be > d.max_batch || L < 1 || L > d.max_len) return fail(EZB_ERR_SHAPE, "set_condition: Be %d / L %d exceed workspace (%d, %d)", Be, L, d.max_batch, d.max_len);
+  cond_Be = Be; cond_L = L;
+  return controlnet_stem(cond, cond_cache, Be, L, st);
+}
+
+// rows [row0, row0 + n) of the layout the last set_condition established (ezb_controlnet_set_condition_rows)
+inline int Dit::set_condition_rows(const float* cond, int row0, int n, int L, cudaStream_t st) {
+  if (!d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_controlnet_set_condition_rows called on a DiT handle");
+  if (!finalized) return fail(EZB_ERR_STATE, "weights not finalized");
+  if (cond_Be < 1) return fail(EZB_ERR_STATE, "set_condition_rows: no ezb_controlnet_set_condition call established the condition layout");
+  if (L != cond_L) return fail(EZB_ERR_STATE, "set_condition_rows: L %d differs from the condition layout (L %d)", L, cond_L);
+  if (row0 < 0 || n < 1 || row0 + n > cond_Be) return fail(EZB_ERR_SHAPE, "set_condition_rows: rows [%d, %d) outside the batch of %d", row0, row0 + n, cond_Be);
+  return controlnet_stem(cond, cond_cache + (size_t)row0 * L * D, n, L, st);
+}
+
+// The trunk with device timestep indices, the cached condition and per-sample scales.  Device indices always gather per-sample modulation
+// rows (no fold mode), as non-uniform host indices do, and the zero-linears run EpiLinearScaled on the tiles EpiLinear<128> takes with a
+// non-zero uniform scale: each sample comes out as ezb_controlnet_forward with its scale and such host indices computes it.
+inline int Dit::controlnet_forward_tdev(const float* x, const int32_t* tdev, const float* scale_dev, float* const* skips_out, int Be, int L, cudaStream_t st) {
+  if (!d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_controlnet_forward_tdev called on a DiT handle");
+  EZB_TRY(check_call(Be, L));
+  if (Be != cond_Be || L != cond_L)
+    return fail(EZB_ERR_STATE, "controlnet_forward_tdev: Be %d / L %d differ from the condition set by ezb_controlnet_set_condition (%d, %d)", Be, L, cond_Be, cond_L);
+  return controlnet_trunk(x, nullptr, nullptr, nullptr, 0, tdev, nullptr, 0.f, scale_dev, skips_out, Be, L, st);
+}
+
+// cond: the raw condition, run through the stem into cond_emb here, or null for the condition cache.  scale_dev (device [Be]) or, when null,
+// the uniform cscale (0 treated as 1).
+inline int Dit::controlnet_trunk(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const int32_t* tdev,
+                                 const float* cond, float cscale, const float* scale_dev, float* const* skips_out, int Be, int L, cudaStream_t st) {
+  lens = nullptr;   // the stem convs cross clip ends: ControlNet batches are uniform in length
+  dev->tmaps.trim();
+  WeightSeqScope ws(dev, this, 2, ((long long)Be << 32) | (unsigned)L);
+  const float *modr, *modf;
+  int mbs, mbsf;
+  EZB_TRY(select_mod(st, tidx, tall, tdev, Be, &modr, &modf, &mbs, &mbsf));
+  const float* cemb = cond_cache;
+  if (cond != nullptr) {
+    EZB_TRY(controlnet_stem(cond, cond_emb, Be, L, st));
+    cemb = cond_emb;
+  }
   FoldCtx fc = fold_ctx(mbs, modr, L);
   const int M = Be * L;
   auto entry_ln = [&](int i, const float* xin) -> LnParams {
@@ -1128,7 +1186,7 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
   };
   bool done = false;
   LnParams nl = entry_ln(0, x0);
-  EZB_TRY(embed(st, x, gt, gt_mask, cond_emb, Be, L, fc, fp8 ? nullptr : &nl, &done));       // x = patch_embed(x) + condition
+  EZB_TRY(embed(st, x, gt, gt_mask, cemb, Be, L, fc, fp8 ? nullptr : &nl, &done));           // x = patch_embed(x) + condition
   const float* xc = x0;
   fc.st_x = st_x0;
   for (int i = 0; i < half; ++i) {
@@ -1145,7 +1203,13 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
     else EZB_TRY(ln(st, skips[i], D, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, 0, L, act, M));
     EpiLinearParams e = epi();
     e.bias = blk[i].zero_b; e.out_scale = cscale; e.out_f32 = skips_out[i]; e.ld32 = D;
-    EZB_TRY(lin(st, A, D, blk[i].zero_w, M, D, e));
+    if (scale_dev == nullptr) {
+      EZB_TRY(lin(st, A, D, blk[i].zero_w, M, D, e));
+    } else if (!(opt_skip() & 8)) {
+      const EpiLinearScaledParams es{e, scale_dev, L};
+      if (pair) EZB_TRY((gemm2<128, EpiLinearScaled<128>>(*dev, st, A, kmul * D, blk[i].zero_w, kmul * D, M, D, kmul * D, es)));
+      else EZB_TRY((gemm<128, EpiLinearScaled<128>>(*dev, st, A, kmul * D, blk[i].zero_w, kmul * D, M, D, kmul * D, es)));
+    }
   }
   ws.ok = true;
   return EZB_OK;

@@ -586,6 +586,19 @@ EZB_API int ezb_dit_forward_tdev(ezb_dit* h, const float* x, const float* gt, co
   if (!h || !x || !out || !t_index_dev) return fail(EZB_ERR_ARG, "ezb_dit_forward_tdev: null argument");
   return reinterpret_cast<Dit*>(h)->forward(x, gt, gt_mask, nullptr, 0, cskips, out, Be, L, lens, ST(stream), t_index_dev);
 }
+EZB_API int ezb_controlnet_set_condition(ezb_dit* h, const float* condition, int Be, int L, void* stream) {
+  if (!h || !condition) return fail(EZB_ERR_ARG, "ezb_controlnet_set_condition: null argument");
+  return reinterpret_cast<Dit*>(h)->set_condition(condition, Be, L, ST(stream));
+}
+EZB_API int ezb_controlnet_set_condition_rows(ezb_dit* h, const float* condition, int row0, int n, int L, void* stream) {
+  if (!h || !condition) return fail(EZB_ERR_ARG, "ezb_controlnet_set_condition_rows: null argument");
+  return reinterpret_cast<Dit*>(h)->set_condition_rows(condition, row0, n, L, ST(stream));
+}
+EZB_API int ezb_controlnet_forward_tdev(ezb_dit* h, const float* x, const int32_t* t_index_dev, const float* scale_dev, float* const* skips_out, int Be,
+                                        int L, void* stream) {
+  if (!h || !x || !t_index_dev || !scale_dev || !skips_out) return fail(EZB_ERR_ARG, "ezb_controlnet_forward_tdev: null argument");
+  return reinterpret_cast<Dit*>(h)->controlnet_forward_tdev(x, t_index_dev, scale_dev, skips_out, Be, L, ST(stream));
+}
 EZB_API int ezb_cfg_ddim_step_slots(int device, const float* model_out, float* latents, const float* noise, const ezb_ddim_slot* slots, int B, int C,
                                     int L, void* stream, const int32_t* lens) {
   if (!model_out || !latents || !slots || B < 1 || C < 1 || L < 1) return fail(EZB_ERR_ARG, "ezb_cfg_ddim_step_slots: bad argument");

@@ -361,6 +361,52 @@ struct EpiLinearLens {
   }
 };
 
+// bias -> f32 with a per-sample scale read when the kernel runs: out[row, col] = (acc + bias[col]) * scale[row / rows_per_batch], the float
+// operations rows_generic applies with a uniform out_scale, so a sample whose scale equals it comes out with the same bits.  A scale of 0 gives
+// zeros (the uniform out_scale treats 0 as 1).  The ControlNet zero-linears of a batch of requests with different conditioning scales.
+struct EpiLinearScaledParams {
+  EpiLinearParams lin;     // bias, out_f32, ld32 (nothing else is read)
+  const float* scale;      // [B] device
+  int rows_per_batch;
+};
+template <int BN>
+struct EpiLinearScaled {
+  using Params = EpiLinearScaledParams;
+  static constexpr int EPI_WARPS = EpiLinear<BN>::EPI_WARPS;
+  static constexpr bool WIDE_REGS = false;
+  static constexpr int STAGE_FLOATS = EPI_STAGE_FLOATS;
+  template <class Wait>
+  static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
+                                             int c_end, Wait wait) {
+    const EpiLinearParams& e = ep.lin;
+    const int nv = nvalid < 32 ? nvalid : 32;
+    wait();
+#pragma unroll 1
+    for (int c = c_begin; c < c_end; c += 64) {
+      const int col = n0 + c + 2 * lane;
+      const bool col_ok = (c + 2 * lane < c_end) && col < N;
+      __syncwarp();
+#pragma unroll
+      for (int hc = 0; hc < 2; ++hc) {
+        uint32_t r[32];
+        acc_ld<32>(ar, c + 32 * hc, lane, r);
+#pragma unroll
+        for (int g = 0; g < 16; ++g) stage_put(st, lane, 16 * hc + g, __uint_as_float(r[2 * g]), __uint_as_float(r[2 * g + 1]));
+      }
+      __syncwarp();
+      if (!col_ok) continue;
+      const float b0 = e.bias != nullptr ? e.bias[col] : 0.f, b1 = e.bias != nullptr ? e.bias[col + 1] : 0.f;
+#pragma unroll 4
+      for (int rr = 0; rr < nv; ++rr) {
+        const int row = row0 + rr;
+        const float s = ep.scale[row / ep.rows_per_batch];
+        const float2 acc = stage_get(st, rr, lane);
+        *reinterpret_cast<float2*>(e.out_f32 + (size_t)row * e.ld32 + col) = make_float2((acc.x + b0) * s, (acc.y + b1) * s);
+      }
+    }
+  }
+};
+
 // GEGLU (src/models/utils/modules.py:274-277): W rows are packed so that an N-tile of BN columns holds BN/2 hidden
 // features followed by the BN/2 matching gate features; out[row, n0/2 + j] = (h_j + bh_j) * gelu_erf(g_j + bg_j).
 struct EpiGegluParams {

@@ -291,6 +291,7 @@ class DiTControlNet:
         self._h = _Handle(cfg, self.cn, precision, max_batch, max_len, max_ctx_len, max_timesteps, device)
         self.device = self._h.device
         self.half = cfg["depth"] // 2
+        self.cond_epoch = 0
 
     def eval(self):
         return self
@@ -308,6 +309,35 @@ class DiTControlNet:
     def set_timesteps(self, ts):
         self._h.set_timesteps(ts)
 
+    def set_context_rows(self, context, context_mask, row0: int):
+        """As MaskDiT.set_context_rows."""
+        self._h.set_context_rows(context, context_mask, row0)
+
+    def _cond(self, condition, n: int, L: int) -> torch.Tensor:
+        cond = _as_f32c(condition).to(self.device)
+        if tuple(cond.shape) != (n, 1, 2 * L):
+            raise ValueError(f"condition must be (n,1,2L)={(n, 1, 2 * L)}, got {tuple(cond.shape)}")
+        return cond
+
+    def set_condition(self, condition):
+        """Runs the stem of condition (Be,1,2L) once into the handle's condition cache, which `forward_step(t_index=, scale=)` reads; this fixes
+        the cache layout (Be, L).  ezb_controlnet_forward (the other call paths) neither reads nor writes the cache."""
+        Be, L = int(condition.shape[0]), int(condition.shape[-1]) // 2
+        cond = self._cond(condition, Be, L)
+        with torch.cuda.device(self._h.dev_index):
+            _lib.check(_lib.lib().ezb_controlnet_set_condition(self._h.h, _lib.ptr(cond), Be, L, _lib.stream_ptr()))
+        self._keep_cond = cond
+        self.cond_epoch += 1   # lets a holder of condition rows (engine.ContinuousEngine) see that the layout was replaced
+
+    def set_condition_rows(self, condition, row0: int):
+        """Replaces the cached condition of samples [row0, row0 + n) (condition (n,1,2L), L that of the last set_condition) without
+        recomputing the other rows; they come out as set_condition of the whole updated batch computes them."""
+        n, L = int(condition.shape[0]), int(condition.shape[-1]) // 2
+        cond = self._cond(condition, n, L)
+        with torch.cuda.device(self._h.dev_index):
+            _lib.check(_lib.lib().ezb_controlnet_set_condition_rows(self._h.h, _lib.ptr(cond), int(row0), n, L, _lib.stream_ptr()))
+        self._keep_cond_rows = cond
+
     def _run(self, x, gt, m8, tidx_arr, tall, condition, scale, outs):
         Be, Cc, L = x.shape
         D = self.cfg["embed_dim"]
@@ -322,8 +352,29 @@ class DiTControlNet:
                                                          float(scale), arr, Be, L, _lib.stream_ptr()))
         return outs
 
-    def forward_step(self, x, step_index, condition, conditioning_scale=1.0, gt=None, gt_mask_u8=None, outs=None):
-        return self._run(x, gt, gt_mask_u8, None, int(step_index), condition, conditioning_scale, outs)
+    def forward_step(self, x, step_index=0, condition=None, conditioning_scale=1.0, gt=None, gt_mask_u8=None, outs=None, t_index=None, scale=None):
+        """One ControlNet forward at table row `step_index` on `condition` (Be,1,2L) with one `conditioning_scale`; returns depth/2 skips
+        (Be,L,D) fp32 (written into `outs` when given).
+        With `t_index` and `scale` -- contiguous cuda int32 / fp32 tensors of shape (Be,), read on the device when the kernels run, like
+        MaskDiT.forward_step's t_index -- sample b runs at table row t_index[b] on the cached condition of set_condition with its skips times
+        scale[b] (0 gives zeros); `condition`, `gt` and `gt_mask_u8` are then not accepted."""
+        if t_index is None and scale is None:
+            return self._run(x, gt, gt_mask_u8, None, int(step_index), condition, conditioning_scale, outs)
+        Be, Cc, L = x.shape
+        if t_index is None or scale is None:
+            raise ValueError("t_index and scale go together")
+        if condition is not None or gt is not None or gt_mask_u8 is not None:
+            raise ValueError("forward_step(t_index=, scale=) reads the condition cache of set_condition and takes no gt")
+        for name, v, dt in (("t_index", t_index, torch.int32), ("scale", scale, torch.float32)):
+            if v.dtype != dt or not v.is_cuda or tuple(v.shape) != (Be,) or not v.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous cuda {dt} tensor of shape ({Be},)")
+        if outs is None:
+            outs = [torch.empty(Be, L, self.cfg["embed_dim"], device=self.device, dtype=torch.float32) for _ in range(self.half)]
+        arr = (C.c_void_p * self.half)(*[o.data_ptr() for o in outs])
+        with torch.cuda.device(self._h.dev_index):
+            _lib.check(_lib.lib().ezb_controlnet_forward_tdev(self._h.h, _lib.ptr(x), _lib.ptr(t_index), _lib.ptr(scale), arr, Be, L,
+                                                              _lib.stream_ptr()))
+        return outs
 
     def __call__(self, x, timesteps, context, x_mask=None, context_mask=None, cls_token=None, condition=None, cond_mask_infer=None,
                  conditioning_scale=1.0):

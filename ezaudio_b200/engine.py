@@ -1,4 +1,4 @@
-"""Continuous batching for text-to-audio: requests join a running batch at step boundaries.
+"""Continuous batching for text-to-audio and ControlNet: requests join a running batch at step boundaries.
 
 `ContinuousEngine` keeps `slots` requests in flight in one padded, CFG-doubled batch (effective batch 2 * slots, clips padded to
 `max_length_s`).  Each denoising step is one replay of one captured CUDA graph: the CFG-doubling copy, the DiT forward with per-sample
@@ -10,23 +10,30 @@ encodes the prompt, replaces that slot's text context row (`MaskDiT.set_context_
 Every request keeps its own step count (one of `ddim_steps`), guidance scale, rescale, eta, length and seed: the denoiser's timestep table
 holds the sorted union of the allowed schedules (with trailing spacing the 25- and 50-step schedules are subsets of the 100-step one).  A
 request's audio does not depend on what it shares the batch with.  Requests have the semantics of `EzAudio.generate_audio` for one prompt
-(`frontend.Request`); the empty prompt "" runs without guidance, as it does there.  Inpainting, ControlNet and the FP8 mode are not served.
+(`frontend.Request`); the empty prompt "" runs without guidance, as it does there.
 
-The host logic (admission, schedules, DDIM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots`, which tests replace
-with a stub."""
+Given an `api.EzAudio_ControlNet`, the engine serves `frontend.ControlRequest`s, with the semantics of `EzAudio_ControlNet.generate_audio`
+for one prompt and one reference clip: 10-s clips, each with its own reference audio, noise gate and conditioning scale besides the
+per-request constants above.  Admission also runs the clip's energy condition through the ControlNet stem once, into that slot's rows of
+the ControlNet's condition cache (`DiTControlNet.set_condition_rows`); each step runs the ControlNet with per-sample timestep rows and
+scales (`DiTControlNet.forward_step(t_index=, scale=)`) before the DiT.  Inpainting and the FP8 mode are not served.
+
+The host logic (admission, schedules, DDIM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots` (`ControlSlots`),
+which tests replace with a stub."""
 from __future__ import annotations
 
 import collections
 import dataclasses
 import math
 import numbers
+import os
 from typing import Iterable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
-from . import _lib
-from .frontend import Request
+from . import _lib, post
+from .frontend import ControlRequest, Request
 from .inference import scale_shift_re
 from .scheduler import DDIMScheduler
 
@@ -43,12 +50,13 @@ class SlotStep:
     coef: List[float]         # DDIMScheduler.step_coefficients
     cfg: bool
     draw_noise: bool          # eta > 0: the slot's generator draws this step's (1, C, frames) noise
+    conditioning_scale: float = 1.0   # ControlNet requests: the factor of the ControlNet skips
 
 
 @dataclasses.dataclass
 class _Active:
     ticket: int
-    req: Request
+    req: object               # Request or ControlRequest
     frames: int
     timesteps: List[int]
     sched: DDIMScheduler
@@ -56,13 +64,15 @@ class _Active:
 
 
 class ContinuousEngine:
-    """Continuous-batching server for `ez` (an `api.EzAudio`): `submit` requests, then `step` / `stream` / `run` them (see the module docstring).
+    """Continuous-batching server for `ez` (an `api.EzAudio`, or an `api.EzAudio_ControlNet`): `submit` requests, then `step` / `stream` /
+    `run` them (see the module docstring).
 
     slots: requests in flight (the denoiser runs 2 * slots samples; ez must have been built with max_batch >= slots).
-    max_length_s: the padded clip length (at most ez.max_length_s); longer requests are rejected.
+    max_length_s: the padded clip length (at most ez.max_length_s); longer requests are rejected.  ControlNet clips are 10 s.
     ddim_steps: the step counts requests may ask for; the union of their schedules must fit the timestep table."""
 
     def __init__(self, ez, slots: int = 4, max_length_s: float = 10.0, ddim_steps: Sequence[int] = (25, 50, 100), *, backend=None):
+        self.control = bool(getattr(backend, "control", False)) if backend is not None else hasattr(ez, "controlnet")
         self.slots = int(slots)
         if self.slots < 1:
             raise ValueError("slots must be >= 1")
@@ -86,20 +96,26 @@ class ContinuousEngine:
         self.ddim_steps = tuple(allowed)
         self.table = table
         self._row = {t: i for i, t in enumerate(table)}
-        self.backend = backend if backend is not None else CudaSlots(ez, self.slots, max_length_s, table)
+        if backend is None:
+            backend = ControlSlots(ez, self.slots, table) if self.control else CudaSlots(ez, self.slots, max_length_s, table)
+        self.backend = backend
         self._queue: collections.deque = collections.deque()
         self._active: List[Optional[_Active]] = [None] * self.slots
         self._tickets = 0
 
     # ---- requests
     def _frames(self, r: Request) -> int:
-        if not isinstance(r.ddim_steps, numbers.Integral) or isinstance(r.ddim_steps, bool) or int(r.ddim_steps) not in self._scheds:
-            raise ValueError(f"ddim_steps {r.ddim_steps} is not one of this engine's step counts {list(self.ddim_steps)}")
+        self._check_common(r)
         if not isinstance(r.length, numbers.Real) or isinstance(r.length, bool) or not math.isfinite(r.length) or r.length <= 0:
             raise ValueError(f"length must be a positive number of seconds, got {r.length!r}")
         frames = int(r.length * self.backend.latent_sr)
         if not 1 <= frames <= self.backend.max_frames:
             raise ValueError(f"length {r.length} s is {frames} frames; this engine serves 1..{self.backend.max_frames}")
+        return frames
+
+    def _check_common(self, r):
+        if not isinstance(r.ddim_steps, numbers.Integral) or isinstance(r.ddim_steps, bool) or int(r.ddim_steps) not in self._scheds:
+            raise ValueError(f"ddim_steps {r.ddim_steps} is not one of this engine's step counts {list(self.ddim_steps)}")
         s = r.random_seed
         if s is not None and (not isinstance(s, numbers.Integral) or isinstance(s, bool) or not 0 <= int(s) < 2 ** 63):
             raise ValueError(f"random_seed must be None or an integer in [0, 2**63), got {s!r}")
@@ -109,16 +125,43 @@ class ContinuousEngine:
                 raise ValueError(f"{name} must be a finite number or None, got {v!r}")
         if (r.eta or 0) < 0:
             raise ValueError(f"eta must be >= 0, got {r.eta}")
-        return frames
+
+    def _control_wave(self, r: ControlRequest) -> np.ndarray:
+        """Checks a ControlNet request and loads its reference clip (host only)."""
+        self._check_common(r)
+        for name in ("surpass_noise", "conditioning_scale"):
+            v = getattr(r, name)
+            if not isinstance(v, numbers.Real) or isinstance(v, bool) or not math.isfinite(v):
+                raise ValueError(f"{name} must be a finite number, got {v!r}")
+        if r.surpass_noise < 0:
+            raise ValueError(f"surpass_noise must be >= 0, got {r.surpass_noise}")
+        a = r.audio
+        if isinstance(a, (str, os.PathLike)):
+            from .api import _load_audio
+            try:
+                a = _load_audio(os.fspath(a), self.backend.sr)
+            except (OSError, ValueError) as e:
+                raise ValueError(f"cannot read the reference clip {r.audio!r}: {e}") from e
+        elif isinstance(a, np.ndarray):
+            a = np.asarray(a, dtype=np.float32)
+        else:
+            raise ValueError(f"audio must be a path or a float32 mono waveform, got {type(a).__name__}")
+        if a.ndim != 1 or a.size < 1 or not np.isfinite(a).all():
+            raise ValueError(f"the reference clip must be a non-empty, finite mono waveform, got shape {a.shape}")
+        return a
 
     def submit(self, prompt: str, **kw) -> int:
-        """Queues a request (the keyword arguments of `frontend.Request`); returns its ticket.  Invalid requests raise ValueError here,
-        before any device work."""
-        r = Request(prompt, **kw)
-        frames = self._frames(r)
+        """Queues a request (the keyword arguments of `frontend.Request`, or of `frontend.ControlRequest` for a ControlNet engine); returns
+        its ticket.  Invalid requests raise ValueError here, before any device work; a reference clip given as a path is read here."""
+        if self.control:
+            r = ControlRequest(prompt, **kw)
+            item = (r, self.backend.max_frames, self._control_wave(r))
+        else:
+            r = Request(prompt, **kw)
+            item = (r, self._frames(r), None)
         t = self._tickets
         self._tickets += 1
-        self._queue.append((t, r, frames))
+        self._queue.append((t,) + item)
         return t
 
     def pending(self) -> int:
@@ -129,8 +172,12 @@ class ContinuousEngine:
     def _admit(self):
         for k in range(self.slots):
             if self._active[k] is None and self._queue:
-                t, r, frames = self._queue.popleft()
-                self.backend.admit(k, r.prompt, None if r.random_seed is None else int(r.random_seed), frames)
+                t, r, frames, wave = self._queue.popleft()
+                seed = None if r.random_seed is None else int(r.random_seed)
+                if self.control:
+                    self.backend.admit(k, r.prompt, seed, frames, audio=wave, surpass_noise=float(r.surpass_noise))
+                else:
+                    self.backend.admit(k, r.prompt, seed, frames)
                 n = int(r.ddim_steps)
                 self._active[k] = _Active(t, r, frames, self._timesteps[n], self._scheds[n])
 
@@ -149,7 +196,7 @@ class ContinuousEngine:
             eta = float(r.eta or 0.0)
             cfg = bool(r.guidance_scale) and r.prompt != ""   # "" switches guidance off (api/ezaudio.py:109-111)
             plan.append(SlotStep(self._row[t], a.frames, float(r.guidance_scale) if cfg else 0.0, float(r.guidance_rescale or 0.0),
-                                 a.sched.step_coefficients(t, eta), cfg, eta > 0))
+                                 a.sched.step_coefficients(t, eta), cfg, eta > 0, float(r.conditioning_scale) if self.control else 1.0))
         self.backend.step(plan)
         done = []
         for k, a in enumerate(self._active):
@@ -175,7 +222,7 @@ class ContinuousEngine:
         if requests is not None:
             tickets = [self.submit(**dataclasses.asdict(r)) for r in requests]
         else:
-            tickets = [t for t, _, _ in self._queue]
+            tickets = [q[0] for q in self._queue]
         pos = {t: i for i, t in enumerate(tickets)}
         out: List[Optional[Tuple[int, object]]] = [None] * len(tickets)
         for t, sr, w in self.stream():
@@ -314,3 +361,76 @@ class CudaSlots:
             self.lat[k].zero_()
             self.gens[k] = None
             return wav[0, 0].cpu().numpy()
+
+
+class ControlSlots(CudaSlots):
+    """Device side of ContinuousEngine for an `api.EzAudio_ControlNet`: CudaSlots plus the ControlNet's context rows, condition cache and
+    per-sample conditioning scales.  Every clip is 10 s long (the reference's), so the step runs without per-sample lengths.
+
+    Between steps the engine also owns the ControlNet's context, timestep table and condition cache; the next step restores whatever a
+    generate_audio call replaced."""
+    control = True
+
+    def __init__(self, ez, slots: int, table: Sequence[int]):
+        super().__init__(ez, slots, 10.0, table)
+        self.cn = ez.controlnet
+        p = ez.params["autoencoder"]
+        self.num_samples = int(10 * self.sr)
+        if round(self.num_samples / self.sr * p["latent_sr"]) != self.max_frames:
+            raise ValueError("the ControlNet clip length does not match the padded length")
+        self.cond_kw = {k: v for k, v in ez.params["conditioner"].items() if k != "condition_type"}
+        S, Be, L, D = self.S, 2 * self.S, self.max_frames, int(self.unet.cfg["embed_dim"])
+        with torch.cuda.device(self.device):
+            self.cond = torch.zeros(Be, 1, 2 * L, device=self.device)   # rows k and S + k: slot k's condition (the CFG rows repeat it)
+            self._sh = torch.zeros(Be, dtype=torch.float32, pin_memory=True)
+            self.scale = torch.zeros(Be, dtype=torch.float32, device=self.device)
+            self.skips = [torch.empty(Be, L, D, device=self.device) for _ in range(self.cn.half)]
+        self.n_samples: List[int] = [0] * S
+        self._cn_ctx_epoch = self._cond_epoch = None
+
+    def _own_denoiser(self):
+        super()._own_denoiser()
+        self.cn.set_timesteps(self.table)
+        h = self.cn._h
+        if self._cn_ctx_epoch != h.ctx_epoch:
+            self.cn.set_context(self.ctx, self.cmask)
+            self._cn_ctx_epoch = h.ctx_epoch
+        if self._cond_epoch != self.cn.cond_epoch:
+            self.cn.set_condition(self.cond)
+            self._cond_epoch = self.cn.cond_epoch
+
+    def admit(self, k: int, prompt: str, seed: Optional[int], frames: int, audio=None, surpass_noise: float = 0.0):
+        from .api import energy_condition
+        super().admit(k, prompt, seed, frames)   # the DiT's context row, the generator and the initial noise
+        with torch.cuda.device(self.device):
+            self.cn.set_context_rows(self.ctx[k:k + 1], self.cmask[k:k + 1], k)
+            # normalise, noise-gate and pad / crop to 10 s, then the energy condition: generate_audio's preparation of one clip
+            wave = post.prepare_wave(torch.from_numpy(audio).to(self.device).unsqueeze(0), self.num_samples, normalize=True, gate=surpass_noise)
+            c = energy_condition(wave, **self.cond_kw)
+            for row in (k, self.S + k):
+                self.cond[row:row + 1].copy_(c)
+                self.cn.set_condition_rows(self.cond[row:row + 1], row)
+            self.n_samples[k] = len(audio)
+
+    def _launch_step(self):
+        S = self.S
+        self.x_in[:S].copy_(self.lat)
+        self.x_in[S:].copy_(self.lat)
+        sk = self.cn.forward_step(self.x_in, t_index=self.t_index, scale=self.scale, outs=self.skips)
+        self.unet.forward_step(self.x_in, 0, controlnet_skips=sk, out=self.out, t_index=self.t_index)
+        _lib.check(_lib.lib().ezb_cfg_ddim_step_slots(self.device.index, _lib.ptr(self.out), _lib.ptr(self.lat), _lib.ptr(self.noise),
+                                                      _lib.ptr(self.slots_dev), S, self.C, self.max_frames, _lib.stream_ptr(), None))
+
+    def step(self, plan: Sequence[Optional[SlotStep]]):
+        with torch.cuda.device(self.device):
+            if self._copied is not None:
+                self._copied.synchronize()   # the previous step's copies have read the pinned blocks
+            sh = self._sh.numpy()
+            for k, e in enumerate(plan):
+                sh[k] = sh[self.S + k] = 0.0 if e is None else e.conditioning_scale
+            self.scale.copy_(self._sh, non_blocking=True)   # ordered before the event CudaSlots.step records after its own copy
+        super().step(plan)
+
+    def finish(self, k: int, frames: int):
+        """As CudaSlots.finish, trimmed to the reference clip's length (api/controlnet.py:159)."""
+        return super().finish(k, frames)[:self.n_samples[k]]

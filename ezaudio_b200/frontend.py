@@ -39,6 +39,22 @@ class Request:
                 self.prompt == "")
 
 
+@dataclasses.dataclass(frozen=True)
+class ControlRequest:
+    """One ControlNet request: the arguments of api/controlnet.py:113-118 (defaults included).  `audio` is the reference clip: a path, or a
+    float32 mono waveform at the model's sample rate.  The clip is 10 s long, like the reference's; its waveform is trimmed to the length of
+    the reference clip."""
+    prompt: str
+    audio: object
+    surpass_noise: float = 0
+    guidance_scale: float = 3.5
+    guidance_rescale: float = 0
+    ddim_steps: int = 50
+    eta: float = 1
+    conditioning_scale: float = 1
+    random_seed: Optional[int] = None
+
+
 def length_bucket_bin(length: float, length_bucket_s: float) -> int:
     """Bucket index of a clip length: ceil(length / bucket), so bucket k holds lengths in ((k - 1) * bucket, k * bucket]."""
     return max(1, math.ceil(length / length_bucket_s - 1e-9))

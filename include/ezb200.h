@@ -8,6 +8,7 @@
  * Conventions: plain pointers and sizes, no torch types.  Every device pointer is owned by the caller (PyTorch) and
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
+ * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev,
  * cfg_ddim_step, cfg_ddim_step_slots, decode, encode, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
@@ -95,6 +96,20 @@ int ezb_dit_set_context_rows(ezb_dit* h, const float* ctx, const uint8_t* ctx_ma
  * t_index_host when they are not all equal (a batch that shares one timestep may take other kernels there). */
 int ezb_dit_forward_tdev(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_dev,
                          const float* const* controlnet_skips, float* out, int Be, int L, void* stream, const int32_t* lens);
+/* ControlNet handles.  ezb_controlnet_set_condition: runs the stem (controlnet_pre, which does not depend on the timestep) of condition
+ * (Be,1,2L) fp32 DEVICE once, into a condition cache [Be, L, embed_dim] the handle owns; ezb_controlnet_forward neither reads nor writes it.
+ * The call fixes the cache layout (Be, L).  ezb_controlnet_set_condition_rows: rows [row0, row0 + n) of that layout from condition (n,1,2L);
+ * the other rows keep what they hold.  It fails with EZB_ERR_STATE when there is no layout or L differs from it, with EZB_ERR_SHAPE when the
+ * rows fall outside the batch; the rows come out bit-identical to ezb_controlnet_set_condition of the whole updated batch.
+ * ezb_controlnet_forward_tdev: ezb_controlnet_forward with the per-sample timestep indices t_index_dev int32 [Be] and conditioning scales
+ * scale_dev fp32 [Be] in DEVICE memory (read when the kernels run, like ezb_dit_forward_tdev's indices) and the condition from the cache;
+ * Be must match the context batch and the condition layout, L the layout.  Sample b's skips are the zero-linear outputs times scale_dev[b]
+ * (0 gives zeros).  For host indices that are not all equal, each sample whose scale s != 0 comes out bit-identical to
+ * ezb_controlnet_forward with those indices, the same condition and conditioning_scale s.  All three are graph-safe, no synchronisation. */
+int ezb_controlnet_set_condition(ezb_dit* h, const float* condition, int Be, int L, void* stream);
+int ezb_controlnet_set_condition_rows(ezb_dit* h, const float* condition, int row0, int n, int L, void* stream);
+int ezb_controlnet_forward_tdev(ezb_dit* h, const float* x, const int32_t* t_index_dev, const float* scale_dev, float* const* skips_out, int Be,
+                                int L, void* stream);
 
 /* --- fused classifier-free guidance + rescale + DDIM update (src/inference.py:12-23,88-100; diffusers DDIMScheduler.step
  * restated, SURVEY Appendix B).  model_out holds B text rows followed by B uncond rows when guidance_scale != 0, else B
