@@ -168,8 +168,15 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank)
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
   return r;
 }
+// Arrive on a barrier of any CTA of the cluster, releasing this thread's prior memory accesses at cluster scope: for barriers that publish
+// generic-proxy data to the peer.  ptxas emits MEMBAR.ALL.CTA + MEMBAR.ALL.GPU before every such arrive.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+// The same arrive without the cluster-scope release (the default .release.cta semantics; a bare SYNCS.ARRIVE, no fence): for barriers
+// whose arrival publishes no generic-proxy data, only that async-proxy work tracked elsewhere (wgmma.wait_group) has completed.
+__device__ __forceinline__ void mbar_arrive_cluster_nofence(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ void mbar_inval(uint64_t* bar) {
   asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");

@@ -809,10 +809,15 @@ __device__ __forceinline__ void gemm_mainloop(float (&d)[GemmCfg<BN, Epi, KSUB>:
                                               uint32_t& stage, uint32_t& phase) {
   using SM = GemmCfg<BN, Epi, KSUB>;
   constexpr int NSUB = SM::NSUB, NH = SM::NH, HN = SM::HN;
-  auto release = [&](uint32_t s) {   // one thread per warpgroup, on the slot's barrier in every CTA of the cluster
+  // One thread per warpgroup arrives on the slot's barrier in every CTA of the cluster, without a release fence: the slot's only readers
+  // are this warpgroup's wgmma (async proxy), complete at the wgmma.wait_group before the release; its only writer is a producer's TMA
+  // (async proxy), issued after that producer's try_wait has observed the arrival; and no generic-proxy data is published through `empty`.
+  // A .release.cluster arrive would put two fences (MEMBAR.ALL.CTA + MEMBAR.ALL.GPU) in front of every arrive of every k-block, and the
+  // warpgroup's next .sync.aligned wgmma would wait for them.
+  auto release = [&](uint32_t s) {
     if ((threadIdx.x & 127) == 0) {
       if (MC == 1) mbar_arrive(&empty[s]);
-      else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
+      else for (int r = 0; r < MC; ++r) mbar_arrive_cluster_nofence(mapa_u32(smem_u32(&empty[s]), r));
     }
   };
   static_assert(HN <= 256 && HN % 8 == 0, "BN");   // HN % 8: the second half starts on a 1024-byte swizzle atom
@@ -1054,7 +1059,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
       EZB_DBG(w4 += clock64() - te;)
       fence_proxy_async_smem();   // this warp's generic accesses to the ring are ordered before the producer's next TMA writes into it
       __syncwarp();
-      if (lane == 0) {
+      if (lane == 0) {   // cluster-scope release (once per tile): the epilogue's generic reads of the ring precede the peers' multicast into it
         if (MC == 1) mbar_arrive(acc_free);
         else for (int r = 0; r < MC; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(acc_free), r));
       }

@@ -1,7 +1,8 @@
 """GEMM micro-benchmark through the C-ABI test hooks: TFLOP/s per kernel variant on the DiT shapes, plus the cycle counters of CTA 0 of the
 2-CTA cluster launches (gemm.cuh GemmShape::dbg; build with EZB_DEBUG=1 for them to count).
   python profiles/gemm_bench.py                  # both sections
-  python profiles/gemm_bench.py heads            # only the fused Q/K/V-heads GEMMs (ezb_test_heads), or `linear` for the others"""
+  python profiles/gemm_bench.py heads            # only the fused Q/K/V-heads GEMMs (ezb_test_heads), or `linear` for the others
+  python profiles/gemm_bench.py m=4000,8000      # only the DiT block's GEGLU / MLP-out / QKV / cross-Q GEMMs and their alternatives, per M"""
 import ctypes as C
 import math
 import os
@@ -22,7 +23,7 @@ def run(M, N, K, bn, kind, label, resid=False, reps=20):
     bias = torch.randn(N, device="cuda")
     e = _lib.TestEpilogue()
     e.bias = bias.data_ptr()
-    geglu = kind in (1, 11)
+    geglu = kind in (1, 11, 12)
     if geglu:
         out = torch.empty(M, N // 2, device="cuda", dtype=torch.bfloat16)
         e.out_bf16, e.ld16 = out.data_ptr(), N // 2
@@ -105,6 +106,22 @@ def heads(B, Lt, H, dh, nsec, variant, label, reps=20):
 
 
 SECTIONS = [a for a in sys.argv[1:] if a in ("linear", "heads")] or ["linear", "heads"]
+# m=4000,8000: token counts of XL at Be = 8 and 16, L = 500; each block GEMM next to the alternatives its runtime options select
+MS = next((list(map(int, a[2:].split(","))) for a in sys.argv[1:] if a.startswith("m=")), None)
+if MS is not None:
+    if "linear" in SECTIONS:
+        for M in MS:
+            run(M, 9216, 1152, 256, 11, "pair geglu 256")
+            run(M, 9216, 1152, 256, 12, "pair geglu 256 ksub2")
+            run(M, 1152, 4608, 256, 20, "swapAB mlp2 resid+gate", resid=True)
+            run(M, 1152, 4608, 128, 10, "pair mlp2 resid+gate 128", resid=True)
+    if "heads" in SECTIONS:
+        for M in MS:
+            heads(M // 500, 500, 16, 72, 3, PACKED3, "XL self-QKV")
+            heads(M // 500, 500, 16, 72, 3, PACKED3_KSUB2, "XL self-QKV")
+            heads(M // 500, 500, 16, 72, 1, PAIR, "XL cross-Q")
+            heads(M // 500, 500, 16, 72, 1, SINGLE, "XL cross-Q")
+    SECTIONS = []
 if "linear" in SECTIONS:
     M = 4000
     run(M, 9216, 1152, 256, 11, "pair geglu 256")
