@@ -83,6 +83,12 @@ class TestStepArgs(C.Structure):
                [("f32_out", C.c_void_p * 3), ("bf_out", C.c_void_p * 3)]
 
 
+class TestCondArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "M", "D", "F", "kmul", "vocab")] + [("eps", C.c_float)] + \
+               [(n, C.c_int32) for n in ("B", "L", "H", "dk", "c0", "c1", "stage")] + \
+               [(n, C.c_void_p) for n in ("in_", "w", "b", "k", "v", "key_mask", "out", "out32", "out_v")]
+
+
 _lib = None
 
 _VP, _I, _F = C.c_void_p, C.c_int, C.c_float
@@ -139,6 +145,7 @@ _SIGS = {
     "ezb_test_vae": ([_I, C.POINTER(TestVaeArgs), _VP], _I),
     "ezb_test_fp8": ([_I, C.POINTER(TestFp8Args), _VP], _I),
     "ezb_test_step": ([_I, C.POINTER(TestStepArgs), _VP], _I),
+    "ezb_test_cond": ([_I, C.POINTER(TestCondArgs), _VP], _I),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -66,11 +66,17 @@ __global__ void __launch_bounds__(SA_WARPS * 32) attn_simt_kernel(const float* _
       sV[r * dh + d] = ok ? vb[(size_t)(k0 + r) * dh + d] : 0.f;
     }
     __syncthreads();
-    bool ok0 = k0 + lane < lk, ok1 = k0 + lane + 32 < lk;
+    const bool in0 = k0 + lane < lk, in1 = k0 + lane + 32 < lk;
+    bool ok0 = in0, ok1 = in1;
     if (key_mask) {
       ok0 = ok0 && key_mask[(size_t)b * Lk + k0 + lane];
       ok1 = ok1 && key_mask[(size_t)b * Lk + k0 + lane + 32];
     }
+    // A masked key scores -inf, so a query whose keys are all masked has l = 0 and is written as zeros (as the tensor-core kernels and SDPA
+    // do).  T5 (bias != null) masks additively with finfo(float32).min instead, as transformers does: the masked scores all stay -FLT_MAX
+    // after the subtract a - mn, so a fully masked row becomes the mean of V over the lk keys.  The zero-filled tile padding past lk stays
+    // -inf in both modes.
+    const float masked = bias != nullptr ? -3.40282347e38f : -INFINITY;
     // scores of this warp's SA_QW queries against the lane's two keys
     float s0[SA_QW], s1[SA_QW];
 #pragma unroll
@@ -99,8 +105,8 @@ __global__ void __launch_bounds__(SA_WARPS * 32) attn_simt_kernel(const float* _
           if (k0 + lane + 32 < Lk) a1 += br[lane + 32];
         }
       }
-      a0 = ok0 ? a0 : -INFINITY;
-      a1 = ok1 ? a1 : -INFINITY;
+      a0 = ok0 ? a0 : (in0 ? masked : -INFINITY);
+      a1 = ok1 ? a1 : (in1 ? masked : -INFINITY);
       const float mn = fmaxf(m[qi], warp_max(fmaxf(a0, a1)));
       const float corr = (mn == -INFINITY) ? 1.f : expf(m[qi] - mn);
       const float p0 = (mn == -INFINITY) ? 0.f : expf(a0 - mn);
@@ -140,7 +146,7 @@ __global__ void __launch_bounds__(SA_WARPS * 32) attn_simt_kernel(const float* _
   for (int qi = 0; qi < SA_QW; ++qi) {
     const int qrow = q0 + warp * SA_QW + qi;
     if (qrow >= Lq) continue;
-    const float inv = 1.f / l[qi];
+    const float inv = l[qi] > 0.f ? 1.f / l[qi] : 0.f;   // l = 0: every key masked (acc is 0 too)
     const bool valid = !VARLEN || qrow < lq;
     __nv_bfloat16* o = out + ((size_t)b * Lq + qrow) * kmul * D;
 #pragma unroll

@@ -1115,22 +1115,34 @@ inline int Dit::controlnet_forward(const float* x, const float* gt, const uint8_
   return controlnet_trunk(x, gt, gt_mask, tidx, tall, nullptr, cond, cscale, nullptr, skips_out, Be, L, st);
 }
 
-// The stem (controlnet_pre, controlnet.py:65-84) of Be conditions (Be,1,2L) into out (Be,L,D).  It depends on the condition only, and every
-// kernel computes each output element on its own, so a clip's rows do not depend on the batch.
+// The four convolutions of the stem (controlnet_pre, controlnet.py:65-84) for conditions of 2L samples, as conv1d_direct_kernel takes them.
+struct StemConv { int Cin, cin_real, Tin, Cout, Tout, K, stride, pad, act, transposed; };
+inline StemConv stem_conv(int stage, int c0, int c1, int D, int L) {
+  const int T = 2 * L;
+  switch (stage) {
+    case 0: return {1, 1, T, c0, T, 1, 1, 0, 0, 0};                 // conv_in
+    case 1: return {c0 + 1, c0, T, c0 + 1, T, 3, 1, 1, 1, 0};       // conv3 + SiLU (mask channel == 0)
+    case 2: return {c0 + 1, c0 + 1, T, c1, L, 3, 2, 1, 1, 0};       // conv3 stride 2 + SiLU
+    default: return {c1, c1, L, D, L, 1, 1, 0, 0, 1};               // conv_out -> (B,L,D)
+  }
+}
+inline int stem_conv_launch(cudaStream_t st, const StemConv& c, const float* in, const float* w, const float* bias, float* out, int B) {
+  const size_t n = (size_t)B * c.Cout * c.Tout;
+  ++launch_counter();
+  conv1d_direct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, w, bias, out, B, c.Cin, c.cin_real, c.Tin, c.Cout, c.Tout, c.K, c.stride, c.pad,
+                                                                     c.act, c.transposed);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+
+// The stem of Be conditions (Be,1,2L) into out (Be,L,D).  It depends on the condition only, and every kernel computes each output element on its
+// own, so a clip's rows do not depend on the batch.
 inline int Dit::controlnet_stem(const float* cond, float* out, int Be, int L, cudaStream_t st) {
-  const int c0 = d.cond_c0, c1 = d.cond_c1, T = 2 * L;
-  auto conv = [&](const float* in, const float* w, const float* b, float* o, int Cin, int cin_real, int Tin, int Cout, int Tout, int K, int stride, int pad,
-                  int act, int tr) -> int {
-    const size_t n = (size_t)Be * Cout * Tout;
-    ++launch_counter();
-    conv1d_direct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, w, b, o, Be, Cin, cin_real, Tin, Cout, Tout, K, stride, pad, act, tr);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
-  };
-  EZB_TRY(conv(cond, cs_in_w, cs_in_b, cs_t0, 1, 1, T, c0, T, 1, 1, 0, 0, 0));              // conv_in
-  EZB_TRY(conv(cs_t0, cs_c0_w, cs_c0_b, cs_t1, c0 + 1, c0, T, c0 + 1, T, 3, 1, 1, 1, 0));    // conv3 + SiLU (mask channel == 0)
-  EZB_TRY(conv(cs_t1, cs_c1_w, cs_c1_b, cs_t2, c0 + 1, c0 + 1, T, c1, L, 3, 2, 1, 1, 0));    // conv3 stride 2 + SiLU
-  EZB_TRY(conv(cs_t2, cs_out_w, cs_out_b, out, c1, c1, L, D, L, 1, 1, 0, 0, 1));             // conv_out -> (B,L,D)
+  const float* const ins[4] = {cond, cs_t0, cs_t1, cs_t2};
+  const float* const ws[4] = {cs_in_w, cs_c0_w, cs_c1_w, cs_out_w};
+  const float* const bs[4] = {cs_in_b, cs_c0_b, cs_c1_b, cs_out_b};
+  float* const outs[4] = {cs_t0, cs_t1, cs_t2, out};
+  for (int s = 0; s < 4; ++s) EZB_TRY(stem_conv_launch(st, stem_conv(s, d.cond_c0, d.cond_c1, D, L), ins[s], ws[s], bs[s], outs[s], Be));
   return EZB_OK;
 }
 
@@ -1164,9 +1176,13 @@ inline int Dit::controlnet_forward_tdev(const float* x, const int32_t* tdev, con
 }
 
 // cond: the raw condition, run through the stem into cond_emb here, or null for the condition cache.  scale_dev (device [Be]) or, when null,
-// the uniform cscale (0 treated as 1).
+// the uniform cscale.  A uniform scale of 0 writes zero skips without running the trunk: the zero-linears' out_scale reads 0 as 1.
 inline int Dit::controlnet_trunk(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const int32_t* tdev,
                                  const float* cond, float cscale, const float* scale_dev, float* const* skips_out, int Be, int L, cudaStream_t st) {
+  if (scale_dev == nullptr && cscale == 0.f) {
+    for (int i = 0; i < half; ++i) EZB_CUDA(cudaMemsetAsync(skips_out[i], 0, (size_t)Be * L * D * sizeof(float), st));
+    return EZB_OK;
+  }
   lens = nullptr;   // the stem convs cross clip ends: ControlNet batches are uniform in length
   dev->tmaps.trim();
   WeightSeqScope ws(dev, this, 2, ((long long)Be << 32) | (unsigned)L);

@@ -525,6 +525,79 @@ __attribute__((visibility("default"))) int ezb_test_step(int device, const ezb_t
   }
 }
 
+}  // extern "C"
+
+namespace {
+int test_cond_check(const ezb_test_cond_args* a) {
+  const int kind = a->kind;
+  if (kind < 0 || kind > 6) return fail(EZB_ERR_ARG, "ezb_test_cond: kind %d", kind);
+  if (!a->in || (!a->out && !(kind == 1 && a->out32))) return fail(EZB_ERR_ARG, "ezb_test_cond: null input or output");
+  if ((kind == 1 || kind == 4 || kind == 5) && a->kmul != 1 && a->kmul != 3)
+    return fail(EZB_ERR_ARG, "ezb_test_cond: kmul %d (1 or 3)", a->kmul);
+  if (kind <= 1) {
+    if (a->M < 1 || a->M > (1 << 24) || a->D < 4 || a->D % 4 || (long long)a->M * a->D > (1LL << 30))
+      return fail(EZB_ERR_SHAPE, "ezb_test_cond: M %d D %d (D a multiple of 4)", a->M, a->D);
+    if (!a->w) return fail(EZB_ERR_ARG, "ezb_test_cond: kind %d needs w", kind);
+    if (kind == 0 && a->vocab < 1) return fail(EZB_ERR_SHAPE, "ezb_test_cond: vocabulary of %d", a->vocab);
+    if (kind == 1 && !(a->eps >= 0.f)) return fail(EZB_ERR_ARG, "ezb_test_cond: eps %g", a->eps);
+    // t5_embed / t5_rms read their rows and write the fp32 output as float4
+    const void* ps[] = {a->in, a->w, kind == 0 ? a->out : nullptr, a->out32};
+    for (const void* p : ps)
+      if (reinterpret_cast<uintptr_t>(p) & 15) return fail(EZB_ERR_ARG, "ezb_test_cond: kind %d pointers must be 16-byte aligned", kind);
+    return EZB_OK;
+  }
+  if (kind == 2 || kind == 3 || kind == 5) {
+    const bool per_head = kind != 3;   // t5_bias has no batch and no head dimension
+    if (a->L < 1 || a->H < 1 || (long long)a->H * a->L * a->L > (1LL << 28) ||
+        (per_head && (a->B < 1 || a->dk < 1 || (long long)a->B * a->L * a->H * a->dk > (1LL << 28) || (long long)a->B * a->H > 65535)))
+      return fail(EZB_ERR_SHAPE, "ezb_test_cond: B %d L %d H %d dk %d", a->B, a->L, a->H, a->dk);
+    if (kind == 2 && (!a->out32 || !a->out_v)) return fail(EZB_ERR_ARG, "ezb_test_cond: t5_heads writes q (out), k (out32) and v (out_v)");
+    if (kind == 3 && !a->w) return fail(EZB_ERR_ARG, "ezb_test_cond: t5_bias needs the bucket table w");
+    if (kind == 5) {
+      if (a->dk % 4 || a->dk > 96) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_cond: T5 attention head dimension %d (a multiple of 4, at most 96)", a->dk);
+      if (!a->k || !a->v || !a->b) return fail(EZB_ERR_ARG, "ezb_test_cond: T5 attention needs k, v and the position bias b");
+      const void* ps[] = {a->in, a->k, a->v};
+      for (const void* p : ps)
+        if (reinterpret_cast<uintptr_t>(p) & 15) return fail(EZB_ERR_ARG, "ezb_test_cond: q, k and v must be 16-byte aligned");
+    }
+    return EZB_OK;
+  }
+  if (kind == 4) {
+    if (a->M < 1 || a->F < 1 || (long long)a->M * a->F > (1LL << 30)) return fail(EZB_ERR_SHAPE, "ezb_test_cond: gated GELU M %d F %d", a->M, a->F);
+    return EZB_OK;
+  }
+  if (a->stage < 0 || a->stage > 3) return fail(EZB_ERR_ARG, "ezb_test_cond: stem stage %d", a->stage);
+  if (a->B < 1 || a->L < 1 || a->c0 < 1 || a->c1 < 1 || a->D < 1 || (long long)a->B * 2 * a->L * (a->c0 + 1 > a->c1 ? a->c0 + 1 : a->c1) > (1LL << 30) ||
+      (long long)a->B * a->L * a->D > (1LL << 30))
+    return fail(EZB_ERR_SHAPE, "ezb_test_cond: stem B %d L %d widths %d, %d, %d", a->B, a->L, a->c0, a->c1, a->D);
+  if (!a->w || !a->b) return fail(EZB_ERR_ARG, "ezb_test_cond: the stem convolution needs w and b");
+  return EZB_OK;
+}
+}  // namespace
+
+extern "C" {
+
+__attribute__((visibility("default"))) int ezb_test_cond(int device, const ezb_test_cond_args* a, void* stream) {
+  if (!a) return fail(EZB_ERR_ARG, "ezb_test_cond: null arguments");
+  EZB_TRY(test_cond_check(a));
+  EZB_CUDA(cudaSetDevice(device));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  __nv_bfloat16* o16 = static_cast<__nv_bfloat16*>(a->out);
+  float* o32 = static_cast<float*>(a->out);
+  const float* x = static_cast<const float*>(a->in);
+  switch (a->kind) {
+    case 0: return t5_embed_launch(st, static_cast<const int32_t*>(a->in), a->w, o32, a->M, a->D, a->vocab);
+    case 1: return t5_rms_launch(st, x, a->w, o16, a->out32, a->M, a->D, a->kmul, a->eps);
+    case 2: return t5_heads_launch(st, x, o32, a->out32, a->out_v, a->B, a->L, a->H, a->dk);
+    case 3: return t5_bias_launch(st, static_cast<const int32_t*>(a->in), a->w, o32, a->H, a->L);
+    case 4: return t5_gated_gelu_launch(st, x, o16, a->M, a->F, a->kmul);
+    case 5:
+      EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+      return t5_attention_launch(st, x, a->k, a->v, a->key_mask, a->b, o16, a->B, a->H, a->L, a->dk, a->kmul);
+    default: return stem_conv_launch(st, stem_conv(a->stage, a->c0, a->c1, a->D, a->L), x, a->w, a->b, o32, a->B);
+  }
+}
+
 #define EZB_API __attribute__((visibility("default")))
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
@@ -661,6 +734,8 @@ EZB_API int ezb_energy_condition(int device, const float* audio, float* out, int
                                  void* stream) {
   if (!audio || !out) return fail(EZB_ERR_ARG, "ezb_energy_condition: null pointer");
   if (B < 1 || hop < 1 || win < hop || T < hop) return fail(EZB_ERR_SHAPE, "ezb_energy_condition: B=%d T=%d hop=%d window=%d", B, T, hop, win);
+  // an odd window - hop: the reference pads (win - hop - 1) / 2 samples per side and returns (T - 1) / hop frames, not the T / hop computed here
+  if ((win - hop) % 2) return fail(EZB_ERR_UNSUPPORTED, "ezb_energy_condition: window %d - hop %d is odd", win, hop);
   const int pad = (win - hop) / 2, n_frames = T / hop;
   if (pad >= T) return fail(EZB_ERR_SHAPE, "ezb_energy_condition: reflect padding %d needs more than %d samples", pad, T);
   if ((size_t)n_frames * sizeof(float) > 200 * 1024) return fail(EZB_ERR_SHAPE, "ezb_energy_condition: %d frames exceed the shared-memory table", n_frames);

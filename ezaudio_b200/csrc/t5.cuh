@@ -76,6 +76,48 @@ __global__ void t5_gated_gelu_kernel(const float* __restrict__ u, __nv_bfloat16*
   store_act(out + (size_t)m * kmul * F, c, F, kmul, 0.5f * g * (1.0f + t) * h);
 }
 
+// The launches of T5::forward (grids and shared memory), shared with the ezb_test_cond hook.
+inline unsigned t5_grid(size_t n) { return (unsigned)((n + 255) / 256); }
+inline int t5_embed_launch(cudaStream_t st, const int32_t* ids, const float* table, float* x, int M, int D, int vocab) {
+  ++launch_counter();
+  t5_embed_kernel<<<t5_grid((size_t)M * (D / 4)), 256, 0, st>>>(ids, table, x, M, D, vocab);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int t5_rms_launch(cudaStream_t st, const float* x, const float* w, __nv_bfloat16* out16, float* out32, int M, int D, int kmul, float eps) {
+  ++launch_counter();
+  t5_rms_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, w, out16, out32, M, D, kmul, eps);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int t5_heads_launch(cudaStream_t st, const float* qkv, float* q, float* k, float* v, int B, int L, int H, int dk) {
+  ++launch_counter();
+  t5_heads_kernel<<<t5_grid((size_t)B * L * 3 * H * dk), 256, 0, st>>>(qkv, q, k, v, B, L, H, dk);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int t5_bias_launch(cudaStream_t st, const int32_t* bucket, const float* table, float* bias, int H, int L) {
+  ++launch_counter();
+  t5_bias_kernel<<<t5_grid((size_t)H * L * L), 256, 0, st>>>(bucket, table, bias, H, L);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int t5_gated_gelu_launch(cudaStream_t st, const float* u, __nv_bfloat16* out, int M, int F, int kmul) {
+  ++launch_counter();
+  t5_gated_gelu_kernel<<<t5_grid((size_t)M * F), 256, 0, st>>>(u, out, M, F, kmul);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// unscaled attention with the position bias [H, L, L] and the key mask [B, L]; the caller has raised the kernel's shared-memory limit to 100 KB
+inline int t5_attention_launch(cudaStream_t st, const float* q, const float* k, const float* v, const uint8_t* mask, const float* bias, __nv_bfloat16* out,
+                               int B, int H, int L, int dk, int kmul) {
+  dim3 ga((L + SA_WARPS * SA_QW - 1) / (SA_WARPS * SA_QW), B * H);
+  ++launch_counter();
+  attn_simt_kernel<false><<<ga, SA_WARPS * 32, attn_simt_smem(dk), st>>>(q, k, v, mask, out, H, L, L, dk, 1.0f /* T5: no 1/sqrt(d) */, kmul, nullptr, bias);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+
 struct T5 {
   ezb_t5_desc d;
   Device* dev = nullptr;
@@ -239,46 +281,33 @@ struct T5 {
       }
       buckets = bucket_d;
     }
-    auto grid = [](size_t n) { return (unsigned)((n + 255) / 256); };
-    launch_counter() += 2;
-    t5_embed_kernel<<<grid((size_t)M * (D / 4)), 256, 0, st>>>(ids, emb, x, M, D, d.vocab_size);
-    t5_bias_kernel<<<grid((size_t)H * L * L), 256, 0, st>>>(buckets, rel, bias, H, L);
-    EZB_CUDA(cudaGetLastError());
+    EZB_TRY(t5_embed_launch(st, ids, emb, x, M, D, d.vocab_size));
+    EZB_TRY(t5_bias_launch(st, buckets, rel, bias, H, L));
     EpiLinearParams z;
     memset(&z, 0, sizeof z);
     static bool attr[16] = {};  // function attributes are per device
     if (!attr[dev->id & 15]) { EZB_CUDA(cudaFuncSetAttribute(attn_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr[dev->id & 15] = true; }
     for (int i = 0; i < nl; ++i) {
       const Layer& w = layers[i];
-      ++launch_counter();
-      t5_rms_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, w.ln0, act, nullptr, M, D, kmul, d.eps);
+      EZB_TRY(t5_rms_launch(st, x, w.ln0, act, nullptr, M, D, kmul, d.eps));
       EpiLinearParams e = z;
       e.out_f32 = qkv32; e.ld32 = 3 * inner;
       EZB_TRY(lin(st, act, D, w.qkv, M, 3 * inner, e));
-      launch_counter() += 2;
-      t5_heads_kernel<<<grid((size_t)M * 3 * inner), 256, 0, st>>>(qkv32, q32, k32, v32, B, L, H, dk);
-      dim3 ga((L + SA_WARPS * SA_QW - 1) / (SA_WARPS * SA_QW), B * H);
-      attn_simt_kernel<false><<<ga, SA_WARPS * 32, attn_simt_smem(dk), st>>>(q32, k32, v32, mask, attn, H, L, L, dk, 1.0f /* T5: no 1/sqrt(d) */, kmul, nullptr, bias);
-      EZB_CUDA(cudaGetLastError());
+      EZB_TRY(t5_heads_launch(st, qkv32, q32, k32, v32, B, L, H, dk));
+      EZB_TRY(t5_attention_launch(st, q32, k32, v32, mask, bias, attn, B, H, L, dk, kmul));
       e = z;
       e.resid = x; e.ldr = D; e.out_f32 = x; e.ld32 = D;
       EZB_TRY(lin(st, attn, inner, w.o, M, D, e));
-      ++launch_counter();
-      t5_rms_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, w.ln1, act, nullptr, M, D, kmul, d.eps);
+      EZB_TRY(t5_rms_launch(st, x, w.ln1, act, nullptr, M, D, kmul, d.eps));
       e = z;
       e.out_f32 = u32; e.ld32 = 2 * F;
       EZB_TRY(lin(st, act, D, w.wi, M, 2 * F, e));
-      ++launch_counter();
-      t5_gated_gelu_kernel<<<grid((size_t)M * F), 256, 0, st>>>(u32, mid, M, F, kmul);
-      EZB_CUDA(cudaGetLastError());
+      EZB_TRY(t5_gated_gelu_launch(st, u32, mid, M, F, kmul));
       e = z;
       e.resid = x; e.ldr = D; e.out_f32 = x; e.ld32 = D;
       EZB_TRY(lin(st, mid, F, w.wo, M, D, e));
     }
-    ++launch_counter();
-    t5_rms_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, lnf, nullptr, out, M, D, kmul, d.eps);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    return t5_rms_launch(st, x, lnf, nullptr, out, M, D, kmul, d.eps);
   }
 };
 

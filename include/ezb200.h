@@ -78,7 +78,7 @@ int ezb_dit_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* 
                     int t_index_all, const float* const* controlnet_skips, float* out, int Be, int L, void* stream,
                     const int32_t* lens);
 /* DiTControlNet.forward (controlnet.py:252-315): condition (Be,1,2L) fp32; writes depth/2 skips (Be,L,D) fp32, already
- * multiplied by conditioning_scale, into skips_out[i]. */
+ * multiplied by conditioning_scale, into skips_out[i] (conditioning_scale 0: zeros, without running the network). */
 int ezb_controlnet_forward(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_host,
                            int t_index_all, const float* condition, float conditioning_scale, float* const* skips_out, int Be,
                            int L, void* stream);
@@ -171,7 +171,8 @@ int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noise, floa
 
 /* EnergyExtractor.forward (src/models/conditions/energy.py:19-56) as wrapped by Conditioner (condition_wrapper.py:26-42): audio (B,T) fp32
  * -> (B, T/hop) fp32 frame energies in dB, normalised per clip when norm != 0; quantize_levels <= 1 disables quantisation. Only the shipped
- * padding mode ('reflect') exists. */
+ * padding mode ('reflect') exists.  Refused (EZB_ERR_UNSUPPORTED): an odd window_size - hop_size.  Refused (EZB_ERR_SHAPE): T < hop_size,
+ * window_size < hop_size, a reflect padding (window_size - hop_size) / 2 >= T, more than 51200 frames (the per-clip shared-memory table). */
 int ezb_energy_condition(int device, const float* audio, float* out, int B, int T, int hop_size, int window_size, float min_db, int norm,
                          int quantize_levels, void* stream);
 
@@ -336,6 +337,34 @@ typedef struct {
   void* out; float* f32_out[3]; void* bf_out[3];
 } ezb_test_step_args;
 int ezb_test_step(int device, const ezb_test_step_args* args, void* stream);
+/* The kernels that turn the prompt and the reference audio into DiT inputs (csrc/t5.cuh, the ControlNet stem's conv1d_direct_kernel),
+   launched one at a time with the grid and shared memory T5::forward and Dit::controlnet_stem use.  Device pointers; in, w and the fp32
+   outputs of kinds 0 and 1, and q, k, v of kind 5, are read / written as float4 and must be 16-byte aligned.  Every argument is checked
+   before any device work.
+   kind 0 t5_embed:      in int32 ids [M] (clamped to [0, vocab)), w table fp32 [vocab, D] -> out fp32 [M, D].  D a multiple of 4.
+   kind 1 t5_rms:        in x fp32 [M, D], w [D], eps -> out bf16 [M, kmul D] ([hi | lo | hi] when kmul is 3) and / or out32 fp32 [M, D].
+                         D a multiple of 4.
+   kind 2 t5_heads:      in qkv fp32 [B*L, 3*H*dk] -> out q, out32 k, out_v v, fp32 [B, H, L, dk] each.
+   kind 3 t5_bias:       in int32 buckets [L, L] (each < the rows of w), w relative_attention_bias fp32 [num_buckets, H] -> out fp32 [H, L, L].
+   kind 4 t5_gated_gelu: in u fp32 [M, 2F] = [h | g] -> out bf16 [M, kmul F] = gelu_new(g) h.
+   kind 5 T5 attention:  attn_simt_kernel with scale 1: in q, k, v fp32 [B, H, L, dk] (dk a multiple of 4, at most 96), b position bias fp32
+                         [H, L, L], key_mask uint8 [B, L] (NULL: every key) -> out bf16 [B, L, kmul H dk].
+   kind 6 conv1d_direct: convolution `stage` of the ControlNet stem (widths c0, c1 = cond_blocks, D = embed_dim) for conditions of 2L samples,
+                         w [Cout, Cin, K], b [Cout]:
+                         0 conv_in         Conv1d(1 -> c0, 1) of in [B, 1, 2L] -> out [B, c0, 2L];
+                         1 conv3 + SiLU    Conv1d(c0 + 1 -> c0 + 1, 3, padding 1) of [in | 0], in [B, c0, 2L] (the all-zero mask channel is
+                                           not read) -> out [B, c0 + 1, 2L];
+                         2 conv3 s2 + SiLU Conv1d(c0 + 1 -> c1, 3, stride 2, padding 1) of in [B, c0 + 1, 2L] -> out [B, c1, L];
+                         3 conv_out        Conv1d(c1 -> D, 1) of in [B, c1, L] -> out transposed, [B, L, D]. */
+typedef struct {
+  int32_t kind, M, D, F, kmul, vocab;
+  float eps;
+  int32_t B, L, H, dk;
+  int32_t c0, c1, stage;
+  const void* in; const float* w; const float* b; const float* k; const float* v; const uint8_t* key_mask;
+  void* out; float* out32; float* out_v;
+} ezb_test_cond_args;
+int ezb_test_cond(int device, const ezb_test_cond_args* args, void* stream);
 /* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7 / 8: that
    generation forced (8 takes dh 64 or 72 only); +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,

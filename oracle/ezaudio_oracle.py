@@ -72,7 +72,8 @@ def rope(q, k, inv_freq):
 
 def attention(x, sd: SD, p: str, H: int, context=None, context_mask=None, use_rope=False):
     """src/models/utils/attention.py:122-150 (Attention.forward), qk_norm='layernorm',
-    SDPA math restated: softmax(q k^T / sqrt(dh) masked with -inf on ~key_mask) v."""
+    SDPA math restated: softmax(q k^T / sqrt(dh) masked with -inf on ~key_mask) v; a query whose keys are all masked gets zeros, as
+    F.scaled_dot_product_attention with a boolean mask returns them."""
     B, L, C = x.shape
     ctx = x if context is None else context
     q = F.linear(x, sd[p + ".to_q.weight"])
@@ -89,6 +90,8 @@ def attention(x, sd: SD, p: str, H: int, context=None, context_mask=None, use_ro
     if context_mask is not None:  # attention.py:30-37,131-135: bool (B,1,L,Lc), True = keep
         s = s.masked_fill(~context_mask[:, None, None, :], float("-inf"))
     a = s.softmax(dim=-1)
+    if context_mask is not None:
+        a = a.masked_fill(~context_mask.any(-1)[:, None, None, None], 0.0)
     o = (a @ v).permute(0, 2, 1, 3).reshape(B, L, C)
     return linear(o, sd, p + ".proj")
 
