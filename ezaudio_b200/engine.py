@@ -1,4 +1,4 @@
-"""Continuous batching for text-to-audio and ControlNet: requests join a running batch at step boundaries.
+"""Continuous batching for text-to-audio, edits and ControlNet: requests join a running batch at step boundaries.
 
 `ContinuousEngine` keeps `slots` requests in flight in one padded, CFG-doubled batch (effective batch 2 * slots, clips padded to
 `max_length_s`).  Each denoising step is one replay of one captured CUDA graph: the CFG-doubling copy, the DiT forward with per-sample
@@ -12,11 +12,22 @@ holds the sorted union of the allowed schedules (with trailing spacing the 25- a
 request's audio does not depend on what it shares the batch with.  Requests have the semantics of `EzAudio.generate_audio` for one prompt
 (`frontend.Request`); the empty prompt "" runs without guidance, as it does there.
 
+The same engine serves edits (`frontend.EditRequest`), with the semantics of `EzAudio.editing_audio` for one clip, next to text-to-audio
+requests.  Every step passes the DiT a per-slot inpainting latent and a per-frame mask byte (rows k and slots + k for slot k): an edit's
+rows hold its crop's VAE latent and its mask (1 on the regenerated frames and past the crop's end), every other slot's rows hold zeros and
+an all-ones mask, which the DiT's input packing turns into exactly the operand it builds without an inpainting latent -- so text-to-audio
+audio is unchanged, and one graph serves every mix.  Admitting an edit peak-normalises and pads its clip on the device and encodes its crop
+alone (`Autoencoder(audio=)`, the scalar call's encode); finishing it pastes the kept frames of the latent back after the rescale, decodes
+the crop alone and splices it into the normalised clip.  The encode draws the VAE bottleneck noise from the global torch RNG when the edit
+is admitted (in queue order within a step), the draw editing_audio makes; text-to-audio admissions do not touch the global RNG.  So an
+edit's audio depends on its own arguments, its seed and the global RNG state at its admission, not on its co-tenants.
+
 Given an `api.EzAudio_ControlNet`, the engine serves `frontend.ControlRequest`s, with the semantics of `EzAudio_ControlNet.generate_audio`
 for one prompt and one reference clip: 10-s clips, each with its own reference audio, noise gate and conditioning scale besides the
 per-request constants above.  Admission also runs the clip's energy condition through the ControlNet stem once, into that slot's rows of
 the ControlNet's condition cache (`DiTControlNet.set_condition_rows`); each step runs the ControlNet with per-sample timestep rows and
-scales (`DiTControlNet.forward_step(t_index=, scale=)`) before the DiT.  Inpainting and the FP8 mode are not served.
+scales (`DiTControlNet.forward_step(t_index=, scale=)`) before the DiT.  A ControlNet engine serves no edits (the ControlNet API has no
+editing call).  The FP8 mode is not served.
 
 The host logic (admission, schedules, DDIM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots` (`ControlSlots`),
 which tests replace with a stub."""
@@ -33,7 +44,7 @@ import numpy as np
 import torch
 
 from . import _lib, post
-from .frontend import ControlRequest, Request
+from .frontend import ControlRequest, EditRequest, Request
 from .inference import scale_shift_re
 from .scheduler import DDIMScheduler
 
@@ -56,7 +67,7 @@ class SlotStep:
 @dataclasses.dataclass
 class _Active:
     ticket: int
-    req: object               # Request or ControlRequest
+    req: object               # Request, EditRequest or ControlRequest
     frames: int
     timesteps: List[int]
     sched: DDIMScheduler
@@ -65,10 +76,12 @@ class _Active:
 
 class ContinuousEngine:
     """Continuous-batching server for `ez` (an `api.EzAudio`, or an `api.EzAudio_ControlNet`): `submit` requests, then `step` / `stream` /
-    `run` them (see the module docstring).
+    `run` them (see the module docstring).  An EzAudio engine serves text-to-audio requests and edits in one queue; a ControlNet engine
+    serves ControlNet requests.
 
     slots: requests in flight (the denoiser runs 2 * slots samples; ez must have been built with max_batch >= slots).
-    max_length_s: the padded clip length (at most ez.max_length_s); longer requests are rejected.  ControlNet clips are 10 s.
+    max_length_s: the padded clip length (at most ez.max_length_s); longer requests, and edits whose crop is longer, are rejected.
+    ControlNet clips are 10 s.
     ddim_steps: the step counts requests may ask for; the union of their schedules must fit the timestep table."""
 
     def __init__(self, ez, slots: int = 4, max_length_s: float = 10.0, ddim_steps: Sequence[int] = (25, 50, 100), *, backend=None):
@@ -126,6 +139,22 @@ class ContinuousEngine:
         if (r.eta or 0) < 0:
             raise ValueError(f"eta must be >= 0, got {r.eta}")
 
+    def _read_clip(self, a, what: str) -> np.ndarray:
+        """A clip given as a path (read here, resampled to the model's rate) or as a float32 mono waveform; checked on the host."""
+        if isinstance(a, (str, os.PathLike)):
+            from .api import _load_audio
+            try:
+                a = _load_audio(os.fspath(a), self.backend.sr)
+            except (OSError, ValueError) as e:
+                raise ValueError(f"cannot read the {what} {a!r}: {e}") from e
+        elif isinstance(a, np.ndarray):
+            a = np.asarray(a, dtype=np.float32)
+        else:
+            raise ValueError(f"the {what} must be a path or a float32 mono waveform, got {type(a).__name__}")
+        if a.ndim != 1 or a.size < 1 or not np.isfinite(a).all():
+            raise ValueError(f"the {what} must be a non-empty, finite mono waveform, got shape {a.shape}")
+        return a
+
     def _control_wave(self, r: ControlRequest) -> np.ndarray:
         """Checks a ControlNet request and loads its reference clip (host only)."""
         self._check_common(r)
@@ -135,30 +164,43 @@ class ContinuousEngine:
                 raise ValueError(f"{name} must be a finite number, got {v!r}")
         if r.surpass_noise < 0:
             raise ValueError(f"surpass_noise must be >= 0, got {r.surpass_noise}")
-        a = r.audio
-        if isinstance(a, (str, os.PathLike)):
-            from .api import _load_audio
-            try:
-                a = _load_audio(os.fspath(a), self.backend.sr)
-            except (OSError, ValueError) as e:
-                raise ValueError(f"cannot read the reference clip {r.audio!r}: {e}") from e
-        elif isinstance(a, np.ndarray):
-            a = np.asarray(a, dtype=np.float32)
-        else:
-            raise ValueError(f"audio must be a path or a float32 mono waveform, got {type(a).__name__}")
-        if a.ndim != 1 or a.size < 1 or not np.isfinite(a).all():
-            raise ValueError(f"the reference clip must be a non-empty, finite mono waveform, got shape {a.shape}")
-        return a
+        return self._read_clip(r.audio, "reference clip")
+
+    def _edit(self, r: EditRequest) -> Tuple[int, Tuple[np.ndarray, dict]]:
+        """Checks an edit and loads its clip (host only); returns (crop frames, (clip, api.edit_plan of the edit))."""
+        from .api import edit_plan
+        self._check_common(r)
+        for name in ("mask_start", "mask_length", "boundary"):
+            v = getattr(r, name)
+            if not isinstance(v, numbers.Real) or isinstance(v, bool) or not math.isfinite(v):
+                raise ValueError(f"{name} must be a finite number of seconds, got {v!r}")
+        if r.mask_start < 0 or r.mask_length <= 0 or r.boundary < 0:
+            raise ValueError(f"mask_start and boundary must be >= 0 and mask_length > 0, got {r.mask_start}, {r.mask_length}, {r.boundary}")
+        wave = self._read_clip(r.gt_file, "clip to edit")
+        plan = edit_plan(len(wave), self.backend.sr, self.backend.latent_sr, self.backend.hop, r.boundary, r.mask_start, r.mask_length)
+        if not 1 <= plan["frames"] <= self.backend.max_frames:
+            raise ValueError(f"the edit's crop is {plan['frames']} frames; this engine serves 1..{self.backend.max_frames}")
+        return plan["frames"], (wave, plan)
 
     def submit(self, prompt: str, **kw) -> int:
-        """Queues a request (the keyword arguments of `frontend.Request`, or of `frontend.ControlRequest` for a ControlNet engine); returns
-        its ticket.  Invalid requests raise ValueError here, before any device work; a reference clip given as a path is read here."""
-        if self.control:
-            r = ControlRequest(prompt, **kw)
+        """Queues a request and returns its ticket: an edit (the keyword arguments of `frontend.EditRequest`) when `gt_file` is given,
+        otherwise a `frontend.Request`, or a `frontend.ControlRequest` for a ControlNet engine.  Invalid requests raise ValueError here,
+        before any device work; a clip given as a path is read here."""
+        if "gt_file" in kw:
+            return self._enqueue(EditRequest(prompt, **kw))
+        return self._enqueue(ControlRequest(prompt, **kw) if self.control else Request(prompt, **kw))
+
+    def _enqueue(self, r) -> int:
+        if isinstance(r, EditRequest):
+            if self.control:
+                raise ValueError("a ControlNet engine serves no edits (EzAudio_ControlNet has no editing call)")
+            item = (r,) + self._edit(r)
+        elif isinstance(r, ControlRequest) and self.control:
             item = (r, self.backend.max_frames, self._control_wave(r))
-        else:
-            r = Request(prompt, **kw)
+        elif isinstance(r, Request) and not self.control:
             item = (r, self._frames(r), None)
+        else:
+            raise ValueError(f"this {'ControlNet' if self.control else 'EzAudio'} engine does not serve {type(r).__name__}")
         t = self._tickets
         self._tickets += 1
         self._queue.append((t,) + item)
@@ -172,10 +214,12 @@ class ContinuousEngine:
     def _admit(self):
         for k in range(self.slots):
             if self._active[k] is None and self._queue:
-                t, r, frames, wave = self._queue.popleft()
+                t, r, frames, extra = self._queue.popleft()
                 seed = None if r.random_seed is None else int(r.random_seed)
                 if self.control:
-                    self.backend.admit(k, r.prompt, seed, frames, audio=wave, surpass_noise=float(r.surpass_noise))
+                    self.backend.admit(k, r.prompt, seed, frames, audio=extra, surpass_noise=float(r.surpass_noise))
+                elif isinstance(r, EditRequest):
+                    self.backend.admit(k, r.prompt, seed, frames, edit=extra)
                 else:
                     self.backend.admit(k, r.prompt, seed, frames)
                 n = int(r.ddim_steps)
@@ -209,18 +253,19 @@ class ContinuousEngine:
                 done.append((a.ticket, self.backend.sr, wav))
         return done
 
-    def stream(self, requests: Optional[Iterable[Request]] = None) -> Iterator[Tuple[int, int, object]]:
-        """Submits `requests` (if given) and yields (ticket, sample_rate, waveform) in completion order until nothing is queued or in flight."""
+    def stream(self, requests: Optional[Iterable[object]] = None) -> Iterator[Tuple[int, int, object]]:
+        """Submits `requests` (if given: Request / EditRequest objects, or ControlRequest objects for a ControlNet engine) and yields
+        (ticket, sample_rate, waveform) in completion order until nothing is queued or in flight."""
         if requests is not None:
             for r in requests:
-                self.submit(**dataclasses.asdict(r))
+                self._enqueue(r)
         while self.pending():
             yield from self.step()
 
-    def run(self, requests: Optional[Iterable[Request]] = None) -> List[Tuple[int, object]]:
+    def run(self, requests: Optional[Iterable[object]] = None) -> List[Tuple[int, object]]:
         """`requests` (default: the queued ones), in request order: result[i] = (sample_rate, waveform)."""
         if requests is not None:
-            tickets = [self.submit(**dataclasses.asdict(r)) for r in requests]
+            tickets = [self._enqueue(r) for r in requests]
         else:
             tickets = [q[0] for q in self._queue]
         pos = {t: i for i, t in enumerate(tickets)}
@@ -234,13 +279,17 @@ class ContinuousEngine:
 class CudaSlots:
     """Device side of ContinuousEngine: the slot buffers, the captured step graph and the per-slot generators of one `api.EzAudio`.
 
+    The inpainting rows (`gt` [2 * slots, C, L] fp32, `gt_mask` [2 * slots, L] uint8, rows k and slots + k for slot k) go to every step:
+    zeros and all ones for a free or text-to-audio slot, an edit's crop latent and mask while it is in flight (`admit(edit=)`); `finish`
+    pastes, decodes and splices an edit, and puts its rows back.
+
     Between steps the engine owns the denoiser's context and timestep table: a generate_audio call on the same EzAudio replaces them, and the
     next step restores them (set_context of the whole batch, set_timesteps of the table)."""
 
     def __init__(self, ez, slots: int, max_length_s: float, table: Sequence[int]):
         p = ez.params["autoencoder"]
         self.ez, self.unet, self.S, self.table = ez, ez.unet, int(slots), [int(t) for t in table]
-        self.sr, self.latent_sr = int(p["sr"]), int(p["latent_sr"])
+        self.sr, self.latent_sr, self.hop = int(p["sr"]), int(p["latent_sr"]), int(ez.autoencoder.decoder.hop)
         self.max_frames = int(round(max_length_s * self.latent_sr))
         desc = self.unet._h.desc
         self.max_timesteps = int(desc.max_timesteps)
@@ -259,6 +308,8 @@ class CudaSlots:
             d = dict(device=self.device, dtype=torch.float32)
             self.lat, self.noise = torch.zeros(S, C, L, **d), torch.zeros(S, C, L, **d)   # padded frames stay zero
             self.x_in, self.out = torch.zeros(Be, C, L, **d), torch.zeros(Be, C, L, **d)
+            self.gt = torch.zeros(Be, C, L, **d)
+            self.gt_mask = torch.ones(Be, L, device=self.device, dtype=torch.uint8)   # 1: the DiT regenerates the frame
             # per-step inputs as one int32 block, staged through pinned memory: t_index [Be] | lens [Be] | ezb_ddim_slot [S] (8 words each)
             words = 2 * Be + 8 * S
             self._h = torch.zeros(words, dtype=torch.int32, pin_memory=True)
@@ -270,6 +321,7 @@ class CudaSlots:
             self.ctx = uemb.to(**d).expand(Be, -1, -1).contiguous()
             self.cmask = umask.to(self.device).bool().expand(Be, -1).contiguous()
         self.gens: List[Optional[torch.Generator]] = [None] * S
+        self.edits: List[Optional[Tuple[torch.Tensor, int, int]]] = [None] * S   # an edit's (normalised clip, s0, n_paste)
         self.graph, self._key, self._launches = None, None, 0
         self.captures = 0   # step graphs captured so far
         self._ctx_epoch = None
@@ -282,8 +334,11 @@ class CudaSlots:
             self.unet.set_context(self.ctx, self.cmask)
             self._ctx_epoch = h.ctx_epoch
 
-    def admit(self, k: int, prompt: str, seed: Optional[int], frames: int):
+    def admit(self, k: int, prompt: str, seed: Optional[int], frames: int, edit: Optional[Tuple[np.ndarray, dict]] = None):
+        """Starts slot k.  `edit`: (clip, api.edit_plan of the edit) for an edit, whose crop is `frames` latent frames long."""
         with torch.cuda.device(self.device):
+            if edit is not None:
+                self._admit_edit(k, frames, *edit)
             self._own_denoiser()
             emb, mask = self.ez.encode_text([prompt])
             if tuple(emb.shape[1:]) != tuple(self.ctx.shape[1:]):
@@ -300,11 +355,28 @@ class CudaSlots:
             self.lat[k].zero_()
             self.lat[k, :, :frames] = torch.randn((1, self.C, frames), generator=g, device=self.device)[0]   # the draw of a solo run
 
+    def _admit_edit(self, k: int, frames: int, wave: np.ndarray, p: dict):
+        """editing_audio's preparation of one clip (api.py): normalise and pad the clip on the device, encode the crop alone -- the
+        bottleneck noise comes from the global RNG -- and write slot k's inpainting rows."""
+        clip = post.prepare_wave(torch.from_numpy(wave).to(self.device).unsqueeze(0), p["n_total"], normalize=True)[0]
+        z = self.ez.autoencoder(audio=clip[p["s0"]:p["s1"]].clone().view(1, 1, -1))
+        if tuple(z.shape) != (1, self.C, frames):
+            raise RuntimeError(f"the VAE encoded the crop to {tuple(z.shape)}, expected (1, {self.C}, {frames})")
+        S = self.S
+        self.gt[k].zero_()
+        self.gt[k, :, :frames] = z[0]
+        self.gt_mask[k].zero_()
+        self.gt_mask[k, p["m0"]:p["m1"]] = 1
+        self.gt_mask[k, frames:] = 1   # past the crop's end nothing of gt is used
+        self.gt[S + k].copy_(self.gt[k])
+        self.gt_mask[S + k].copy_(self.gt_mask[k])
+        self.edits[k] = (clip, int(p["s0"]), int(p["n_paste"]))
+
     def _launch_step(self):
         S = self.S
         self.x_in[:S].copy_(self.lat)
         self.x_in[S:].copy_(self.lat)
-        self.unet.forward_step(self.x_in, 0, out=self.out, lengths=self.lens, t_index=self.t_index)
+        self.unet.forward_step(self.x_in, 0, gt=self.gt, gt_mask_u8=self.gt_mask, out=self.out, lengths=self.lens, t_index=self.t_index)
         _lib.check(_lib.lib().ezb_cfg_ddim_step_slots(self.device.index, _lib.ptr(self.out), _lib.ptr(self.lat), _lib.ptr(self.noise),
                                                       _lib.ptr(self.slots_dev), S, self.C, self.max_frames, _lib.stream_ptr(),
                                                       _lib.ptr(self.lens[:S])))
@@ -353,14 +425,27 @@ class CudaSlots:
             self.lat.copy_(snap)   # capture does not execute; keep the eager result
 
     def finish(self, k: int, frames: int):
-        """Decodes slot k alone at its own length (as inference() does) and frees it; returns the float32 waveform (hop * frames,)."""
+        """Decodes slot k alone at its own length (as inference() does) and frees it; returns the float32 waveform (hop * frames,), or for
+        an edit the whole edited clip (n_total,), as editing_audio returns it."""
         with torch.cuda.device(self.device):
             p = self.ez.params["autoencoder"]
-            pred = scale_shift_re(self.lat[k:k + 1, :, :frames], p["scale"], p["shift"]).contiguous()
-            wav = self.ez.autoencoder(embedding=pred)
+            pred = scale_shift_re(self.lat[k:k + 1, :, :frames], p["scale"], p["shift"])
+            edit = self.edits[k]
+            if edit is not None:   # src/inference.py:104-105: the kept frames are the crop's latent, after the rescale
+                regen = self.gt_mask[k, :frames].bool().view(1, 1, frames)
+                pred = torch.where(regen, pred, self.gt[k:k + 1, :, :frames])
+            wav = self.ez.autoencoder(embedding=pred.contiguous())
             self.lat[k].zero_()
             self.gens[k] = None
-            return wav[0, 0].cpu().numpy()
+            if edit is None:
+                return wav[0, 0].cpu().numpy()
+            clip, s0, n = edit
+            post.splice_wave(clip, wav[0, 0], s0, n)
+            for row in (k, self.S + k):
+                self.gt[row].zero_()
+                self.gt_mask[row].fill_(1)
+            self.edits[k] = None
+            return clip.cpu().numpy()
 
 
 class ControlSlots(CudaSlots):

@@ -55,6 +55,23 @@ class ControlRequest:
     random_seed: Optional[int] = None
 
 
+@dataclasses.dataclass(frozen=True)
+class EditRequest:
+    """One edit (inpainting / outpainting): the arguments of `EzAudio.editing_audio` for one clip (defaults included).  `gt_file` is the
+    clip: a path, or a float32 mono waveform at the model's sample rate.  The result is the whole edited clip, as editing_audio returns it:
+    the normalised original with the regenerated span spliced in, extended to the mask's end when the mask runs past the clip."""
+    prompt: str
+    boundary: float
+    gt_file: object
+    mask_start: float
+    mask_length: float
+    guidance_scale: float = 3.5
+    guidance_rescale: float = 0
+    ddim_steps: int = 100
+    eta: float = 1
+    random_seed: Optional[int] = None
+
+
 def length_bucket_bin(length: float, length_bucket_s: float) -> int:
     """Bucket index of a clip length: ceil(length / bucket), so bucket k holds lengths in ((k - 1) * bucket, k * bucket]."""
     return max(1, math.ceil(length / length_bucket_s - 1e-9))
