@@ -6,8 +6,9 @@
 //                                      slot once its MMAs have completed, then park the finished 128 x BN fp32 tile in shared memory
 //                                      (over the ring, which is idle then); every consumer warp runs the fused epilogue on 32 rows
 //                                      (thread == row) of it.  The producer refills the ring for the next tile once the epilogue is done.
-//   An epilogue that works on the wgmma fragment itself (FRAG, the plain GEGLU: EpiGegluFrag) keeps the accumulator out of the ring instead:
-//   the producer streams the next tile's k-blocks while the MMA warpgroups run the epilogue from their registers and store through TMA.
+//   An epilogue that works on the wgmma fragment itself (FRAG: the plain GEGLU, EpiGegluFrag, and the plain Q/K/V heads, EpiHeadsFrag) keeps
+//   the accumulator out of the ring instead: the producer streams the next tile's k-blocks while the MMA warpgroups run the epilogue from
+//   their registers.
 //
 // A can also be addressed as an implicit-GEMM operand of a 1-D convolution over channels-last activations
 // [B, T, C]: k-block kb -> tap = kb / cin_blocks, rows shifted by (tap - center) * dilation with TMA zero fill at
@@ -548,8 +549,8 @@ struct EpiGegluFrag {
   static constexpr int STAGE_FLOATS = 32 * 32;          // 8 warps x 4 KB = two 16 KB output tiles
   static constexpr int HALF = 128;
   // d: this thread's m64n256 fragment of the warpgroup's rows m0 + 64 wg ..; tile: the warpgroup's 16 KB output tile (1024-byte aligned)
-  static __device__ __forceinline__ void frag(const Params& ep, const CUtensorMap* out, float (&d)[128], uint8_t* tile, int m0, int n0, int wg, int lg,
-                                              int lane) {
+  static __device__ __forceinline__ void frag(const Params& ep, const CUtensorMap* out, float (&d)[128], uint8_t* tile, int m0, int n0, const GemmShape&,
+                                              int wg, int lg, int lane) {
     const int q = lane & 3;
     const int r0 = 16 * lg + (lane >> 2);   // row of registers 4i, 4i + 1; registers 4i + 2, 4i + 3 hold row r0 + 8 (same swizzle phase)
     const float2* bh = reinterpret_cast<const float2*>(ep.bias + n0) + q;
@@ -1012,7 +1013,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-    if constexpr (SM::PRODUCER_WG) setmaxnreg_inc<SM::REGS_LAUNCH>();   // back to the launch split for whatever follows (gemm_ln_kernel's tail)
   } else {
     // ------------------------------------------------ consumers: wgmma mainloop (MMA warpgroups), accumulator -> smem, epilogue (all)
     if constexpr (SM::PRODUCER_WG) setmaxnreg_inc<SM::REGS_CONSUMER>();
@@ -1026,13 +1026,15 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
         EZB_DBG(const long long tm = clock64();)
-        float d[NSUB][SM::NH][SM::HN / 2];
+        // defined before the mainloop (whose first MMA ignores it) so that the previous tile's accumulator is not kept live through the
+        // epilogue as the operand of that first MMA: with it, the heads epilogue's dh-wide rows spilled
+        float d[NSUB][SM::NH][SM::HN / 2] = {};
         gemm_mainloop<BN, Epi, MC, KSUB>(d, wg * NSUB, sA, sB, full, empty, g.num_k_blocks, stage, phase);
         EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
         if ((threadIdx.x & 127) == 0) bulk_wait_group_read<0>();   // the previous tile's store has left this warpgroup's output tile
         warpgroup_bar_sync(wg);
         EZB_DBG(const long long te = clock64(); w1 += te - ta;)
-        Epi::frag(ep, tmC, d[0][0], tile_buf, mt * GEMM_BM, nt * BN, wg, lg, lane);
+        Epi::frag(ep, tmC, d[0][0], tile_buf, mt * GEMM_BM, nt * BN, g, wg, lg, lane);
         EZB_DBG(w4 += clock64() - te;)
       }
       if ((threadIdx.x & 127) == 0) bulk_wait_group<0>();
@@ -1074,6 +1076,11 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     }
   })
   __syncthreads();
+  // The producer warpgroup takes its registers back (the launch split, for whatever follows: gemm_ln_kernel's tail) only once every consumer
+  // warp has given its extra ones back: setmaxnreg allocates per warp from the CTA's pool, so a producer-warpgroup warp that asked earlier
+  // (its idle warps reach this point at once) could take registers a consumer warp's setmaxnreg.inc is still waiting for, and both would wait
+  // for ever.
+  if constexpr (SM::PRODUCER_WG) if (warp >= PRODUCER) setmaxnreg_inc<SM::REGS_LAUNCH>();
   if (MC > 1) cluster_sync_all();  // nobody leaves while a peer may still multicast into this CTA or arrive on its barriers
   if (FIRST_PHASE) {
     if (warp == PRODUCER && lane == 0) {
@@ -1133,6 +1140,74 @@ struct EpiHeadsParams {
   FoldIn fin;                  // LayerNorm (+ AdaLN modulate) of the block input folded into this projection
 };
 
+// The per-row steps of the heads epilogue, shared by the parked-tile (EpiHeads) and register-fragment (EpiHeadsFrag) schedules so that both
+// run the same float operations in the same order.  Head hh of the N-tile at n0 -> section (q / k / v of the reference column order) and head
+// index; false: the tile's pair slot hh lies past N.
+constexpr int heads_bn(int dh, int hpt) { return hpt == 3 ? (dh == 72 ? 224 : 3 * dh) : 2 * dh; }
+template <int DH, int HPT>
+__device__ __forceinline__ bool head_of_tile(const EpiHeadsParams& ep, int n0, int hh, int N, int& sec, int& head) {
+  if (HPT == 3) {
+    const int g = (n0 / heads_bn(DH, HPT)) * 3 + hh;   // global head index in [q heads | k heads | v heads]
+    sec = g / ep.H;
+    head = g - sec * ep.H;
+    return true;
+  }
+  const int n = n0 + hh * DH;
+  if (n >= N) return false;
+  sec = n / ep.D;
+  head = (n - sec * ep.D) / DH;
+  return true;
+}
+// LayerNorm(dh) with the affine of `kind` (0 q, 1 k), then rotate-half RoPE at position l, in place on one token row of one head.
+template <int DH, bool DBG>
+__device__ __forceinline__ void head_ln_rope(const EpiHeadsParams& ep, float (&v)[DH], int kind, int l) {
+  float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < DH; ++i) { s1[i & 3] += v[i]; s2[i & 3] = fmaf(v[i], v[i], s2[i & 3]); }
+  const float mean = ((s1[0] + s1[1]) + (s1[2] + s1[3])) * (1.0f / DH);
+  const float var = fmaxf(((s2[0] + s2[1]) + (s2[2] + s2[3])) * (1.0f / DH) - mean * mean, 0.f);
+  const float rstd = rsqrtf(var + 1e-5f);
+  const float nmr = -mean * rstd;
+  if (DBG && (ep.dbg & 2)) {
+  } else if (kind == 0) {
+#pragma unroll
+    for (int i = 0; i < DH; ++i) v[i] = fmaf(fmaf(v[i], rstd, nmr), ep.nw[0][i], ep.nb[0][i]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < DH; ++i) v[i] = fmaf(fmaf(v[i], rstd, nmr), ep.nw[1][i], ep.nb[1][i]);
+  }
+  if (ep.rope != nullptr && ((ep.rope_kinds >> kind) & 1) && !(DBG && (ep.dbg & 1))) {
+    const float2* cs = ep.rope + (size_t)l * (DH / 2);
+    const float lf = (float)l;
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) {
+      float2 c;
+      if (ep.rope_mufu) __sincosf(lf * ep.inv_freq[i], &c.y, &c.x);
+      else c = __ldg(cs + i);
+      const float a = v[i], bq = v[i + DH / 2];
+      v[i] = a * c.x - bq * c.y;
+      v[i + DH / 2] = bq * c.x + a * c.y;
+    }
+  }
+}
+// q / k row bh * L + l as dh bf16 with 16-byte stores (out[kind] 16-byte aligned, ld_qk a multiple of 8)
+template <int DH>
+__device__ __forceinline__ void head_store_row(const EpiHeadsParams& ep, const float (&v)[DH], int kind, size_t bh, int l) {
+  uint4* dst = reinterpret_cast<uint4*>(ep.out[kind] + (bh * ep.L + l) * (size_t)ep.ld_qk);
+#pragma unroll
+  for (int g = 0; g < DH / 8; ++g)
+    dst[g] = make_uint4(pack_bf16(v[8 * g], v[8 * g + 1]), pack_bf16(v[8 * g + 2], v[8 * g + 3]), pack_bf16(v[8 * g + 4], v[8 * g + 5]),
+                        pack_bf16(v[8 * g + 6], v[8 * g + 7]));
+}
+// V^T column l of head bh: dh values, then zeros up to dvp
+template <int DH>
+__device__ __forceinline__ void head_store_vt(const EpiHeadsParams& ep, const float (&v)[DH], size_t bh, int l) {
+  __nv_bfloat16* dst = ep.out[2] + bh * ep.dvp * ep.Lpad + l;
+#pragma unroll
+  for (int i = 0; i < DH; ++i) { *dst = __float2bfloat16_rn(v[i]); dst += ep.Lpad; }
+  for (int i = DH; i < ep.dvp; ++i) { *dst = __float2bfloat16_rn(0.f); dst += ep.Lpad; }
+}
+
 // HPT = 2: tile = two adjacent heads of the reference column order (N-tile 2*dh).  HPT = 3: the packed QKV layout -- the
 // 3H heads of [q | k | v] are regrouped three per tile (N-tile 224 for dh = 72: 3 x 72 + 8 zero columns; 192 for dh = 64), which
 // makes the tile wide enough for the tensor pipe (narrow tiles are operand-bandwidth bound).
@@ -1146,7 +1221,7 @@ struct EpiHeadsParams {
 template <int DH, int HPT = 2, bool DIRECT = false, bool FOLD = false, bool DBG = false>
 struct EpiHeads {
   using Params = EpiHeadsParams;
-  static constexpr int BN = HPT == 3 ? (DH == 72 ? 224 : 3 * DH) : 2 * DH;
+  static constexpr int BN = heads_bn(DH, HPT);
   static constexpr int EPI_WARPS = 8;
   static constexpr bool WIDE_REGS = HPT == 3;
   static constexpr int STAGE_FLOATS = DIRECT ? 0 : EPI_STAGE_FLOATS;
@@ -1163,16 +1238,7 @@ struct EpiHeads {
 #pragma unroll 1
     for (int hh = threadIdx.x >> 7; hh < HPT; hh += 2) {   // gemm_body's consumer warp 4 wg + (32-row group): heads wg, wg + 2
       int sec, head;
-      if (HPT == 3) {
-        const int g = (n0 / BN) * 3 + hh;     // global head index in [q heads | k heads | v heads]
-        sec = g / ep.H;
-        head = g - sec * ep.H;
-      } else {
-        const int n = n0 + hh * DH;
-        if (n >= N) break;
-        sec = n / ep.D;
-        head = (n - sec * ep.D) / DH;
-      }
+      if (!head_of_tile<DH, HPT>(ep, n0, hh, N, sec, head)) break;
       const int kind = ep.kind[sec];
       uint32_t r[DH];
       __syncwarp();
@@ -1195,42 +1261,9 @@ struct EpiHeads {
       }
       const size_t bh = (size_t)b * ep.H + head;
       if (kind < 2) {
-        float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < DH; ++i) { s1[i & 3] += v[i]; s2[i & 3] = fmaf(v[i], v[i], s2[i & 3]); }
-        const float mean = ((s1[0] + s1[1]) + (s1[2] + s1[3])) * (1.0f / DH);
-        const float var = fmaxf(((s2[0] + s2[1]) + (s2[2] + s2[3])) * (1.0f / DH) - mean * mean, 0.f);
-        const float rstd = rsqrtf(var + 1e-5f);
-        const float nmr = -mean * rstd;
-        if (DBG && (ep.dbg & 2)) {
-        } else if (kind == 0) {
-#pragma unroll
-          for (int i = 0; i < DH; ++i) v[i] = fmaf(fmaf(v[i], rstd, nmr), ep.nw[0][i], ep.nb[0][i]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < DH; ++i) v[i] = fmaf(fmaf(v[i], rstd, nmr), ep.nw[1][i], ep.nb[1][i]);
-        }
-        if (ep.rope != nullptr && ((ep.rope_kinds >> kind) & 1) && !(DBG && (ep.dbg & 1))) {
-          const float2* cs = ep.rope + (size_t)l * (DH / 2);
-          const float lf = (float)l;
-#pragma unroll
-          for (int i = 0; i < DH / 2; ++i) {
-            float2 c;
-            if (ep.rope_mufu) __sincosf(lf * ep.inv_freq[i], &c.y, &c.x);
-            else c = __ldg(cs + i);
-            const float a = v[i], bq = v[i + DH / 2];
-            v[i] = a * c.x - bq * c.y;
-            v[i + DH / 2] = bq * c.x + a * c.y;
-          }
-        }
+        head_ln_rope<DH, DBG>(ep, v, kind, l);
         if constexpr (DIRECT) {
-          if (row_ok) {
-            uint4* dst = reinterpret_cast<uint4*>(ep.out[kind] + (bh * ep.L + l) * (size_t)ep.ld_qk);
-#pragma unroll
-            for (int g = 0; g < DH / 8; ++g)
-              dst[g] = make_uint4(pack_bf16(v[8 * g], v[8 * g + 1]), pack_bf16(v[8 * g + 2], v[8 * g + 3]), pack_bf16(v[8 * g + 4], v[8 * g + 5]),
-                                  pack_bf16(v[8 * g + 6], v[8 * g + 7]));
-          }
+          if (row_ok) head_store_row<DH>(ep, v, kind, bh, l);
           continue;
         }
         // bf16 pairs -> staging granules (4 bf16 each) -> coalesced row stores
@@ -1251,10 +1284,71 @@ struct EpiHeads {
           }
         }
       } else if (row_ok && !(DBG && (ep.dbg & 4))) {
-        __nv_bfloat16* dst = ep.out[2] + bh * ep.dvp * ep.Lpad + l;
+        head_store_vt<DH>(ep, v, bh, l);
+      }
+    }
+  }
+};
+
+// The heads epilogue of the plain bf16 path (no LayerNorm fold, no profiling) on the wgmma fragment, for gemm_body's overlapped schedule (FRAG):
+// the accumulator stays in the MMA warpgroups' registers, so the producer streams the next tile's k-blocks while this runs, and the ring gets
+// the shared memory the parked tile and the staging tiles took (4 stages of the 224-wide tile instead of 3).  Each MMA warpgroup moves one head
+// slice at a time (its 64 rows x dh fp32) from the fragment into its own shared-memory buffer; its first two warps take head hh, its last two
+// head hh + 1, one token row per thread, and run EpiHeads' per-row code on them with the direct q / k row stores (bit-identical to the staged
+// ones), so the outputs are the same bits.
+template <int DH, int HPT>
+struct EpiHeadsFrag {
+  using Params = EpiHeadsParams;
+  static constexpr bool FRAG = true;
+  static constexpr int BN = heads_bn(DH, HPT);
+  static constexpr int EPI_WARPS = 8;
+  static constexpr bool WIDE_REGS = true;              // the producer warpgroup's registers: dh-wide rows next to the fragment, spill-free
+  static constexpr int PITCH = DH + 4;                 // the thread == row 16-byte reads of 8 consecutive rows hit distinct banks
+  static constexpr int STAGE_FLOATS = 64 * PITCH / 4;  // a warpgroup's four warps share one 64-row head slice
+  static_assert(DH % 8 == 0, "head slices start on a fragment register quad");
+  // d: this thread's m64nBN fragment of the warpgroup's rows m0 + 64 wg ..; tile: the warpgroup's head-slice buffer.  Rows >= g.M are not stored.
+  static __device__ __forceinline__ void frag(const Params& ep, const CUtensorMap*, float (&d)[BN / 2], uint8_t* tile, int m0, int n0, const GemmShape& g,
+                                              int wg, int lg, int lane) {
+    float* buf = reinterpret_cast<float*>(tile);
+    const int t = threadIdx.x & 127, half = t >> 6;   // half: warps 0-1 or 2-3 of the warpgroup
+    const int row = m0 + 64 * wg + (t & 63);
+    const bool row_ok = row < g.M;
+    const int b = row_ok ? row / ep.L : 0, l = row_ok ? row - b * ep.L : 0;
+    float* w0 = buf + (16 * lg + (lane >> 2)) * PITCH + 2 * (lane & 3);   // fragment row r0 (registers 4i, 4i + 1); r0 + 8: 4i + 2, 4i + 3
+    const float4* rd = reinterpret_cast<const float4*>(buf + (t & 63) * PITCH);
 #pragma unroll
-        for (int i = 0; i < DH; ++i) { *dst = __float2bfloat16_rn(v[i]); dst += ep.Lpad; }
-        for (int i = DH; i < ep.dvp; ++i) { *dst = __float2bfloat16_rn(0.f); dst += ep.Lpad; }
+    for (int p = 0; p < HPT; p += 2) {
+      float v[DH];
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const int hh = p + s;
+        if (hh >= HPT) break;
+        if (hh > 0) warpgroup_bar_sync(wg);   // the buffer's previous head has been read (gemm_body's barrier covers the previous tile)
+#pragma unroll
+        for (int i = 0; i < DH / 8; ++i) {
+          const int j = 4 * (hh * DH / 8 + i);
+          *reinterpret_cast<float2*>(w0 + 8 * i) = make_float2(d[j], d[j + 1]);
+          *reinterpret_cast<float2*>(w0 + 8 * PITCH + 8 * i) = make_float2(d[j + 2], d[j + 3]);
+        }
+        warpgroup_bar_sync(wg);
+        if (half == s) {
+#pragma unroll
+          for (int i = 0; i < DH / 4; ++i) {
+            const float4 x = rd[i];
+            v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
+          }
+        }
+      }
+      const int hh = p + half;
+      int sec, head;
+      if (hh >= HPT || !head_of_tile<DH, HPT>(ep, n0, hh, g.N, sec, head)) continue;
+      const int kind = ep.kind[sec];
+      const size_t bh = (size_t)b * ep.H + head;
+      if (kind < 2) {
+        head_ln_rope<DH, false>(ep, v, kind, l);
+        if (row_ok) head_store_row<DH>(ep, v, kind, bh, l);
+      } else if (row_ok) {
+        head_store_vt<DH>(ep, v, bh, l);
       }
     }
   }

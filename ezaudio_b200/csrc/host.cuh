@@ -466,6 +466,19 @@ int resident_clusters2(Device& dev, Kern kern, int smem, int threads, int* n) {
   if (*n <= 0) return fail(EZB_ERR_CUDA, "no 2-CTA cluster of this GEMM fits on the device");
   return EZB_OK;
 }
+// Checks of the fragment epilogues' operands and the output map of those that store through TMA.  EpiGegluFrag stores bf16 [M, N / 2] in
+// {64 features, 64 rows} boxes; EpiHeadsFrag stores its rows itself (no map).
+inline int frag_out_map(Device& dev, const EpiGegluParams& ep, int M, int N, int BN, const CUtensorMap** tC) {
+  if (ep.split_stride != 0 || ep.fin.u != nullptr || N % BN)
+    return fail(EZB_ERR_ARG, "gemm2: the fragment GEGLU epilogue writes plain bf16 of whole %d-column tiles (N %d)", BN, N);
+  return dev.tmaps.get2d(ep.out_bf16, (uint64_t)N / 2, (uint64_t)M, (uint64_t)ep.ld16, 64, tC);
+}
+inline int frag_out_map(Device&, const EpiHeadsParams& ep, int, int N, int BN, const CUtensorMap** tC) {
+  *tC = nullptr;
+  if (ep.fin.u != nullptr || ep.dbg || N % BN)
+    return fail(EZB_ERR_ARG, "gemm2: the fragment heads epilogue has no fold or profiling variant and takes whole %d-column tiles (N %d)", BN, N);
+  return EZB_OK;
+}
 template <int BN, class Epi, int KSUB = 1>
 int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
           const typename Epi::Params& ep) {
@@ -482,14 +495,10 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
   const CUtensorMap *tA, *tB;
   EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, GEMM_BM, &tA));
   EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, McSub<BN>::ROWS, &tB));
-  // An epilogue on the register fragment (EpiGegluFrag, the overlapped schedule) stores bf16 [M, N / 2] through a tensor map of its output
+  // An epilogue on the register fragment (the overlapped schedule) may store through a tensor map of its output (frag_out_map)
   constexpr bool FRAG = GemmCfg<BN, Epi, KSUB>::FRAG;
   const CUtensorMap* tC = nullptr;
-  if constexpr (FRAG) {
-    if (ep.split_stride != 0 || ep.fin.u != nullptr || N % BN)
-      return fail(EZB_ERR_ARG, "gemm2: the fragment GEGLU epilogue writes plain bf16 of whole %d-column tiles (N %d)", BN, N);
-    EZB_TRY(dev.tmaps.get2d(ep.out_bf16, (uint64_t)N / 2, (uint64_t)M, (uint64_t)ep.ld16, 64, &tC));
-  }
+  if constexpr (FRAG) EZB_TRY(frag_out_map(dev, ep, M, N, BN, &tC));
   auto kern = [] {
     if constexpr (FRAG) return gemm_frag_kernel<BN, Epi>;
     else return gemm_wgmma_kernel<BN, Epi, 2, KSUB>;
@@ -514,7 +523,7 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
     gp.flops.push_back(2.0 * (double)M * (double)N * (double)g.num_k_blocks * GEMM_BK);
     EZB_CUDA(cudaEventRecord(e0, st));
   }
-  if constexpr (FRAG) EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, *tC, g, ep));
+  if constexpr (FRAG) EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, *(tC ? tC : tA), g, ep));   // tA: unused placeholder
   else EZB_TRY(launch_k(kern, dim3(ctas), dim3(GEMM_THREADS), smem, st, 2, *tA, *tB, g, ep));
   if (gp.on) EZB_CUDA(cudaEventRecord(e1, st));
   return EZB_OK;
@@ -658,10 +667,11 @@ int gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __
 // Kernel instantiations of the fused heads epilogue (gemm.cuh EpiHeads).  Dit::lin_heads picks one from the options and the ezb_test_heads
 // hook from its argument, and both launch through heads_gemm, so the kernel-level tests run exactly what the model dispatches.
 enum HeadsVariant {
-  HEADS_PACKED3 = 0,         // three heads per N-tile (W packed by pack_weight_kernel's h3 mode), shared-memory staged q / k stores
-  HEADS_PACKED3_DIRECT = 1,  // the same without staging (every thread stores its own q / k row)
+  HEADS_PACKED3 = 0,         // three heads per N-tile (W packed by pack_weight_kernel's h3 mode); without fold: the register-fragment schedule
+                             // (EpiHeadsFrag), with fold: parked tile, shared-memory staged q / k stores
+  HEADS_PACKED3_DIRECT = 1,  // parked tile without staging (every thread stores its own q / k row)
   HEADS_PACKED3_KSUB2 = 2,   // DIRECT with 128-deep ring slots (dh = 72, no fold)
-  HEADS_PAIR = 3,            // two heads per N-tile of the reference column order, 2-CTA clusters, staged stores
+  HEADS_PAIR = 3,            // two heads per N-tile of the reference column order, 2-CTA clusters; fragment schedule / staged as HEADS_PACKED3
   HEADS_PAIR_DIRECT = 4,
   HEADS_SINGLE = 5,          // two heads per N-tile on the single-CTA kernel, staged stores (no fold)
 };
@@ -681,6 +691,17 @@ inline int heads_gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, cons
   if (e.dbg) {   // profiling instantiation: parts of the epilogue removed
     if (variant != HEADS_PACKED3 || dh != 72 || fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: the profiling epilogue is packed-3, dh 72, unfolded");
     return gemm2<224, EpiHeads<72, 3, false, false, true>>(dev, st, A, D, W, D, M, H * 224, D, e);
+  }
+  // The plain packed-3 and pair kernels run on the register fragment (EpiHeadsFrag, the overlapped schedule; same bits as the parked tile).
+  // Its q / k rows go out as 16-byte stores, so outputs that are not 16-byte aligned keep the parked, staged epilogue.
+  const bool rows16 = (reinterpret_cast<uintptr_t>(e.out[0]) & 15) == 0 && (reinterpret_cast<uintptr_t>(e.out[1]) & 15) == 0 && e.ld_qk % 8 == 0;
+  if (!fo && rows16 && variant == HEADS_PACKED3) {
+    if (dh == 72) return gemm2<224, EpiHeadsFrag<72, 3>>(dev, st, A, D, W, D, M, H * 224, D, e);
+    return gemm2<192, EpiHeadsFrag<64, 3>>(dev, st, A, D, W, D, M, H * 192, D, e);
+  }
+  if (!fo && rows16 && variant == HEADS_PAIR && N % (2 * dh) == 0) {
+    if (dh == 72) return gemm2<144, EpiHeadsFrag<72, 2>>(dev, st, A, D, W, D, M, N, D, e);
+    return gemm2<128, EpiHeadsFrag<64, 2>>(dev, st, A, D, W, D, M, N, D, e);
   }
   switch (variant) {
     case HEADS_PACKED3_KSUB2:   // 128-deep slots (needs the staging-free epilogue)
