@@ -709,16 +709,15 @@ struct Dit {
                 int L, bf16* qo, bf16* ko, bf16* vto, int Lpad, const FoldIn* fin = nullptr) {
     if (opt_skip() & 4) return EZB_OK;
     EpiHeadsParams e = heads_params(N, kinds, nq, nk, rope, L, qo, ko, vto, Lpad, fin);
-    const bool direct = opt_heads_direct() != 0, fo = fin != nullptr;
+    const bool fo = fin != nullptr;
     int variant;
     if (qkv3_bn > 0 && N == 3 * D) {  // packed self-attention QKV: three heads per tile
-      if (dh == 72 && opt_heads_dbg() && !fo) { e.dbg = opt_heads_dbg(); variant = HEADS_PACKED3; }   // profiling instantiation
-      else if (dh == 72 && (opt_ksub2() & 2) && !fo) variant = HEADS_PACKED3_KSUB2;
-      else variant = direct ? HEADS_PACKED3_DIRECT : HEADS_PACKED3;
+      if (dh == 72 && opt_heads_dbg() && !fo) e.dbg = opt_heads_dbg();   // profiling instantiation
+      variant = HEADS_PACKED3;
     } else if (!pair || (opt_cq_single() && !fo && N == D && dh == 72)) {   // cross-Q as 256 single-CTA tiles of 128 x 144 (1.73 waves of half-size tiles)
       variant = HEADS_SINGLE;
     } else {
-      variant = direct ? HEADS_PAIR_DIRECT : HEADS_PAIR;
+      variant = HEADS_PAIR;
     }
     return heads_gemm(*dev, st, A, W, M, N, dh, variant, e);
   }
@@ -988,7 +987,6 @@ struct Dit {
       else if (fp8 && geglu_bn == 256) EZB_TRY((gemm2_fp8<256, EpiGeglu<256>>(*dev, st, act8, act8_s, w.mlp18, w.s_mlp1, M, 2 * inner, D, g)));
       else if (fp8) EZB_TRY((gemm2_fp8<128, EpiGeglu<128>>(*dev, st, act8, act8_s, w.mlp18, w.s_mlp1, M, 2 * inner, D, g)));   // inner % 128 != 0
       else if (geglu_bn == 256 && fc.on) EZB_TRY((gemm2<256, EpiGeglu<256, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
-      else if (geglu_bn == 256 && (opt_ksub2() & 1) && kmul == 1) EZB_TRY((gemm2<256, EpiGeglu<256>, 2>(*dev, st, act, D, w.mlp1, D, M, 2 * inner, D, g)));   // 128-deep slots
       else if (geglu_bn == 256) EZB_TRY(gemm2_geglu(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g));
       else if (fc.on) EZB_TRY((gemm<128, EpiGeglu<128, true>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));
       else EZB_TRY((gemm<128, EpiGeglu<128>>(*dev, st, act, kmul * D, w.mlp1, kmul * D, M, 2 * inner, kmul * D, g)));

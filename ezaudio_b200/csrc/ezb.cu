@@ -89,12 +89,12 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
     }
     return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm pair: bn=%d", bn);
   }
-  if (epi_kind == 12) {  // the MLP's GEGLU GEMM with 128-deep ring slots (option ksub2 bit 0)
-    if (cp || bn != 256) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm: 128-deep slots exist for the plain bn=256 cluster GEGLU only");
+  if (epi_kind == 12) {  // the parked-tile cluster GEGLU, which bf16x3 and outputs not 16-byte aligned run
+    if (cp || bn != 256) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm: the parked cluster GEGLU is the plain bn=256 kernel");
     EpiGegluParams p;
     memset(&p, 0, sizeof p);
     p.bias = e->bias; p.out_bf16 = reinterpret_cast<__nv_bfloat16*>(e->out_bf16); p.ld16 = e->ld16; p.split_stride = e->split_stride;
-    return gemm2<256, EpiGeglu<256>, 2>(dev, st, a, lda, w, ldw, M, N, K, p);
+    return gemm2<256, EpiGeglu<256>>(dev, st, a, lda, w, ldw, M, N, K, p);
   }
   if (epi_kind == 0) {
     EpiLinearParams p = to_epi(e);
@@ -113,7 +113,8 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
 
 __attribute__((visibility("default"))) int ezb_test_heads(int device, const void* A, const float* W, const ezb_test_heads_args* a, void* stream) {
   if (!A || !W || !a) return fail(EZB_ERR_ARG, "ezb_test_heads: null pointer");
-  const int B = a->B, L = a->L, D = a->D, H = a->H, dh = a->dh, nsec = a->nsec, variant = a->variant;
+  const int B = a->B, L = a->L, D = a->D, H = a->H, dh = a->dh, nsec = a->nsec;
+  const int variant = a->variant == 2 ? HEADS_PACKED3_PARKED : a->variant;   // 2: the retired 128-deep-slot id runs the parked packed-3 kernel
   if (dh != 64 && dh != 72) return fail(EZB_ERR_SHAPE, "ezb_test_heads: head dimension %d (64 or 72)", dh);
   if (H < 2 || H % 2) return fail(EZB_ERR_SHAPE, "ezb_test_heads: %d heads (a positive even count)", H);
   if (D != H * dh) return fail(EZB_ERR_SHAPE, "ezb_test_heads: D %d != H %d x dh %d", D, H, dh);
@@ -122,8 +123,8 @@ __attribute__((visibility("default"))) int ezb_test_heads(int device, const void
   if (a->ld_qk < dh || a->ld_qk % 8) return fail(EZB_ERR_SHAPE, "ezb_test_heads: q / k pitch %d (>= dh %d, a multiple of 8)", a->ld_qk, dh);
   if (a->Lpad < L) return fail(EZB_ERR_SHAPE, "ezb_test_heads: V^T pitch %d < L %d", a->Lpad, L);
   if (a->dvp < dh) return fail(EZB_ERR_SHAPE, "ezb_test_heads: V^T rows %d < dh %d", a->dvp, dh);
-  if (variant < HEADS_PACKED3 || variant > HEADS_SINGLE) return fail(EZB_ERR_ARG, "ezb_test_heads: variant %d", variant);
-  const bool packed = variant <= HEADS_PACKED3_KSUB2;
+  if (a->variant < HEADS_PACKED3 || a->variant > HEADS_SINGLE) return fail(EZB_ERR_ARG, "ezb_test_heads: variant %d", a->variant);
+  const bool packed = variant == HEADS_PACKED3 || variant == HEADS_PACKED3_PARKED;
   if (packed && nsec != 3) return fail(EZB_ERR_SHAPE, "ezb_test_heads: the packed-3 layout needs q, k and v sections");
   for (int s = 0; s < nsec; ++s) {
     const int kd = a->kinds[s];
@@ -214,7 +215,7 @@ __attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* 
   if (variant == 0) {
     rc = mlp_fused<EpiGeglu<256>, EpiLinearT<256>>(dev, st, a16, W1p, M, 2 * inner, D, g, m16, w2, D, inner, p, reinterpret_cast<GridBarrier*>(bar));
   } else {
-    rc = variant == 2 ? gemm2<256, EpiGeglu<256>, 2>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g) : gemm2_geglu(dev, st, a16, D, W1p, D, M, 2 * inner, D, g);
+    rc = variant == 2 ? gemm2<256, EpiGeglu<256>>(dev, st, a16, D, W1p, D, M, 2 * inner, D, g) : gemm2_geglu(dev, st, a16, D, W1p, D, M, 2 * inner, D, g);
     if (rc == EZB_OK) rc = gemm_swapped<EpiLinearT>(dev, st, m16, inner, w2, inner, M, D, inner, p);
   }
   EZB_CUDA(cudaFreeAsync(W1p, st));
@@ -843,7 +844,6 @@ EZB_API int ezb_set_option(const char* name, int value) {
   if (name && !strcmp(name, "heads_dbg")) { opt_heads_dbg() = value; return EZB_OK; }
   if (name && !strcmp(name, "mlp2_pair")) { opt_mlp2_pair() = value; return EZB_OK; }
   if (name && !strcmp(name, "cq_single")) { opt_cq_single() = value; return EZB_OK; }
-  if (name && !strcmp(name, "ksub2")) { opt_ksub2() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn6")) { opt_attn6() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn7")) { opt_attn7() = value; return EZB_OK; }
   if (name && !strcmp(name, "attn8")) { opt_attn8() = value; return EZB_OK; }
@@ -859,7 +859,6 @@ EZB_API int ezb_set_option(const char* name, int value) {
   if (name && !strcmp(name, "w_prefetch")) { opt_w_prefetch() = value; return EZB_OK; }
   if (name && !strcmp(name, "ln_variant")) { opt_ln_variant() = value; return EZB_OK; }
   if (name && !strcmp(name, "mlp_fused")) { opt_mlp_fused() = value; return EZB_OK; }
-  if (name && !strcmp(name, "heads_direct")) { opt_heads_direct() = value; return EZB_OK; }
   if (name && !strcmp(name, "dhp80")) { opt_dhp80() = value; return EZB_OK; }
   if (name && !strcmp(name, "ln_fold")) { opt_fold() = value; return EZB_OK; }
   if (name && !strcmp(name, "skip")) { opt_skip() = value; return EZB_OK; }

@@ -759,15 +759,11 @@ struct Fp8Scales {
 };
 
 // Shared-memory plan of one CTA: the STAGES-deep operand ring (which also holds the finished fp32 accumulator tile between the
-// mainloop and the epilogue of a tile), the epilogues' per-warp transpose tiles, the barriers.
-// KSUB: 64-wide k-blocks per ring slot.  KSUB = 2 gives 128-deep slots: half as many full / empty barrier round trips (and wgmma
-// commit / wait pairs) per k, with the same bytes in flight.
-template <int BN, class Epi, int KSUB = 1>
+// mainloop and the epilogue of a tile), the epilogues' per-warp transpose tiles, the barriers.  A ring slot holds one 64-wide k-block.
+template <int BN, class Epi>
 struct GemmCfg {
-  static constexpr int A_SUB = GEMM_BM * GEMM_BK * 2;
-  static constexpr int B_SUB = BN * GEMM_BK * 2;
-  static constexpr int A_BYTES = KSUB * A_SUB;
-  static constexpr int B_BYTES = KSUB * B_SUB;
+  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
+  static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int EPI_WARPS = Epi::EPI_WARPS;
   // Every consumer warpgroup issues wgmma over the full BN columns.  One warpgroup: both 64-row halves of the tile.  Two: one half each.
   static constexpr int MMA_WG = EPI_WARPS / 4;
@@ -804,11 +800,11 @@ struct GemmCfg {
 // One consumer warpgroup's k-loop over a tile: all BN accumulator columns of NSUB 64-row halves from 64-row block row64 (slot s is released
 // once wgmma.wait_group shows its MMAs complete, while slot s + 1's are in flight).  Returns with every MMA of this warpgroup complete.
 // FP8: the ring slots hold 128-element e4m3 k-blocks (the same 128-byte rows), issued as four k32 MMAs at the bf16 descriptor steps.
-template <int BN, class Epi, int MC, int KSUB, bool FP8 = false>
-__device__ __forceinline__ void gemm_mainloop(float (&d)[GemmCfg<BN, Epi, KSUB>::NSUB][GemmCfg<BN, Epi, KSUB>::NH][GemmCfg<BN, Epi, KSUB>::HN / 2],
+template <int BN, class Epi, int MC, bool FP8 = false>
+__device__ __forceinline__ void gemm_mainloop(float (&d)[GemmCfg<BN, Epi>::NSUB][GemmCfg<BN, Epi>::NH][GemmCfg<BN, Epi>::HN / 2],
                                               int row64, const uint8_t* sA, const uint8_t* sB, uint64_t* full, uint64_t* empty, int num_k_blocks,
                                               uint32_t& stage, uint32_t& phase) {
-  using SM = GemmCfg<BN, Epi, KSUB>;
+  using SM = GemmCfg<BN, Epi>;
   constexpr int NSUB = SM::NSUB, NH = SM::NH, HN = SM::HN;
   // One thread per warpgroup arrives on the slot's barrier in every CTA of the cluster, without a release fence: the slot's only readers
   // are this warpgroup's wgmma (async proxy), complete at the wgmma.wait_group before the release; its only writer is a producer's TMA
@@ -823,24 +819,19 @@ __device__ __forceinline__ void gemm_mainloop(float (&d)[GemmCfg<BN, Epi, KSUB>:
   };
   static_assert(HN <= 256 && HN % 8 == 0, "BN");   // HN % 8: the second half starts on a 1024-byte swizzle atom
   uint32_t prev = 0;
-  for (int kb = 0; kb < num_k_blocks; kb += KSUB) {
+  for (int kb = 0; kb < num_k_blocks; ++kb) {
     mbar_wait(&full[stage], phase);
     wgmma_fence();
-    const int nsub = num_k_blocks - kb < KSUB ? num_k_blocks - kb : KSUB;
+    const uint32_t a0 = smem_u32(sA + stage * SM::A_BYTES + row64 * 8192);
+    const uint32_t b0 = smem_u32(sB + stage * SM::B_BYTES);
 #pragma unroll
-    for (int sub = 0; sub < KSUB; ++sub) {
-      if (sub >= nsub) break;
-      const uint32_t a0 = smem_u32(sA + stage * SM::A_BYTES + sub * SM::A_SUB + row64 * 8192);
-      const uint32_t b0 = smem_u32(sB + stage * SM::B_BYTES + sub * SM::B_SUB);
+    for (int k = 0; k < GEMM_BK / 16; ++k) {
 #pragma unroll
-      for (int k = 0; k < GEMM_BK / 16; ++k) {
+      for (int s = 0; s < NSUB; ++s)
 #pragma unroll
-        for (int s = 0; s < NSUB; ++s)
-#pragma unroll
-          for (int h = 0; h < NH; ++h)
-            if constexpr (FP8) WgmmaE4m3<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | sub | k) != 0);
-            else Wgmma<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | sub | k) != 0);
-      }
+        for (int h = 0; h < NH; ++h)
+          if constexpr (FP8) WgmmaE4m3<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | k) != 0);
+          else Wgmma<HN>::mma(d[s][h], wgmma_desc_sw128(a0 + s * 8192) + 2 * k, wgmma_desc_sw128(b0 + h * HN * 128) + 2 * k, (kb | k) != 0);
     }
     wgmma_commit();
     if (kb > 0) { wgmma_wait<1>(); release(prev); }
@@ -858,14 +849,14 @@ __device__ __forceinline__ void gemm_mainloop(float (&d)[GemmCfg<BN, Epi, KSUB>:
 // Parked-tile schedule: the k-loop, then, after every warpgroup's MMAs have completed, the fragments written into the accumulator tile in
 // shared memory (over the ring).  FP8: the accumulator is dequantised with the scales of global rows m0 + .. (< M) and columns n0 + .. on its
 // way to shared memory.
-template <int BN, class Epi, int MC, int KSUB, bool FP8 = false>
+template <int BN, class Epi, int MC, bool FP8 = false>
 __device__ __forceinline__ void gemm_mma_part(int row64, const uint8_t* sA, const uint8_t* sB, float* sAcc, uint64_t* full, uint64_t* empty,
                                               int num_k_blocks, uint32_t& stage, uint32_t& phase, int lg, int lane, const Fp8Scales& fs = Fp8Scales{},
                                               int m0 = 0, int M = 0, int n0 = 0) {
-  using SM = GemmCfg<BN, Epi, KSUB>;
+  using SM = GemmCfg<BN, Epi>;
   constexpr int NSUB = SM::NSUB, NH = SM::NH, HN = SM::HN;
   float d[NSUB][NH][HN / 2];
-  gemm_mainloop<BN, Epi, MC, KSUB, FP8>(d, row64, sA, sB, full, empty, num_k_blocks, stage, phase);
+  gemm_mainloop<BN, Epi, MC, FP8>(d, row64, sA, sB, full, empty, num_k_blocks, stage, phase);
   named_bar_sync(1, 32 * SM::EPI_WARPS);   // every MMA of the tile has completed: the ring may now hold the accumulator
   // m64nN fragment: register 4i + {0,1} -> row 16 * (warp % 4) + lane / 4, columns 8i + 2 (lane % 4) + {0,1}; 4i + {2,3} -> row + 8
   if constexpr (FP8) {
@@ -915,10 +906,10 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, int KSUB = 1, bool FP8 = false>
+template <int BN, class Epi, int MC = 1, bool FIRST_PHASE = false, bool FP8 = false>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& g, const typename Epi::Params& ep, uint8_t* smem_raw,
                                           const Fp8Scales& fs = Fp8Scales{}, const CUtensorMap* tmC = nullptr) {
-  using SM = GemmCfg<BN, Epi, KSUB>;
+  using SM = GemmCfg<BN, Epi>;
   constexpr int KB_ELEMS = FP8 ? 2 * GEMM_BK : GEMM_BK;   // elements per 128-byte k-block row
   // BN > 256: two TMA boxes and two wgmma halves per warpgroup, single CTA, one 64-row half per MMA warpgroup (the 288-token swap-AB tile)
   static_assert(BN % 16 == 0 && BN >= 64 && (BN <= 256 || (BN <= 512 && BN % 32 == 0 && MC == 1 && SM::MMA_WG == 2)), "BN");
@@ -974,17 +965,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
       // `empty` alone (which counts the releases of every MMA warpgroup of the cluster before a slot is multicast into again).
       if (!SM::FRAG && !first) { mbar_wait(acc_free, af_phase); af_phase ^= 1; }
       first = false;
-      for (int kb0 = 0; kb0 < g.num_k_blocks; kb0 += KSUB) {
+      for (int kb = 0; kb < g.num_k_blocks; ++kb) {
         EZB_DBG(const long long tq = clock64();)
         mbar_wait(&empty[stage], phase ^ 1);
         EZB_DBG(w0 += clock64() - tq;)
-        const int nsub = g.num_k_blocks - kb0 < KSUB ? g.num_k_blocks - kb0 : KSUB;
         if (elect_one()) {
-          mbar_expect_tx(&full[stage], nsub * (SM::A_SUB + SM::B_SUB));
-          for (int sub = 0; sub < nsub; ++sub) {
-          const int kb = kb0 + sub;
-          uint8_t* dA = sA + stage * SM::A_BYTES + sub * SM::A_SUB;
-          uint8_t* dB = sB + stage * SM::B_BYTES + sub * SM::B_SUB;
+          mbar_expect_tx(&full[stage], SM::A_BYTES + SM::B_BYTES);
+          uint8_t* dA = sA + stage * SM::A_BYTES;
+          uint8_t* dB = sB + stage * SM::B_BYTES;
           if (g.taps == 0) {
             tma_load_2d(dA, &tmA, &full[stage], kb * KB_ELEMS, mt * GEMM_BM);
           } else {
@@ -1007,7 +995,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
             for (int j = (int)cluster_ctarank(); j < BN / SR; j += MC)
               tma_load_2d_mc(dB + j * SR * 128, &tmB, &full[stage], kb * KB_ELEMS, n0 + j * SR, MC_MASK);
           }
-          }
         }
         __syncwarp();
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -1021,7 +1008,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     if constexpr (SM::FRAG) {
       // Overlapped schedule: mainloop, then the epilogue on this warpgroup's registers, then straight into the next tile, whose first k-blocks
       // the producer has already loaded.  Counters: [0] mainloop, [1] wait for the output tile's previous store, [4] epilogue.
-      static_assert(!FP8 && !FIRST_PHASE && KSUB == 1, "FRAG: bf16 kernels of one phase (gemm_frag_kernel)");
+      static_assert(!FP8 && !FIRST_PHASE, "FRAG: bf16 kernels of one phase (gemm_frag_kernel)");
       uint8_t* tile_buf = reinterpret_cast<uint8_t*>(sStage) + wg * (SM::STAGE_BYTES / 2);
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
@@ -1029,7 +1016,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
         // defined before the mainloop (whose first MMA ignores it) so that the previous tile's accumulator is not kept live through the
         // epilogue as the operand of that first MMA: with it, the heads epilogue's dh-wide rows spilled
         float d[NSUB][SM::NH][SM::HN / 2] = {};
-        gemm_mainloop<BN, Epi, MC, KSUB>(d, wg * NSUB, sA, sB, full, empty, g.num_k_blocks, stage, phase);
+        gemm_mainloop<BN, Epi, MC>(d, wg * NSUB, sA, sB, full, empty, g.num_k_blocks, stage, phase);
         EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
         if ((threadIdx.x & 127) == 0) bulk_wait_group_read<0>();   // the previous tile's store has left this warpgroup's output tile
         warpgroup_bar_sync(wg);
@@ -1042,7 +1029,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile % g.num_m_tiles, nt = tile / g.num_m_tiles;
       EZB_DBG(const long long tm = clock64();)
-      gemm_mma_part<BN, Epi, MC, KSUB, FP8>(wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane, fs, mt * GEMM_BM, g.M, nt * BN);
+      gemm_mma_part<BN, Epi, MC, FP8>(wg * NSUB, sA, sB, sAcc, full, empty, g.num_k_blocks, stage, phase, lg, lane, fs, mt * GEMM_BM, g.M, nt * BN);
       EZB_DBG(const long long ta = clock64(); w0 += ta - tm;)
       named_bar_sync(1, 32 * EPI_WARPS);     // accumulator tile complete in shared memory
       EZB_DBG(const long long te = clock64(); w1 += te - ta;)
@@ -1090,12 +1077,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     __syncthreads();
   }
 }
-template <int BN, class Epi, int MC = 1, int KSUB = 1>
-__global__ void __launch_bounds__((GemmCfg<BN, Epi, KSUB>::THREADS), 1)
+template <int BN, class Epi, int MC = 1>
+__global__ void __launch_bounds__((GemmCfg<BN, Epi>::THREADS), 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g,
                   const typename Epi::Params ep) {
   extern __shared__ uint8_t smem_dyn[];
-  gemm_body<BN, Epi, MC, false, KSUB>(tmA, tmB, g, ep, smem_dyn);
+  gemm_body<BN, Epi, MC>(tmA, tmB, g, ep, smem_dyn);
 }
 // gemm_wgmma_kernel<BN, Epi, 2> for an epilogue on the register fragment (epi_frag): tmC is the map its output stores go through.
 template <int BN, class Epi>
@@ -1112,7 +1099,7 @@ __global__ void __launch_bounds__((GemmCfg<BN, Epi>::THREADS), 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape g, const typename Epi::Params ep,
                 const Fp8Scales fs) {
   extern __shared__ uint8_t smem_dyn[];
-  gemm_body<BN, Epi, 2, false, 1, true>(tmA, tmB, g, ep, smem_dyn, fs);
+  gemm_body<BN, Epi, 2, false, true>(tmA, tmB, g, ep, smem_dyn, fs);
 }
 
 }  // namespace ezb
@@ -1215,16 +1202,13 @@ __device__ __forceinline__ void head_store_vt(const EpiHeadsParams& ep, const fl
 // at HPT = 3 warpgroup 0 takes heads 0 and 2 and warpgroup 1 head 1 (12 head x row-group units on 8 warps take two rounds however they are
 // dealt).  The packed tile runs with the producer warpgroup's registers (GemmCfg::PRODUCER_WG): 112 accumulators per thread in the mainloop,
 // two dh-wide rows per thread in the epilogue.
-// DIRECT: every thread stores its own q / k row (dh bf16 = 128 or 144 contiguous bytes) with 16-byte stores instead of transposing it through a
-// per-warp 8 KB shared-memory tile.  The staging tiles of the 8 epilogue warps take 64 KB, which leaves the 128 x 224 QKV tile three 44 KB
-// pipeline stages; without them it gets five.
-template <int DH, int HPT = 2, bool DIRECT = false, bool FOLD = false, bool DBG = false>
+template <int DH, int HPT = 2, bool FOLD = false, bool DBG = false>
 struct EpiHeads {
   using Params = EpiHeadsParams;
   static constexpr int BN = heads_bn(DH, HPT);
   static constexpr int EPI_WARPS = 8;
   static constexpr bool WIDE_REGS = HPT == 3;
-  static constexpr int STAGE_FLOATS = DIRECT ? 0 : EPI_STAGE_FLOATS;
+  static constexpr int STAGE_FLOATS = EPI_STAGE_FLOATS;
   template <class Wait>
   static __device__ __forceinline__ void run(const Params& ep, float* st, const AccRows& ar, int row0, int nvalid, int n0, int N, int lane, int c_begin,
                                              int c_end, Wait wait) {
@@ -1262,10 +1246,6 @@ struct EpiHeads {
       const size_t bh = (size_t)b * ep.H + head;
       if (kind < 2) {
         head_ln_rope<DH, DBG>(ep, v, kind, l);
-        if constexpr (DIRECT) {
-          if (row_ok) head_store_row<DH>(ep, v, kind, bh, l);
-          continue;
-        }
         // bf16 pairs -> staging granules (4 bf16 each) -> coalesced row stores
 #pragma unroll
         for (int g = 0; g < DH / 4; ++g)
@@ -1294,8 +1274,8 @@ struct EpiHeads {
 // the accumulator stays in the MMA warpgroups' registers, so the producer streams the next tile's k-blocks while this runs, and the ring gets
 // the shared memory the parked tile and the staging tiles took (4 stages of the 224-wide tile instead of 3).  Each MMA warpgroup moves one head
 // slice at a time (its 64 rows x dh fp32) from the fragment into its own shared-memory buffer; its first two warps take head hh, its last two
-// head hh + 1, one token row per thread, and run EpiHeads' per-row code on them with the direct q / k row stores (bit-identical to the staged
-// ones), so the outputs are the same bits.
+// head hh + 1, one token row per thread, and run EpiHeads' per-row code on them; each thread stores its own q / k row with 16-byte stores
+// (head_store_row) where EpiHeads transposes it through the staging tile, so the outputs are the same bits.
 template <int DH, int HPT>
 struct EpiHeadsFrag {
   using Params = EpiHeadsParams;

@@ -249,22 +249,12 @@ inline int& opt_skip() {
   static int v = 0;
   return v;
 }
-inline int& opt_heads_direct() {   // EpiHeads without shared-memory staging (deeper TMA pipeline), see gemm.cuh
-  static int v = [] { const char* e = getenv("EZB_HEADS_DIRECT"); return e ? atoi(e) : 0; }();
-  return v;
-}
 inline int& opt_heads_dbg() {
   static int v = 0;
   return v;
 }
 inline int& opt_mlp2_pair() {   // MLP output projection (K = 4608) on the 2-CTA cluster kernel instead of the swap-AB kernel
   static int v = [] { const char* e = getenv("EZB_MLP2_PAIR"); return e ? atoi(e) : 0; }();
-  return v;
-}
-// 128-deep ring slots (gemm.cuh GemmCfg KSUB = 2): bit 0 GEGLU GEMM, bit 1 packed QKV GEMM (with the staging-free epilogue).  Off by default:
-// ptxas serialises the wgmma of the KSUB = 2 GEGLU instantiation (register pressure of the two-k-block slot at BN = 256).
-inline int& opt_ksub2() {
-  static int v = [] { const char* e = getenv("EZB_KSUB2"); return e ? atoi(e) : 0; }();
   return v;
 }
 inline int& opt_cq_single() {   // cross-attention Q projection on the single-CTA kernel (no cluster pairing) instead of 2-CTA clusters
@@ -479,7 +469,7 @@ inline int frag_out_map(Device&, const EpiHeadsParams& ep, int, int N, int BN, c
     return fail(EZB_ERR_ARG, "gemm2: the fragment heads epilogue has no fold or profiling variant and takes whole %d-column tiles (N %d)", BN, N);
   return EZB_OK;
 }
-template <int BN, class Epi, int KSUB = 1>
+template <int BN, class Epi>
 int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, int M, int N, int K,
           const typename Epi::Params& ep) {
   if (M <= 0 || N <= 0 || K <= 0) return fail(EZB_ERR_SHAPE, "gemm2: empty problem %d %d %d", M, N, K);
@@ -496,15 +486,15 @@ int gemm2(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const _
   EZB_TRY(dev.tmaps.get2d(A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, GEMM_BM, &tA));
   EZB_TRY(dev.tmaps.get2d(W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, McSub<BN>::ROWS, &tB));
   // An epilogue on the register fragment (the overlapped schedule) may store through a tensor map of its output (frag_out_map)
-  constexpr bool FRAG = GemmCfg<BN, Epi, KSUB>::FRAG;
+  constexpr bool FRAG = GemmCfg<BN, Epi>::FRAG;
   const CUtensorMap* tC = nullptr;
   if constexpr (FRAG) EZB_TRY(frag_out_map(dev, ep, M, N, BN, &tC));
   auto kern = [] {
     if constexpr (FRAG) return gemm_frag_kernel<BN, Epi>;
-    else return gemm_wgmma_kernel<BN, Epi, 2, KSUB>;
+    else return gemm_wgmma_kernel<BN, Epi, 2>;
   }();
-  constexpr int smem = GemmCfg<BN, Epi, KSUB>::BYTES;
-  constexpr int GEMM_THREADS = GemmCfg<BN, Epi, KSUB>::THREADS;
+  constexpr int smem = GemmCfg<BN, Epi>::BYTES;
+  constexpr int GEMM_THREADS = GemmCfg<BN, Epi>::THREADS;
   static int clusters[16] = {};
   if (!clusters[dev.id & 15]) {
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -666,61 +656,53 @@ int gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, int lda, const __
 
 // Kernel instantiations of the fused heads epilogue (gemm.cuh EpiHeads).  Dit::lin_heads picks one from the options and the ezb_test_heads
 // hook from its argument, and both launch through heads_gemm, so the kernel-level tests run exactly what the model dispatches.
+// The values are ezb_test_heads' variant ids (include/ezb200.h), which keep their numbers: 2 was the retired 128-deep-slot kernel.
 enum HeadsVariant {
-  HEADS_PACKED3 = 0,         // three heads per N-tile (W packed by pack_weight_kernel's h3 mode); without fold: the register-fragment schedule
-                             // (EpiHeadsFrag), with fold: parked tile, shared-memory staged q / k stores
-  HEADS_PACKED3_DIRECT = 1,  // parked tile without staging (every thread stores its own q / k row)
-  HEADS_PACKED3_KSUB2 = 2,   // DIRECT with 128-deep ring slots (dh = 72, no fold)
-  HEADS_PAIR = 3,            // two heads per N-tile of the reference column order, 2-CTA clusters; fragment schedule / staged as HEADS_PACKED3
-  HEADS_PAIR_DIRECT = 4,
-  HEADS_SINGLE = 5,          // two heads per N-tile on the single-CTA kernel, staged stores (no fold)
+  HEADS_PACKED3 = 0,          // three heads per N-tile (W packed by pack_weight_kernel's h3 mode) on the register-fragment schedule (EpiHeadsFrag)
+  HEADS_PACKED3_PARKED = 1,   // the same on the parked tile with shared-memory staged q / k stores (EpiHeads); the _PARKED ids are for the
+                              // test and benchmark hooks, the model reaches the parked tile through the cases heads_gemm lists below
+  HEADS_PAIR = 3,             // two heads per N-tile of the reference column order, 2-CTA clusters, register-fragment schedule
+  HEADS_PAIR_PARKED = 4,      // the same on the parked tile, staged stores
+  HEADS_SINGLE = 5,           // two heads per N-tile on the single-CTA kernel, staged stores (no fold)
 };
+// One heads kernel of DH, HPT: the register-fragment schedule, or the parked tile with or without the LayerNorm fold (e.fin.u).
+template <int DH, int HPT>
+int heads_gemm_at(Device& dev, cudaStream_t st, const __nv_bfloat16* A, const __nv_bfloat16* W, int M, int N, bool frag, const EpiHeadsParams& e) {
+  constexpr int BN = heads_bn(DH, HPT);
+  const int D = e.D, n = HPT == 3 ? e.H * BN : N;   // packed-3: H tiles of three heads
+  if (frag) return gemm2<BN, EpiHeadsFrag<DH, HPT>>(dev, st, A, D, W, D, M, n, D, e);
+  if (e.fin.u != nullptr) return gemm2<BN, EpiHeads<DH, HPT, true>>(dev, st, A, D, W, D, M, n, D, e);
+  return gemm2<BN, EpiHeads<DH, HPT>>(dev, st, A, D, W, D, M, n, D, e);
+}
 // A [M, D] bf16; W packed for the variant (packed-3: H * BN rows; otherwise N = sections * D rows).  The LayerNorm fold is on when e.fin.u
-// is set; e.dbg selects the profiling instantiation (packed-3, dh = 72, no fold).
+// is set; e.dbg selects the profiling instantiation (packed-3, dh = 72, no fold).  The fold, the profiling epilogue and q / k outputs that
+// are not 16-byte aligned (the fragment epilogue stores whole rows as 16-byte stores) take the parked tile whatever the variant.
 inline int heads_gemm(Device& dev, cudaStream_t st, const __nv_bfloat16* A, const __nv_bfloat16* W, int M, int N, int dh, int variant,
                       const EpiHeadsParams& e) {
   const int D = e.D, H = e.H;
   const bool fo = e.fin.u != nullptr;
-  const bool packed = variant == HEADS_PACKED3 || variant == HEADS_PACKED3_DIRECT || variant == HEADS_PACKED3_KSUB2;
-  const bool direct = variant == HEADS_PACKED3_DIRECT || variant == HEADS_PAIR_DIRECT;
+  const bool packed = variant == HEADS_PACKED3 || variant == HEADS_PACKED3_PARKED;
   if (dh != 72 && dh != 64) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: head dimension %d", dh);
   if (packed && N != 3 * D) return fail(EZB_ERR_SHAPE, "heads_gemm: the packed-3 layout holds q, k and v (N %d, D %d)", N, D);
-#define EZB_HEADS(BN_, DH_, HPT_, N_)                                                                                                          \
-  (fo ? (direct ? gemm2<BN_, EpiHeads<DH_, HPT_, true, true>>(dev, st, A, D, W, D, M, N_, D, e) : gemm2<BN_, EpiHeads<DH_, HPT_, false, true>>(dev, st, A, D, W, D, M, N_, D, e)) \
-      : (direct ? gemm2<BN_, EpiHeads<DH_, HPT_, true, false>>(dev, st, A, D, W, D, M, N_, D, e) : gemm2<BN_, EpiHeads<DH_, HPT_, false, false>>(dev, st, A, D, W, D, M, N_, D, e)))
   if (e.dbg) {   // profiling instantiation: parts of the epilogue removed
     if (variant != HEADS_PACKED3 || dh != 72 || fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: the profiling epilogue is packed-3, dh 72, unfolded");
-    return gemm2<224, EpiHeads<72, 3, false, false, true>>(dev, st, A, D, W, D, M, H * 224, D, e);
+    return gemm2<224, EpiHeads<72, 3, false, true>>(dev, st, A, D, W, D, M, H * 224, D, e);
   }
-  // The plain packed-3 and pair kernels run on the register fragment (EpiHeadsFrag, the overlapped schedule; same bits as the parked tile).
-  // Its q / k rows go out as 16-byte stores, so outputs that are not 16-byte aligned keep the parked, staged epilogue.
   const bool rows16 = (reinterpret_cast<uintptr_t>(e.out[0]) & 15) == 0 && (reinterpret_cast<uintptr_t>(e.out[1]) & 15) == 0 && e.ld_qk % 8 == 0;
-  if (!fo && rows16 && variant == HEADS_PACKED3) {
-    if (dh == 72) return gemm2<224, EpiHeadsFrag<72, 3>>(dev, st, A, D, W, D, M, H * 224, D, e);
-    return gemm2<192, EpiHeadsFrag<64, 3>>(dev, st, A, D, W, D, M, H * 192, D, e);
-  }
-  if (!fo && rows16 && variant == HEADS_PAIR && N % (2 * dh) == 0) {
-    if (dh == 72) return gemm2<144, EpiHeadsFrag<72, 2>>(dev, st, A, D, W, D, M, N, D, e);
-    return gemm2<128, EpiHeadsFrag<64, 2>>(dev, st, A, D, W, D, M, N, D, e);
-  }
+  const bool frag = !fo && rows16 && variant != HEADS_PACKED3_PARKED && variant != HEADS_PAIR_PARKED;
   switch (variant) {
-    case HEADS_PACKED3_KSUB2:   // 128-deep slots (needs the staging-free epilogue)
-      if (dh != 72 || fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: 128-deep slots exist for dh 72 without fold only");
-      return gemm2<224, EpiHeads<72, 3, true, false>, 2>(dev, st, A, D, W, D, M, H * 224, D, e);
     case HEADS_PACKED3:
-    case HEADS_PACKED3_DIRECT:
-      if (dh == 72) return EZB_HEADS(224, 72, 3, H * 224);
-      return EZB_HEADS(192, 64, 3, H * 192);
+    case HEADS_PACKED3_PARKED:
+      return dh == 72 ? heads_gemm_at<72, 3>(dev, st, A, W, M, N, frag, e) : heads_gemm_at<64, 3>(dev, st, A, W, M, N, frag, e);
     case HEADS_PAIR:
-    case HEADS_PAIR_DIRECT:
-      if (dh == 72) return EZB_HEADS(144, 72, 2, N);
-      return EZB_HEADS(128, 64, 2, N);
+    case HEADS_PAIR_PARKED:
+      return dh == 72 ? heads_gemm_at<72, 2>(dev, st, A, W, M, N, frag && N % (2 * dh) == 0, e)
+                      : heads_gemm_at<64, 2>(dev, st, A, W, M, N, frag && N % (2 * dh) == 0, e);
     case HEADS_SINGLE:
       if (fo) return fail(EZB_ERR_UNSUPPORTED, "heads_gemm: the single-CTA heads kernel has no fold");
       if (dh == 72) return gemm<144, EpiHeads<72>>(dev, st, A, D, W, D, M, N, D, e);
       return gemm<128, EpiHeads<64>>(dev, st, A, D, W, D, M, N, D, e);
   }
-#undef EZB_HEADS
   return fail(EZB_ERR_ARG, "heads_gemm: variant %d", variant);
 }
 // FP8 mode's packed self-attention QKV: the one kernel it runs (three heads per N-tile, staged q / k stores, no fold).  A [M, D] e4m3 with row

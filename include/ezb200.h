@@ -223,7 +223,7 @@ typedef struct {
   void* fout_st; int32_t fout_ld_st; void* fout_a0; int32_t fout_ld0; const float* fout_g0; void* fout_a1; int32_t fout_ld1; const float* fout_g1;
 } ezb_test_epilogue;
 /* C = A[M,K] W[N,K]^T through the wgmma GEMM; epi_kind 0 = linear epilogue, 1 = GEGLU (packed W); 10 / 11 = the same on 2-CTA
-   clusters; 12 = the cluster GEGLU with 128-deep ring slots (two 64-wide k-blocks per slot); 20 = swap-AB as the model dispatches it
+   clusters (11: the GEGLU kernel the model dispatches); 12 = the parked-tile cluster GEGLU; 20 = swap-AB as the model dispatches it
    (token width chosen from the shape, fold epilogue when a fold is set); 21 = the same with the token width bn (256 or 288).
    conv_* = 0 for plain. */
 int ezb_test_gemm(int device, const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K, int bn, int epi_kind,
@@ -247,8 +247,9 @@ typedef struct {
      in the packed output-column order (packed-3: H * N-tile entries, 0 in the pad columns) */
   const void* fold_st; int32_t fold_slots, fold_ld_st;
   const float* fold_u; const float* fold_v;
-  /* 0 / 1 / 2: three heads per N-tile with staged / direct q, k stores / direct with 128-deep ring slots (nsec 3);
-     3 / 4: two heads per N-tile on 2-CTA clusters, staged / direct; 5: two heads per N-tile on the single-CTA kernel */
+  /* 0 / 1: three heads per N-tile (nsec 3) on the register-fragment schedule / on the parked tile with staged q, k stores (2: as 1);
+     3 / 4: two heads per N-tile on 2-CTA clusters, fragment / parked; 5: two heads per N-tile on the single-CTA kernel.  The fold and
+     q / k outputs that are not 16-byte aligned run the parked tile under every variant. */
   int32_t variant;
 } ezb_test_heads_args;
 int ezb_test_heads(int device, const void* A_bf16, const float* W_f32, const ezb_test_heads_args* args, void* stream);
@@ -256,7 +257,8 @@ int ezb_test_heads(int device, const void* A_bf16, const float* W_f32, const ezb
    Device pointers.  A [M, D] bf16; W1 [2*inner, D] and b1 [2*inner] fp32 in the reference layout ([hidden; gate] rows), packed by the
    library; W2 [D, inner] bf16; b2 [D]; x [M, D] fp32 updated in place; gate row stride gate_bstride; mid [M, inner] bf16 receives the GEGLU
    output; grid_barrier: two zeroed uint32 (count, generation), left with count 0.  variant 0: one persistent launch (GEGLU, grid barrier,
-   swap-AB output projection); 1: the same two GEMMs as two launches; 2: as 1 with 128-deep ring slots in the GEGLU GEMM. */
+   swap-AB output projection); 1: the same two GEMMs as two launches; 2: as 1 with the parked-tile GEGLU kernel (the one bf16x3 and
+   outputs without 16-byte alignment run). */
 int ezb_test_mlp(int device, const void* A_bf16, const float* W1_f32, const float* b1_f32, const void* W2_bf16, const float* b2, float* x,
                  const float* gate, int gate_bstride, int rows_per_batch, void* mid_bf16, void* grid_barrier, int M, int D, int inner,
                  int variant, void* stream);
@@ -375,7 +377,7 @@ int ezb_test_attention_lens(int device, const void* q, const void* k, const void
                             int L, int dh, int impl, void* stream);
 
 /* runtime switches for A/B measurements and profiling (csrc/host.cuh, csrc/ezb.cu list them): e.g. "pair_gemm" (1 = 2-CTA cluster tiles
-   sharing the weight tile, default), "attn6" / "attn7" / "attn8" / "attn_res" (attention variant), "ksub2", "ln_variant", "skip" (profiling: kernel classes not launched).  Products never need to call this. */
+   sharing the weight tile, default), "attn6" / "attn7" / "attn8" / "attn_res" (attention variant), "ln_variant", "skip" (profiling: kernel classes not launched).  Products never need to call this. */
 int ezb_set_option(const char* name, int value);
 /* incremented by every ezb_set_option call: hosts that cache captured CUDA graphs key them on it (options change kernel selection) */
 unsigned long long ezb_option_epoch(void);

@@ -14,15 +14,15 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ezaudio_b200 import _lib, api  # noqa: E402
 from ezaudio_b200.inference import _ddim_step  # noqa: E402
 
-DEFAULTS = {"attn7": 0, "w_prefetch": 0, "attn6": 5, "attn_pp": 0, "attn_res": 0, "attn_poly": 0, "cq_single": 0, "heads_direct": 0, "ksub2": 0, "mlp2_pair": 0, "swap_mc": 0,
+DEFAULTS = {"attn7": 0, "w_prefetch": 0, "attn6": 5, "attn_pp": 0, "attn_res": 0, "attn_poly": 0, "cq_single": 0, "mlp2_pair": 0, "swap_mc": 0,
             "mlp_fused": 0, "ln_variant": 2, "ln_tail": 0, "skip": 0}
 for a in sys.argv[1:]:
     if a.startswith("default:"):   # e.g. default:attn_res=1 changes the baseline every set is applied on top of
         k, v = a[8:].split("=")
         DEFAULTS[k] = int(v)
 SETS = [a for a in sys.argv[1:] if not a.startswith("default:")] or [
-    "", "attn_res=1", "attn_poly=1", "attn_res=1,attn_poly=1", "cq_single=1", "heads_direct=1,ksub2=3", "mlp2_pair=1", "swap_mc=1",
-    "mlp_fused=1", "ksub2=1", "",
+    "", "attn_res=1", "attn_poly=1", "attn_res=1,attn_poly=1", "cq_single=1", "mlp2_pair=1", "swap_mc=1",
+    "mlp_fused=1", "",
     "skip=1", "skip=2", "skip=4", "skip=8", "skip=16", "skip=31", ""]
 
 B, L = 4, 500

@@ -56,9 +56,8 @@ def run(M, N, K, bn, kind, label, resid=False, reps=20):
 
 
 # heads_gemm variants (csrc/host.cuh HeadsVariant)
-PACKED3, PACKED3_DIRECT, PACKED3_KSUB2, PAIR, PAIR_DIRECT, SINGLE = range(6)
-HEADS_NAMES = {PACKED3: "packed-3 staged", PACKED3_DIRECT: "packed-3 direct", PACKED3_KSUB2: "packed-3 direct ksub2", PAIR: "pair-2 staged",
-               PAIR_DIRECT: "pair-2 direct", SINGLE: "single-CTA"}
+PACKED3, PACKED3_PARKED, PAIR, PAIR_PARKED, SINGLE = 0, 1, 3, 4, 5
+HEADS_NAMES = {PACKED3: "packed-3", PACKED3_PARKED: "packed-3 parked", PAIR: "pair-2", PAIR_PARKED: "pair-2 parked", SINGLE: "single-CTA"}
 
 
 def heads(B, Lt, H, dh, nsec, variant, label, reps=20):
@@ -112,13 +111,13 @@ if MS is not None:
     if "linear" in SECTIONS:
         for M in MS:
             run(M, 9216, 1152, 256, 11, "pair geglu 256")
-            run(M, 9216, 1152, 256, 12, "pair geglu 256 ksub2")
+            run(M, 9216, 1152, 256, 12, "pair geglu 256 parked")
             run(M, 1152, 4608, 256, 20, "swapAB mlp2 resid+gate", resid=True)
             run(M, 1152, 4608, 128, 10, "pair mlp2 resid+gate 128", resid=True)
     if "heads" in SECTIONS:
         for M in MS:
             heads(M // 500, 500, 16, 72, 3, PACKED3, "XL self-QKV")
-            heads(M // 500, 500, 16, 72, 3, PACKED3_KSUB2, "XL self-QKV")
+            heads(M // 500, 500, 16, 72, 3, PACKED3_PARKED, "XL self-QKV")
             heads(M // 500, 500, 16, 72, 1, PAIR, "XL cross-Q")
             heads(M // 500, 500, 16, 72, 1, SINGLE, "XL cross-Q")
     SECTIONS = []
@@ -140,11 +139,11 @@ if "linear" in SECTIONS:
     run(8192, 8192, 8192, 128, 0, "1cta 8192^3 bf16 128", reps=5)
 if "heads" in SECTIONS:
     for B in (8, 16):   # XL self-attention QKV (Be = 8 / 16, L = 500)
-        for v in (PACKED3, PACKED3_DIRECT, PACKED3_KSUB2, PAIR, PAIR_DIRECT, SINGLE):
+        for v in (PACKED3, PACKED3_PARKED, PAIR, PAIR_PARKED, SINGLE):
             heads(B, 500, 16, 72, 3, v, "XL self-QKV")
-    for v in (PAIR, PAIR_DIRECT, SINGLE):
+    for v in (PAIR, PAIR_PARKED, SINGLE):
         heads(8, 500, 16, 72, 1, v, "XL cross-Q")
-    for v in (PACKED3, PACKED3_DIRECT, PAIR, PAIR_DIRECT, SINGLE):   # EzAudio-L: D = 1024, dh = 64
+    for v in (PACKED3, PACKED3_PARKED, PAIR, PAIR_PARKED, SINGLE):   # EzAudio-L: D = 1024, dh = 64
         heads(8, 500, 16, 64, 3, v, "L self-QKV")
-    for v in (PAIR, PAIR_DIRECT, SINGLE):
+    for v in (PAIR, PAIR_PARKED, SINGLE):
         heads(8, 500, 16, 64, 1, v, "L cross-Q")

@@ -35,8 +35,8 @@ gpu = pytest.mark.gpu
 EPS_ABS = 1e-4
 SENT = 0x7FAB   # a bf16 NaN pattern no epilogue produces
 
-# heads_gemm variants (csrc/host.cuh HeadsVariant)
-PACKED3, PACKED3_DIRECT, PACKED3_KSUB2, PAIR, PAIR_DIRECT, SINGLE = range(6)
+# heads_gemm variants (csrc/host.cuh HeadsVariant; 2 is the retired 128-deep-slot id)
+PACKED3, PACKED3_PARKED, PAIR, PAIR_PARKED, SINGLE = 0, 1, 3, 4, 5
 ROPE_NONE, ROPE_TABLE, ROPE_MUFU = 0, 1, 2
 
 
@@ -146,8 +146,8 @@ def _same_bits(a, b):
 
 
 # dh, H, B, L, ld_qk, RoPE.  H = 16: the XL shape (5 1/3 packed tiles per section, tiles straddle q / k / v); H = 2 / 4 at dh = 72: K = 144 /
-# 288, i.e. 3 / 5 64-wide k-blocks, the odd tail of the 128-deep slots.  M = 25 / 75 / 200: clips shorter than a 32-row group; M = 320: three
-# 128-row tiles (the cluster kernels' empty fourth tile); L = 1500: positions up to 1499.
+# 288, i.e. 3 / 5 64-wide k-blocks.  M = 25 / 75 / 200: clips shorter than a 32-row group; M = 320: three 128-row tiles (the cluster kernels'
+# empty fourth tile); L = 1500: positions up to 1499.
 SELF = [(72, 16, 2, 1500, 80, ROPE_MUFU), (72, 16, 2, 1500, 80, ROPE_TABLE), (72, 16, 1, 25, 128, ROPE_MUFU), (72, 2, 3, 130, 80, ROPE_TABLE),
         (72, 2, 8, 40, 128, ROPE_MUFU), (72, 4, 1, 500, 80, ROPE_TABLE), (72, 4, 3, 25, 80, ROPE_MUFU), (72, 2, 2, 1500, 128, ROPE_MUFU),
         (64, 4, 3, 130, 64, ROPE_TABLE), (64, 16, 2, 1500, 64, ROPE_MUFU), (64, 4, 8, 25, 64, ROPE_MUFU), (64, 16, 1, 40, 64, ROPE_TABLE)]
@@ -156,9 +156,9 @@ SELF = [(72, 16, 2, 1500, 80, ROPE_MUFU), (72, 16, 2, 1500, 80, ROPE_TABLE), (72
 @gpu
 @pytest.mark.parametrize("dh,H,B,L,ld_qk,rope", SELF)
 def test_self_attention_qkv_heads(dh, H, B, L, ld_qk, rope):
-    """nsec = 3 (q, k, v) with RoPE: every instantiation the model can dispatch for it.  Three heads per tile staged / direct / direct with
-    128-deep slots run the same MMAs in the same k order and the same epilogue arithmetic, so they must agree bit for bit; so must the
-    two-heads-per-tile cluster and single-CTA kernels."""
+    """nsec = 3 (q, k, v) with RoPE: every instantiation the model can dispatch for it.  Three heads per tile on the register fragment and on
+    the parked tile run the same MMAs in the same k order and the same epilogue arithmetic, so they must agree bit for bit; so must the
+    two-heads-per-tile cluster kernels on either schedule and the single-CTA kernel."""
     D, M, kinds = H * dh, B * L, (0, 1, 2)
     A, W, nq, nk, inv_freq = _inputs(dh * 1000 + H * 100 + L + B, M, D, 3, dh)
     kw = dict(B=B, L=L, H=H, dh=dh, kinds=kinds, rope=rope, nq=nq, nk=nk, inv_freq=inv_freq, ld_qk=ld_qk)
@@ -166,12 +166,10 @@ def test_self_attention_qkv_heads(dh, H, B, L, ld_qk, rope):
     refs = _reference(u, B=B, L=L, H=H, dh=dh, kinds=kinds, nq=nq, nk=nk, inv_freq=inv_freq, rope=rope)
     packed = _run(A, W, variant=PACKED3, **kw)
     excess = _check(packed, refs, B=B, L=L, H=H, dh=dh, tag=f"qkv dh{dh} H{H} B{B} L{L} ld{ld_qk} rope{rope} packed-3")
-    assert _same_bits(packed, _run(A, W, variant=PACKED3_DIRECT, **kw)), "packed-3 direct != staged"
-    if dh == 72:
-        assert _same_bits(packed, _run(A, W, variant=PACKED3_KSUB2, **kw)), "packed-3 KSUB = 2 != staged"
+    assert _same_bits(packed, _run(A, W, variant=PACKED3_PARKED, **kw)), "packed-3 fragment != parked"
     pair = _run(A, W, variant=PAIR, **kw)
     _check(pair, refs, B=B, L=L, H=H, dh=dh, tag=f"qkv dh{dh} H{H} B{B} L{L} ld{ld_qk} rope{rope} pair-2")
-    assert _same_bits(pair, _run(A, W, variant=PAIR_DIRECT, **kw)), "pair-2 direct != staged"
+    assert _same_bits(pair, _run(A, W, variant=PAIR_PARKED, **kw)), "pair-2 fragment != parked"
     assert _same_bits(pair, _run(A, W, variant=SINGLE, **kw)), "single-CTA != pair-2"
     if rope == ROPE_MUFU:   # on record: what __sincosf costs against the table at these angles
         trefs = _reference(u, B=B, L=L, H=H, dh=dh, kinds=kinds, nq=nq, nk=nk, inv_freq=inv_freq, rope=ROPE_TABLE)
@@ -191,7 +189,7 @@ def test_cross_attention_kv_cache_heads(dh, H, B, Lc):
     refs = _reference(A.double() @ W.bfloat16().double().t(), B=B, L=Lc, H=H, dh=dh, kinds=kinds, nq=None, nk=nk, inv_freq=None, rope=ROPE_NONE)
     pair = _run(A, W, variant=PAIR, **kw)
     _check(pair, refs, B=B, L=Lc, H=H, dh=dh, tag=f"ctx-kv dh{dh} H{H} B{B} Lc{Lc}")
-    assert _same_bits(pair, _run(A, W, variant=PAIR_DIRECT, **kw)), "pair-2 direct != staged"
+    assert _same_bits(pair, _run(A, W, variant=PAIR_PARKED, **kw)), "pair-2 fragment != parked"
     assert _same_bits(pair, _run(A, W, variant=SINGLE, **kw)), "single-CTA != pair-2"
 
 
@@ -206,7 +204,7 @@ def test_cross_attention_q_heads(dh, H, B, L):
     refs = _reference(A.double() @ W.bfloat16().double().t(), B=B, L=L, H=H, dh=dh, kinds=kinds, nq=nq, nk=None, inv_freq=None, rope=ROPE_NONE)
     pair = _run(A, W, variant=PAIR, **kw)
     _check(pair, refs, B=B, L=L, H=H, dh=dh, tag=f"cross-q dh{dh} H{H} B{B} L{L}")
-    assert _same_bits(pair, _run(A, W, variant=PAIR_DIRECT, **kw)), "pair-2 direct != staged"
+    assert _same_bits(pair, _run(A, W, variant=PAIR_PARKED, **kw)), "pair-2 fragment != parked"
     assert _same_bits(pair, _run(A, W, variant=SINGLE, **kw)), "single-CTA != pair-2"
 
 
@@ -255,13 +253,11 @@ def test_folded_layernorm_heads(dh, H, B, L, ld_qk, rope, nsec):
     kinds = (0, 1, 2) if nsec == 3 else (0,)
     _, W, nq, nk, inv_freq = _inputs(dh * 1000 + H * 100 + L + B + 11, M, D, nsec, dh)
     kw = dict(B=B, L=L, H=H, dh=dh, kinds=kinds, rope=rope, nq=nq, nk=nk if nsec == 3 else None, inv_freq=inv_freq, ld_qk=ld_qk)
-    variants = ((PACKED3, PACKED3_DIRECT), (PAIR, PAIR_DIRECT)) if nsec == 3 else ((PAIR, PAIR_DIRECT),)
-    for staged, direct in variants:
-        A, fold, uref = _fold_inputs(M + nsec, M, D, W, H, dh, nsec, staged == PACKED3)
+    for variant in ((PACKED3, PAIR) if nsec == 3 else (PAIR,)):
+        A, fold, uref = _fold_inputs(M + nsec, M, D, W, H, dh, nsec, variant == PACKED3)
         refs = _reference(uref, B=B, L=L, H=H, dh=dh, kinds=kinds, nq=nq, nk=nk, inv_freq=inv_freq, rope=rope)
-        out = _run(A, W, variant=staged, fold=fold, **kw)
-        _check(out, refs, B=B, L=L, H=H, dh=dh, tag=f"fold nsec{nsec} dh{dh} H{H} B{B} L{L} rope{rope} variant{staged}")
-        assert _same_bits(out, _run(A, W, variant=direct, fold=fold, **kw)), f"fold: direct != staged (variant {staged})"
+        out = _run(A, W, variant=variant, fold=fold, **kw)
+        _check(out, refs, B=B, L=L, H=H, dh=dh, tag=f"fold nsec{nsec} dh{dh} H{H} B{B} L{L} rope{rope} variant{variant}")
 
 
 def test_heads_hook_rejects_bad_arguments():
