@@ -57,6 +57,14 @@ class TestHeadsArgs(C.Structure):
                 ("fold_v", C.c_void_p), ("variant", C.c_int32)]
 
 
+class TestLinearArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("M", "N", "K", "kmul", "lda")] + [(n, C.c_void_p) for n in ("A", "W", "w_packed", "bias", "resid")] + \
+               [("ldr", C.c_int32), ("gate", C.c_void_p)] + [(n, C.c_int32) for n in ("gate_bstride", "rows_per_batch")] + \
+               [("out_f32", C.c_void_p), ("ld32", C.c_int32), ("out_bf16", C.c_void_p)] + [(n, C.c_int32) for n in ("ld16", "split", "act")] + \
+               [("out_scale", C.c_float), ("scale", C.c_void_p)] + [(n, C.c_int32) for n in ("kernel", "pair", "swap_ab", "m_select")] + \
+               [("ran", C.POINTER(C.c_int32))]
+
+
 class TestVaeArgs(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("kind", "precision", "B", "T", "cin", "cout", "taps", "dil", "stride")] + \
                [(n, C.c_void_p) for n in ("weight_v", "weight_g", "bias", "alpha", "beta", "x", "resid", "noise", "raw", "act", "out",
@@ -142,6 +150,7 @@ _SIGS = {
     "ezb_test_attention_lens": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_test_heads": ([_I, _VP, _VP, C.POINTER(TestHeadsArgs), _VP], _I),
     "ezb_test_mlp": ([_I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _I, _VP], _I),
+    "ezb_test_linear": ([_I, C.POINTER(TestLinearArgs), _VP], _I),
     "ezb_test_vae": ([_I, C.POINTER(TestVaeArgs), _VP], _I),
     "ezb_test_fp8": ([_I, C.POINTER(TestFp8Args), _VP], _I),
     "ezb_test_step": ([_I, C.POINTER(TestStepArgs), _VP], _I),

@@ -126,6 +126,16 @@ inline int timestep_embed_launch(cudaStream_t st, const float* t, float* out, in
   return EZB_OK;
 }
 
+// Does Dit::lin run this linear as swap-AB tiles (host.cuh gemm_swapped) rather than on the 128-wide N-tiles of EpiLinear?  Only fp32-output
+// layers without a uniform scale, in bf16 operands, on at least 512 tokens (m_select, 0: M) or with a folded LayerNorm; clips of fewer than 32
+// rows stay on EpiLinear, whose generic path looks up each row's gate.  Shared with the test hook ezb_test_linear.
+inline bool lin_takes_swap_ab(const EpiLinearParams& e, int M, int m_select, bool pair, bool swap_ab, int kmul) {
+  const bool folded = e.fin.u != nullptr || e.fout.st != nullptr;
+  const bool short_clips = e.gate != nullptr && e.rows_per_batch < 32;
+  return pair && swap_ab && kmul == 1 && e.out_bf16 == nullptr && e.out_f32 != nullptr && e.out_scale == 0.f && e.bias_mod == 0 && !short_clips &&
+         ((m_select ? m_select : M) >= 512 || folded);
+}
+
 struct FoldCtx {
   bool on = false;
   int t = 0;                  // timestep index (uniform over the batch)
@@ -641,9 +651,7 @@ struct Dit {
     if ((opt_skip() & 8) && e.out_f32 != nullptr && e.out_bf16 == nullptr) return EZB_OK;
     // fp32-output layers (residual / gated-residual / plain): swap-AB tiles of 128 features x 256 or 288 tokens (host.cuh swapped_bn)
     const bool folded = e.fin.u != nullptr || e.fout.st != nullptr;   // fold epilogues exist in the swap-AB kernel only
-    const bool short_clips = e.gate != nullptr && e.rows_per_batch < 32;  // per-token gate lookup lives in the generic (non swap-AB) epilogue
-    if (pair && swap_ab && kmul == 1 && e.out_bf16 == nullptr && e.out_f32 != nullptr && e.out_scale == 0.f && e.bias_mod == 0 && !short_clips &&
-        ((m_select ? m_select : M) >= 512 || folded)) {
+    if (lin_takes_swap_ab(e, M, m_select, pair, swap_ab, kmul)) {
       if (folded) return gemm_swapped<EpiLinearTF>(*dev, st, A, K, W, K, M, N, K, e);
       if (tail != nullptr && tail_done != nullptr && opt_ln_tail() && !(opt_skip() & 9))
         return gemm_swapped_ln<EpiLinearT>(*dev, st, A, K, W, K, M, N, K, e, *tail, grid_bar, tail_done);

@@ -111,6 +111,82 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
   return fail(EZB_ERR_UNSUPPORTED, "ezb_test_gemm: bn=%d epi=%d", bn, epi_kind);
 }
 
+}  // extern "C"
+
+namespace {
+bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+int test_linear_check(const ezb_test_linear_args* a) {
+  const int M = a->M, N = a->N, K = a->K, km = a->kmul;
+  if (!a->A || !a->W) return fail(EZB_ERR_ARG, "ezb_test_linear: null A or W");
+  if (!a->out_f32 && !a->out_bf16) return fail(EZB_ERR_ARG, "ezb_test_linear: no output");
+  if (km != 1 && km != 3) return fail(EZB_ERR_ARG, "ezb_test_linear: kmul %d (1 or 3)", km);
+  if (a->kernel < 0 || a->kernel > 4) return fail(EZB_ERR_ARG, "ezb_test_linear: kernel %d (0 to 4)", a->kernel);
+  if ((a->kernel == 1 || a->kernel == 2) && a->scale) return fail(EZB_ERR_ARG, "ezb_test_linear: kernel %d is EpiLinear, scale selects EpiLinearScaled", a->kernel);
+  if (a->kernel >= 3 && !a->scale) return fail(EZB_ERR_ARG, "ezb_test_linear: kernel %d (EpiLinearScaled) needs scale", a->kernel);
+  if (a->act != ACT_NONE && a->act != ACT_SILU) return fail(EZB_ERR_ARG, "ezb_test_linear: act %d (0 none, 1 SiLU)", a->act);
+  if (a->split && (km != 3 || !a->out_bf16)) return fail(EZB_ERR_ARG, "ezb_test_linear: the split bf16 output needs kmul 3 and out_bf16");
+  if (a->gate && !a->resid) return fail(EZB_ERR_ARG, "ezb_test_linear: a gate needs the residual it gates into");
+  if (a->scale && (a->resid || a->gate || a->out_bf16 || !a->out_f32 || a->out_scale != 0.f))
+    return fail(EZB_ERR_UNSUPPORTED, "ezb_test_linear: EpiLinearScaled reads bias and writes out_f32 only");
+  if (M < 1 || M > (1 << 24) || N < 8 || N % 8 || K < 8 || K % 8 || (long long)N * K > (1LL << 28))
+    return fail(EZB_ERR_SHAPE, "ezb_test_linear: M %d N %d K %d (N, K multiples of 8)", M, N, K);
+  if (a->lda < km * K || a->lda % 8) return fail(EZB_ERR_SHAPE, "ezb_test_linear: A pitch %d (>= %d, a multiple of 8)", a->lda, km * K);
+  if ((a->gate || a->scale) && a->rows_per_batch < 1) return fail(EZB_ERR_SHAPE, "ezb_test_linear: %d rows per clip", a->rows_per_batch);
+  // the epilogue reads and writes column pairs: fp32 as float2, bf16 as 4-byte pairs
+  if ((a->resid && (a->ldr < N || a->ldr % 2)) || (a->gate && (a->gate_bstride < 0 || a->gate_bstride % 2)) ||
+      (a->out_f32 && (a->ld32 < N || a->ld32 % 2)) || (a->out_bf16 && (a->ld16 < (a->split ? 3 * N : N) || a->ld16 % 2)))
+    return fail(EZB_ERR_SHAPE, "ezb_test_linear: row pitches ldr %d gate %d ld32 %d ld16 %d for N %d", a->ldr, a->gate_bstride, a->ld32, a->ld16, N);
+  if (!aligned(a->A, 16) || !aligned(a->resid, 8) || !aligned(a->gate, 8) || !aligned(a->out_f32, 8) || !aligned(a->out_bf16, 4) || !aligned(a->bias, 4))
+    return fail(EZB_ERR_ARG, "ezb_test_linear: A must be 16-byte aligned, resid / gate / out_f32 8-byte, out_bf16 and bias 4-byte");
+  return EZB_OK;
+}
+int test_linear_run(Device& dev, cudaStream_t st, const ezb_test_linear_args* a, int kernel, __nv_bfloat16* Wp) {
+  const int M = a->M, N = a->N, K = a->K, km = a->kmul;
+  pack_weight_kernel<<<(unsigned)(((size_t)N * K + 255) / 256), 256, 0, st>>>(a->W, N, K, Wp, K, km, 0, 0, 0, 0, 0, 0);
+  EZB_CUDA(cudaGetLastError());
+  if (a->w_packed) EZB_CUDA(cudaMemcpyAsync(a->w_packed, Wp, (size_t)N * km * K * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice, st));
+  const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(a->A);
+  EpiLinearParams e;
+  memset(&e, 0, sizeof e);
+  e.bias = a->bias; e.resid = a->resid; e.ldr = a->ldr; e.gate = a->gate; e.gate_bstride = a->gate_bstride; e.rows_per_batch = a->rows_per_batch;
+  e.out_f32 = a->out_f32; e.ld32 = a->ld32; e.out_bf16 = static_cast<__nv_bfloat16*>(a->out_bf16); e.ld16 = a->ld16;
+  e.split_stride = a->split ? N : 0; e.act = a->act; e.out_scale = a->out_scale;
+  const EpiLinearScaledParams es{e, a->scale, a->rows_per_batch};
+  if (kernel == 0) {   // Dit::lin, or the ControlNet trunk's zero-linears for per-sample scales
+    if (a->scale) kernel = a->pair ? 4 : 3;
+    else if (!lin_takes_swap_ab(e, M, a->m_select, a->pair != 0, a->swap_ab != 0, km)) kernel = a->pair ? 2 : 1;
+    else {
+      if (a->ran) *a->ran = swapped_bn(dev, M, N);
+      return opt_swap_mc() ? gemm_swapped_mc<EpiLinearT, 3>(dev, st, A, a->lda, Wp, K, M, N, K, e) : gemm_swapped<EpiLinearT>(dev, st, A, a->lda, Wp, K, M, N, K, e);
+    }
+  }
+  if (a->ran) *a->ran = kernel;
+  const int ldw = km * K;
+  switch (kernel) {
+    case 1: return gemm<128, EpiLinear<128>>(dev, st, A, a->lda, Wp, ldw, M, N, ldw, e);
+    case 2: return gemm2<128, EpiLinear<128>>(dev, st, A, a->lda, Wp, ldw, M, N, ldw, e);
+    case 3: return gemm<128, EpiLinearScaled<128>>(dev, st, A, a->lda, Wp, ldw, M, N, ldw, es);
+    default: return gemm2<128, EpiLinearScaled<128>>(dev, st, A, a->lda, Wp, ldw, M, N, ldw, es);
+  }
+}
+}  // namespace
+
+extern "C" {
+
+__attribute__((visibility("default"))) int ezb_test_linear(int device, const ezb_test_linear_args* a, void* stream) {
+  if (!a) return fail(EZB_ERR_ARG, "ezb_test_linear: null arguments");
+  EZB_TRY(test_linear_check(a));
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  dev.tmaps.trim();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  __nv_bfloat16* Wp = nullptr;
+  EZB_CUDA(cudaMallocAsync(&Wp, (size_t)a->N * a->kmul * a->K * sizeof(__nv_bfloat16), st));
+  const int rc = test_linear_run(dev, st, a, a->kernel, Wp);
+  EZB_CUDA(cudaFreeAsync(Wp, st));
+  return rc;
+}
+
 __attribute__((visibility("default"))) int ezb_test_heads(int device, const void* A, const float* W, const ezb_test_heads_args* a, void* stream) {
   if (!A || !W || !a) return fail(EZB_ERR_ARG, "ezb_test_heads: null pointer");
   const int B = a->B, L = a->L, D = a->D, H = a->H, dh = a->dh, nsec = a->nsec;

@@ -229,6 +229,34 @@ typedef struct {
 int ezb_test_gemm(int device, const void* A_bf16, int lda, const void* W_bf16, int ldw, int M, int N, int K, int bn, int epi_kind,
                   const ezb_test_epilogue* e, int conv_taps, int conv_center, int conv_dil, int conv_cin_pad, int conv_T,
                   int conv_B, void* stream);
+/* The DiT's linears on 128-wide N-tiles (csrc/gemm.cuh EpiLinear, EpiLinearScaled), launched as Dit::lin and the ControlNet zero-linears
+   launch them, from a reference-layout weight.  Device pointers unless noted.
+   W fp32 [N, K], packed by the library as Dit::init packs it into W' bf16 [N, kmul*K]: kmul 1 bf16(W); kmul 3 (bf16x3) [hi | hi | lo] with
+   hi = bf16(W), lo = bf16(W - hi).  w_packed (optional) receives W'.  A bf16 [M, kmul*K], row pitch lda >= kmul*K ([hi | lo | hi] in bf16x3).
+   Epilogue of EpiLinear, per row r and column c < N:  v = (A W'^T + bias)[r, c] * out_scale (out_scale 0 reads as 1; bias optional);
+   with resid (pitch ldr)  v = resid[r, c] + v, or with gate too  v = resid[r, c] + (1 - gate[b * gate_bstride + c]) v,  b = r / rows_per_batch;
+   out_f32 (pitch ld32) receives v; out_bf16 (pitch ld16) receives bf16(act(v)) (act 0 none, 1 SiLU), and when split (kmul 3 only) also the
+   remainder bf16(act(v) - hi) at column c + N and hi again at c + 2N.  scale, fp32 [B], selects EpiLinearScaled instead:
+   out_f32 = (A W'^T + bias) * scale[r / rows_per_batch] (bias and out_f32 only; a scale of 0 gives zeros).
+   kernel: 1 single-CTA gemm<128, EpiLinear<128>>; 2 2-CTA cluster gemm2<128, EpiLinear<128>>; 3 / 4 the same two with EpiLinearScaled (scale
+   set); 0 the kernel Dit::lin runs for these pair / swap_ab (the model's runtime switches), kmul, m_select (the token count the kernel is
+   chosen for, 0: M) and epilogue -- which can be the swap-AB kernel -- or, with scale, the one the ControlNet trunk runs for pair.
+   ran (optional HOST pointer) receives the kernel that ran: 1 to 4, or 256 / 288, the token width of the swap-AB tiles.
+   Every argument is checked before any device work. */
+typedef struct {
+  int32_t M, N, K, kmul, lda;
+  const void* A; const float* W; void* w_packed;
+  const float* bias;
+  const float* resid; int32_t ldr;
+  const float* gate; int32_t gate_bstride; int32_t rows_per_batch;
+  float* out_f32; int32_t ld32;
+  void* out_bf16; int32_t ld16; int32_t split; int32_t act;
+  float out_scale;
+  const float* scale;
+  int32_t kernel, pair, swap_ab, m_select;
+  int32_t* ran;
+} ezb_test_linear_args;
+int ezb_test_linear(int device, const ezb_test_linear_args* args, void* stream);
 /* Q/K/V-type projection with the fused per-head LayerNorm(dh) + RoPE + attention-layout epilogue (the fast mode's Q/K/V, cross-Q and
    cross-K/V GEMMs).  Device pointers.  A [B*L, D] bf16; W [nsec*D, D] fp32 in the reference layout (section s = rows s*D ..), packed and
    rounded to bf16 by the library as the model packs it.  Section s has kind kinds[s]: 0 q, 1 k (both LayerNorm(dh) -> optional RoPE at the
