@@ -46,7 +46,8 @@ class TestEpilogue(C.Structure):
                 ("split_stride", C.c_int32), ("act", C.c_int32), ("act_a", C.c_void_p), ("act_b", C.c_void_p),
                 ("fin_st", C.c_void_p), ("fin_slots", C.c_int32), ("fin_ld_st", C.c_int32), ("fin_inv_dim", C.c_float), ("fin_u", C.c_void_p),
                 ("fin_v", C.c_void_p), ("fout_st", C.c_void_p), ("fout_ld_st", C.c_int32), ("fout_a0", C.c_void_p), ("fout_ld0", C.c_int32),
-                ("fout_g0", C.c_void_p), ("fout_a1", C.c_void_p), ("fout_ld1", C.c_int32), ("fout_g1", C.c_void_p)]
+                ("fout_g0", C.c_void_p), ("fout_a1", C.c_void_p), ("fout_ld1", C.c_int32), ("fout_g1", C.c_void_p),
+                ("fin_st1", C.c_void_p), ("fin_slots1", C.c_int32)]
 
 
 class TestHeadsArgs(C.Structure):
@@ -89,6 +90,16 @@ class TestStepArgs(C.Structure):
                [(n, C.c_void_p) for n in ("x", "x2", "x3", "w", "b", "shift", "scale", "G", "Cc", "gt", "gt_mask", "mask_embed", "add", "lens",
                                           "norm_q", "norm_k", "inv_freq", "out")] + \
                [("f32_out", C.c_void_p * 3), ("bf_out", C.c_void_p * 3)]
+
+
+class TestFoldArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "variant", "M", "N", "K", "R", "inner", "geglu_bn", "bn")] + \
+               [(n, C.c_void_p) for n in ("w", "b", "shift", "scale")] + [(n, C.c_int32) for n in ("ld_mod", "rows_per_batch")] + \
+               [(n, C.c_void_p) for n in ("W", "bias", "add_v", "w_packed", "G", "Cc", "u", "v", "A", "st")] + \
+               [(n, C.c_int32) for n in ("slots", "ld_st")] + \
+               [(n, C.c_void_p) for n in ("out", "W2", "b2", "x", "gate")] + [("gate_bstride", C.c_int32)] + \
+               [(n, C.c_void_p) for n in ("fout_st", "a0", "g0", "grid_barrier", "W16", "resid", "out_f32", "x2", "x3")] + \
+               [("D2", C.c_int32), ("ln_out", C.c_void_p), ("ran_bn", C.c_int32), ("ran_fused", C.c_int32)]
 
 
 class TestCondArgs(C.Structure):
@@ -155,6 +166,7 @@ _SIGS = {
     "ezb_test_fp8": ([_I, C.POINTER(TestFp8Args), _VP], _I),
     "ezb_test_step": ([_I, C.POINTER(TestStepArgs), _VP], _I),
     "ezb_test_cond": ([_I, C.POINTER(TestCondArgs), _VP], _I),
+    "ezb_test_fold": ([_I, C.POINTER(TestFoldArgs), _VP], _I),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -125,6 +125,24 @@ inline int timestep_embed_launch(cudaStream_t st, const float* t, float* out, in
   EZB_CUDA(cudaGetLastError());
   return EZB_OK;
 }
+// Tables of the folded LayerNorm (elementwise.cuh fold_gc_kernel / fold_uv_kernel), as Dit::build_fold_tables and Dit::finalize build them.
+// fold_uv_kernel keeps a lane's share of a W row in 72 registers: K <= 72 * 32.
+constexpr int FOLD_MAX_K = 72 * 32;
+inline int fold_gc_launch(cudaStream_t st, const float* w, const float* b, const float* shift, const float* scale, int ld_mod, float* G, float* Cc, int R,
+                          int D) {
+  ++launch_counter();
+  fold_gc_kernel<<<(R * D + 255) / 256, 256, 0, st>>>(w, b, shift, scale, ld_mod, G, Cc, R, D);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+inline int fold_uv_launch(cudaStream_t st, const bf16* W, int ldw, const float* G, const float* Cc, const float* add_v, float* U, float* V, int N, int K,
+                          int R) {
+  if (K > FOLD_MAX_K) return fail(EZB_ERR_UNSUPPORTED, "fold_uv: K %d", K);
+  ++launch_counter();
+  fold_uv_kernel<<<(N + 7) / 8, 256, 0, st>>>(W, ldw, G, Cc, add_v, U, V, N, K, R);
+  EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
 
 // Does Dit::lin run this linear as swap-AB tiles (host.cuh gemm_swapped) rather than on the 128-wide N-tiles of EpiLinear?  Only fp32-output
 // layers without a uniform scale, in bf16 operands, on at least 512 tokens (m_select, 0: M) or with a folded LayerNorm; clips of fewer than 32
@@ -540,11 +558,7 @@ struct Dit {
     return EZB_OK;
   }
   int fold_uv(cudaStream_t st, const bf16* W, int ldw, const float* G, const float* Cc, const float* add_v, float* U, float* V, int N, int K, int R) {
-    if (K > 72 * 32) return fail(EZB_ERR_UNSUPPORTED, "fold_uv: K %d", K);
-    ++launch_counter();
-    fold_uv_kernel<<<(N + 7) / 8, 256, 0, st>>>(W, ldw, G, Cc, add_v, U, V, N, K, R);
-    EZB_CUDA(cudaGetLastError());
-    return EZB_OK;
+    return fold_uv_launch(st, W, ldw, G, Cc, add_v, U, V, N, K, R);
   }
   // per-timestep tables of the modulated sites (called at the end of set_timesteps)
   int build_gc_tables(int n, cudaStream_t st) {
@@ -552,10 +566,7 @@ struct Dit {
     if (gc_T == 0 || n > gc_T) return EZB_OK;
     const int ldm = nblk * 6 * D;
     auto gc = [&](const float* w_, const float* b_, const float* shift, const float* scale, int ld, float* G, float* Cc) -> int {
-      ++launch_counter();
-      fold_gc_kernel<<<(n * D + 255) / 256, 256, 0, st>>>(w_, b_, shift, scale, ld, G, Cc, n, D);
-      EZB_CUDA(cudaGetLastError());
-      return EZB_OK;
+      return fold_gc_launch(st, w_, b_, shift, scale, ld, G, Cc, n, D);
     };
     for (int i = 0; i < nblk; ++i) {
       BlockW& w = blk[i];
@@ -573,10 +584,7 @@ struct Dit {
     if (!fold_cfg || n > fold_T) return EZB_OK;
     const int ldm = nblk * 6 * D;
     auto gc = [&](const float* w_, const float* b_, const float* shift, const float* scale, int ld, float* G) -> int {
-      ++launch_counter();
-      fold_gc_kernel<<<(n * D + 255) / 256, 256, 0, st>>>(w_, b_, shift, scale, ld, G, gc_C, n, D);
-      EZB_CUDA(cudaGetLastError());
-      return EZB_OK;
+      return fold_gc_launch(st, w_, b_, shift, scale, ld, G, gc_C, n, D);
     };
     for (int i = 0; i < nblk; ++i) {
       BlockW& w = blk[i];

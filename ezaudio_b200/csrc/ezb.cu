@@ -31,6 +31,7 @@ EpiLinearParams to_epi(const ezb_test_epilogue* e) {
   if (e->fin_u) {
     p.fin.st0 = static_cast<const float2*>(e->fin_st); p.fin.slots0 = e->fin_slots; p.fin.ld_st = e->fin_ld_st; p.fin.inv_dim = e->fin_inv_dim;
     p.fin.u = e->fin_u; p.fin.v = e->fin_v;
+    p.fin.st1 = static_cast<const float2*>(e->fin_st1); p.fin.slots1 = e->fin_st1 ? e->fin_slots1 : 0;
   }
   if (e->fout_st) {
     p.fout.st = static_cast<float2*>(e->fout_st); p.fout.ld_st = e->fout_ld_st;
@@ -63,6 +64,8 @@ __attribute__((visibility("default"))) int ezb_test_gemm(int device, const void*
     EpiLinearParams p = to_epi(e);
     if ((p.fin.u && (!p.fin.st0 || !p.fin.v)) || (p.fout.st && !p.fout.a0))
       return fail(EZB_ERR_ARG, "ezb_test_gemm: fold-in needs its partials and v, fold-out its first operand");
+    if (p.fin.u && (p.fin.slots0 < 1 || (p.fin.st1 != nullptr && p.fin.slots1 < 1)))
+      return fail(EZB_ERR_ARG, "ezb_test_gemm: fold-in with %d + %d partial slots", p.fin.slots0, p.fin.slots1);
     const bool fold = p.fin.u || p.fout.st;
     if (epi_kind == 20) {   // what Dit::lin dispatches
       if (fold) return gemm_swapped<EpiLinearTF>(dev, st, a, lda, w, ldw, M, N, K, p);
@@ -296,6 +299,138 @@ __attribute__((visibility("default"))) int ezb_test_mlp(int device, const void* 
   }
   EZB_CUDA(cudaFreeAsync(W1p, st));
   EZB_CUDA(cudaFreeAsync(b1p, st));
+  return rc;
+}
+
+}  // extern "C"
+
+namespace {
+int test_fold_check(const ezb_test_fold_args* a) {
+  const int kind = a->kind, M = a->M, N = a->N, K = a->K;
+  if (kind < 0 || kind > 3) return fail(EZB_ERR_ARG, "ezb_test_fold: kind %d", kind);
+  if (!a->shift != !a->scale) return fail(EZB_ERR_ARG, "ezb_test_fold: shift and scale come in pairs");
+  if (kind <= 2) {
+    if (!a->W || !a->w || !a->b || !a->G || !a->Cc || !a->u || !a->v) return fail(EZB_ERR_ARG, "ezb_test_fold: the tables need W, w, b, G, Cc, u and v");
+    if (K > FOLD_MAX_K) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_fold: K %d (the tables take at most %d)", K, FOLD_MAX_K);
+    if (K < 8 || K % 8) return fail(EZB_ERR_SHAPE, "ezb_test_fold: K %d (a multiple of 8)", K);
+    if (a->shift && a->R > 1 && a->ld_mod < K) return fail(EZB_ERR_SHAPE, "ezb_test_fold: modulation rows %d apart, narrower than K %d", a->ld_mod, K);
+  }
+  if (kind == 0) {
+    if (!a->w_packed) return fail(EZB_ERR_ARG, "ezb_test_fold: the tables write the packed weight");
+    if (N < 1 || a->R < 1 || a->R > 128 || (long long)N * K > (1LL << 28)) return fail(EZB_ERR_SHAPE, "ezb_test_fold: tables N %d R %d", N, a->R);
+    return EZB_OK;
+  }
+  if (kind <= 2) {
+    const int inner = a->inner, bn = kind == 2 ? 256 : a->geglu_bn;
+    if (!a->A || !a->st || !a->bias || !a->out) return fail(EZB_ERR_ARG, "ezb_test_fold: the GEGLU needs A, st, bias and out");
+    if (a->R != 1) return fail(EZB_ERR_ARG, "ezb_test_fold: the GEGLU tables take one modulation row (R 1, not %d)", a->R);
+    if (M < 1 || M > (1 << 24) || inner < 64 || inner % 64) return fail(EZB_ERR_SHAPE, "ezb_test_fold: M %d inner %d (a multiple of 64)", M, inner);
+    if (bn != 0 && bn != 128 && bn != 256) return fail(EZB_ERR_ARG, "ezb_test_fold: geglu_bn %d (0, 128 or 256)", bn);
+    if (bn == 256 && inner % 128) return fail(EZB_ERR_UNSUPPORTED, "ezb_test_fold: 256-wide GEGLU tiles need inner %d to be a multiple of 128", inner);
+    if (a->slots < 1 || a->ld_st < M) return fail(EZB_ERR_SHAPE, "ezb_test_fold: %d partial slots of pitch %d for %d rows", a->slots, a->ld_st, M);
+  }
+  if (kind == 2) {
+    if (!a->W2 || !a->b2 || !a->x || !a->fout_st || !a->a0 || !a->g0 || !a->grid_barrier)
+      return fail(EZB_ERR_ARG, "ezb_test_fold: the fused MLP needs W2, b2, x, fout_st, a0, g0 and grid_barrier");
+    if (K % 32) return fail(EZB_ERR_SHAPE, "ezb_test_fold: the folded-out partials need K %d to be a multiple of 32", K);
+    if (a->gate && a->rows_per_batch < 32) return fail(EZB_ERR_SHAPE, "ezb_test_fold: %d rows per clip (>= 32)", a->rows_per_batch);
+    if (a->variant < 0 || a->variant > 1) return fail(EZB_ERR_ARG, "ezb_test_fold: variant %d", a->variant);
+  }
+  if (kind == 3) {
+    if (!a->A || !a->W16 || !a->out_f32 || !a->ln_out || !a->w || !a->b || !a->grid_barrier)
+      return fail(EZB_ERR_ARG, "ezb_test_fold: the LayerNorm tail needs A, W16, out_f32, ln_out, w, b and grid_barrier");
+    if (M < 1 || M > (1 << 24) || N < 4 || N % 4 || K < 8 || K % 8 || a->D2 < 0 || a->D2 % 4)
+      return fail(EZB_ERR_SHAPE, "ezb_test_fold: tail M %d N %d K %d D2 %d", M, N, K, a->D2);
+    if ((a->D2 > 0) != (a->x2 != nullptr) || (a->x3 && !a->x2)) return fail(EZB_ERR_ARG, "ezb_test_fold: x2 must come with D2 > 0, x3 with x2");
+    if (a->shift && (a->x2 || a->rows_per_batch < 1 || a->ld_mod < 0 || a->ld_mod % 4))
+      return fail(EZB_ERR_ARG, "ezb_test_fold: modulation needs one source, rows_per_batch >= 1 and ld_mod a multiple of 4");
+    if (a->gate && (!a->resid || a->rows_per_batch < 32)) return fail(EZB_ERR_ARG, "ezb_test_fold: a gate needs a residual and clips of >= 32 rows");
+    if (a->bn != 0 && a->bn != 256 && a->bn != 288) return fail(EZB_ERR_ARG, "ezb_test_fold: bn %d (0, 256 or 288)", a->bn);
+    const void* ps[] = {a->out_f32, a->x2, a->x3, a->w, a->b, a->shift, a->scale, a->ln_out, a->A};
+    for (const void* q : ps)
+      if (!aligned(q, 16)) return fail(EZB_ERR_ARG, "ezb_test_fold: LayerNorm pointers and A must be 16-byte aligned");
+  }
+  return EZB_OK;
+}
+// kinds 1 / 2: W and its bias packed as Dit::init packs them, the site-3 tables as Dit::build_fold_tables builds them, then the GEMM(s)
+int test_fold_run(Device& dev, cudaStream_t st, ezb_test_fold_args* a, __nv_bfloat16* Wp, float* bp) {
+  const int M = a->M, D = a->K, inner = a->inner;
+  const int bn = a->kind == 2 ? 256 : a->geglu_bn ? a->geglu_bn : (inner % 128 == 0 ? 256 : 128), gh = bn / 2;
+  pack_weight_kernel<<<(unsigned)(((size_t)2 * inner * D + 255) / 256), 256, 0, st>>>(a->W, 2 * inner, D, Wp, D, 1, 0, inner, gh, 0, 0, 0);
+  pack_geglu_bias_kernel<<<(2 * inner + 255) / 256, 256, 0, st>>>(a->bias, bp, inner, gh);
+  EZB_CUDA(cudaGetLastError());
+  if (a->w_packed) EZB_CUDA(cudaMemcpyAsync(a->w_packed, Wp, (size_t)2 * inner * D * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice, st));
+  EZB_TRY(fold_gc_launch(st, a->w, a->b, a->shift, a->scale, a->ld_mod, a->G, a->Cc, 1, D));
+  EZB_TRY(fold_uv_launch(st, Wp, D, a->G, a->Cc, bp, a->u, a->v, 2 * inner, D, 1));   // v carries the packed GEGLU bias
+  EpiGegluParams g;
+  memset(&g, 0, sizeof g);
+  g.bias = bp; g.out_bf16 = static_cast<__nv_bfloat16*>(a->out); g.ld16 = inner;
+  g.fin.st0 = static_cast<const float2*>(a->st); g.fin.slots0 = a->slots; g.fin.ld_st = a->ld_st; g.fin.inv_dim = 1.0f / (float)D;
+  g.fin.u = a->u; g.fin.v = a->v;
+  const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(a->A);
+  if (a->kind == 1) {
+    if (bn == 256) return gemm2<256, EpiGeglu<256, true>>(dev, st, A, D, Wp, D, M, 2 * inner, D, g);
+    return gemm<128, EpiGeglu<128, true>>(dev, st, A, D, Wp, D, M, 2 * inner, D, g);
+  }
+  EpiLinearParams e;
+  memset(&e, 0, sizeof e);
+  e.bias = a->b2; e.resid = a->x; e.ldr = D; e.gate = a->gate; e.gate_bstride = a->gate_bstride; e.rows_per_batch = a->gate ? a->rows_per_batch : 1;
+  e.out_f32 = a->x; e.ld32 = D;
+  e.fout.st = static_cast<float2*>(a->fout_st); e.fout.ld_st = a->ld_st; e.fout.a0 = static_cast<__nv_bfloat16*>(a->a0); e.fout.ld0 = D; e.fout.g0 = a->g0;
+  const __nv_bfloat16* mid = static_cast<const __nv_bfloat16*>(a->out);
+  const __nv_bfloat16* W2 = static_cast<const __nv_bfloat16*>(a->W2);
+  if (a->variant == 0)
+    return mlp_fused<EpiGeglu<256, true>, EpiLinearTF<256>>(dev, st, A, Wp, M, 2 * inner, D, g, mid, W2, D, inner, e, static_cast<GridBarrier*>(a->grid_barrier));
+  EZB_TRY((gemm2<256, EpiGeglu<256, true>>(dev, st, A, D, Wp, D, M, 2 * inner, D, g)));
+  return gemm_swapped<EpiLinearTF>(dev, st, mid, inner, W2, inner, M, D, inner, e);
+}
+}  // namespace
+
+extern "C" {
+
+__attribute__((visibility("default"))) int ezb_test_fold(int device, ezb_test_fold_args* a, void* stream) {
+  if (!a) return fail(EZB_ERR_ARG, "ezb_test_fold: null arguments");
+  EZB_TRY(test_fold_check(a));
+  EZB_CUDA(cudaSetDevice(device));
+  Device& dev = device_ctx(device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int M = a->M, N = a->N, K = a->K;
+  if (a->kind == 0) {   // Dit::build_fold_tables / Dit::finalize
+    __nv_bfloat16* Wp = static_cast<__nv_bfloat16*>(a->w_packed);
+    pack_weight_kernel<<<(unsigned)(((size_t)N * K + 255) / 256), 256, 0, st>>>(a->W, N, K, Wp, K, 1, 0, 0, 0, 0, 0, 0);
+    EZB_CUDA(cudaGetLastError());
+    EZB_TRY(fold_gc_launch(st, a->w, a->b, a->shift, a->scale, a->ld_mod, a->G, a->Cc, a->R, K));
+    return fold_uv_launch(st, Wp, K, a->G, a->Cc, a->add_v, a->u, a->v, N, K, a->R);
+  }
+  if (a->kind == 3) {   // Dit::lin with a LayerNorm tail (gemm_swapped_ln)
+    LnParams lp;
+    memset(&lp, 0, sizeof lp);
+    lp.x = a->out_f32; lp.x2 = a->x2; lp.x3 = a->x3; lp.D1 = N; lp.D2 = a->D2; lp.w = a->w; lp.b = a->b; lp.shift = a->shift; lp.scale = a->scale;
+    lp.mod_bstride = a->ld_mod; lp.rows_per_batch = a->shift ? a->rows_per_batch : 1; lp.out = static_cast<__nv_bfloat16*>(a->ln_out); lp.kmul = 1;
+    lp.M = M;
+    EpiLinearParams e;
+    memset(&e, 0, sizeof e);
+    e.bias = a->bias; e.resid = a->resid; e.ldr = N; e.gate = a->gate; e.gate_bstride = a->gate_bstride; e.rows_per_batch = a->gate ? a->rows_per_batch : 1;
+    e.out_f32 = a->out_f32; e.ld32 = N;
+    const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(a->A);
+    const __nv_bfloat16* W = static_cast<const __nv_bfloat16*>(a->W16);
+    GridBarrier* bar = static_cast<GridBarrier*>(a->grid_barrier);
+    const int bn = a->bn ? a->bn : swapped_bn(dev, M, N);
+    bool fused = false;
+    const int rc = bn == 288 ? gemm_swapped_ln_at<288, EpiLinearT<288>>(dev, st, A, K, W, K, M, N, K, e, lp, bar, &fused)
+                             : gemm_swapped_ln_at<256, EpiLinearT<256>>(dev, st, A, K, W, K, M, N, K, e, lp, bar, &fused);
+    a->ran_bn = bn;
+    a->ran_fused = fused ? 1 : 0;
+    return rc;
+  }
+  dev.tmaps.trim();
+  __nv_bfloat16* Wp = nullptr;
+  float* bp = nullptr;
+  EZB_CUDA(cudaMallocAsync(&Wp, (size_t)2 * a->inner * K * sizeof(__nv_bfloat16), st));
+  EZB_CUDA(cudaMallocAsync(&bp, (size_t)2 * a->inner * sizeof(float), st));
+  const int rc = test_fold_run(dev, st, a, Wp, bp);
+  EZB_CUDA(cudaFreeAsync(Wp, st));
+  EZB_CUDA(cudaFreeAsync(bp, st));
   return rc;
 }
 

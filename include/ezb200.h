@@ -221,6 +221,8 @@ typedef struct {
      are float2 (sum, sum of squares) partials, slot-major with pitch fin_ld_st / fout_ld_st. */
   const void* fin_st; int32_t fin_slots; int32_t fin_ld_st; float fin_inv_dim; const float* fin_u; const float* fin_v;
   void* fout_st; int32_t fout_ld_st; void* fout_a0; int32_t fout_ld0; const float* fout_g0; void* fout_a1; int32_t fout_ld1; const float* fout_g1;
+  /* second fold-in source (the out-blocks' skip_norm over [x | skip]): its partials follow fin_st's in the row statistics; NULL: none */
+  const void* fin_st1; int32_t fin_slots1;
 } ezb_test_epilogue;
 /* C = A[M,K] W[N,K]^T through the wgmma GEMM; epi_kind 0 = linear epilogue, 1 = GEGLU (packed W); 10 / 11 = the same on 2-CTA
    clusters (11: the GEGLU kernel the model dispatches); 12 = the parked-tile cluster GEGLU; 20 = swap-AB as the model dispatches it
@@ -290,6 +292,42 @@ int ezb_test_heads(int device, const void* A_bf16, const float* W_f32, const ezb
 int ezb_test_mlp(int device, const void* A_bf16, const float* W1_f32, const float* b1_f32, const void* W2_bf16, const float* b2, float* x,
                  const float* gate, int gate_bstride, int rows_per_batch, void* mid_bf16, void* grid_barrier, int M, int D, int inner,
                  int variant, void* stream);
+/* The folded LayerNorm (csrc/gemm.cuh FoldIn / FoldOut, csrc/dit.cuh build_fold_tables) and the LayerNorm tail of a swap-AB GEMM
+   (csrc/gemm_ln.cuh), launched as Dit launches them.  Device pointers unless noted; every argument is checked before any device work.
+   Tables (kinds 0-2): G = w (1 + scale), Cc = b (1 + scale) + shift for R modulation rows (row r of shift / scale at r * ld_mod; both NULL:
+   G = w, Cc = b) -> G, Cc fp32 [R, K]; then U = G W'^T, V = Cc W'^T (+ add_v) -> u, v fp32 [R, N], W' the packed bf16 weight.
+   kind 0 tables:        W fp32 [N, K] in the reference layout, packed plainly (bf16(W)) into w_packed [N, K]; add_v [N] optional.  K at most
+                         2304 (a larger K is refused with EZB_ERR_UNSUPPORTED).
+   kind 1 FoldIn GEGLU:  W fp32 [2 inner, K] ([hidden; gate] rows) and bias [2 inner], packed as Dit::init packs them for GEGLU N-tiles of
+                         geglu_bn columns (0: what Dit picks, 256 when inner % 128 == 0, else 128); the tables with R = 1, N = 2 inner and
+                         add_v = the packed bias (u, v in the packed order); then the GEGLU GEMM with the LayerNorm folded in: A bf16 [M, K]
+                         = bf16(x G) of the rows x whose (sum, sum of squares) partials are st, float2 [slots][ld_st] -> out bf16 [M, inner].
+                         w_packed (optional) receives W'.
+   kind 2 fused MLP:     kind 1 with geglu_bn 256 into out = mid bf16 [M, inner], then x += (1 - gate[b]) (mid W2^T + b2) in place, x fp32
+                         [M, K], W2 bf16 [K, inner], b = row / rows_per_batch (gate NULL: plain residual), folded out: a0 bf16 [M, K] =
+                         bf16(x g0) and fout_st float2 [K / 32][ld_st] partials of the new x.  variant 0: one persistent launch on
+                         grid_barrier (two zeroed uint32, left with count 0); 1: the same two GEMMs as two launches.
+   kind 3 LayerNorm tail: x = A W16^T + bias (+ resid, gated as kind 2) -> out_f32 fp32 [M, N] (A bf16 [M, K], W16 bf16 [N, K], resid pitch
+                         N), on swap-AB tiles of bn tokens (0: the width gemm_swapped_ln picks; 256 or 288), and the LayerNorm of the row
+                         [x | x2 (+ x3)] (x2 / x3 fp32 [M, D2], optional) with w / b, optional modulation shift / scale (row
+                         (row / rows_per_batch) * ld_mod) -> ln_out bf16 [M, N + D2]: as the tail phase of the same launch behind
+                         grid_barrier when the tiles fit one wave, else not at all (the caller launches it).  ran_bn and ran_fused receive
+                         the token width and whether the tail ran.  LayerNorm pointers 16-byte aligned, N, D2 and ld_mod multiples of 4. */
+typedef struct {
+  int32_t kind, variant;
+  int32_t M, N, K, R, inner, geglu_bn, bn;
+  const float* w; const float* b; const float* shift; const float* scale; int32_t ld_mod, rows_per_batch;
+  const float* W; const float* bias; const float* add_v;
+  void* w_packed; float* G; float* Cc; float* u; float* v;
+  const void* A; const void* st; int32_t slots, ld_st;
+  void* out;
+  const void* W2; const float* b2; float* x; const float* gate; int32_t gate_bstride;
+  void* fout_st; void* a0; const float* g0;
+  void* grid_barrier;
+  const void* W16; const float* resid; float* out_f32; const float* x2; const float* x3; int32_t D2; void* ln_out;
+  int32_t ran_bn, ran_fused;
+} ezb_test_fold_args;
+int ezb_test_fold(int device, ezb_test_fold_args* args, void* stream);
 /* One layer of the Oobleck VAE, launched as Vae::decode / Vae::encode launch it (csrc/vae.cuh vae_conv and friends), from reference-layout
    fp32 weights that the library weight-norms and packs.  Device pointers; kmul = 3 when precision is 1 (bf16x3), else 1.
    kind 0 conv:       Conv1d(cin -> cout, taps, dilation dil, padding dil * (taps - 1) / 2), taps odd.  x: bf16 A [B, T, kmul*cin];

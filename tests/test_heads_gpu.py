@@ -248,7 +248,7 @@ def _fold_inputs(seed, M, D, W, H, dh, nsec, packed):
                                                       (64, 4, 3, 25, 64, ROPE_NONE, 1)])
 def test_folded_layernorm_heads(dh, H, B, L, ld_qk, rope, nsec):
     """FOLD instantiations (LayerNorm of the block input folded into the projection): the epilogue's rstd * (A W^T - mu u) + v followed by
-    the same per-head LayerNorm, RoPE and layout.  Whether the fold equals the true LayerNorm is test_fold_gpu.py's job."""
+    the same per-head LayerNorm, RoPE and layout.  Whether the fold equals the true LayerNorm is test_fold_layers_gpu.py's job."""
     D, M = H * dh, B * L
     kinds = (0, 1, 2) if nsec == 3 else (0,)
     _, W, nq, nk, inv_freq = _inputs(dh * 1000 + H * 100 + L + B + 11, M, D, nsec, dh)
