@@ -1000,28 +1000,38 @@ EZB_API int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noi
 }  // extern "C"
 
 namespace {
-// impl 0: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]); impl 1/4/6/7/8 (+100): tensor-core kernel (q,k bf16 [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad])
+// impl 0 / 3: fp32 CUDA-core kernel (q,k,v fp32 [B,H,L,dh]; 3 writes bf16x3 rows); impl 1/4/6/7/8 (+100): tensor-core kernel (q,k bf16
+// [B*H,L,DHP], vt bf16 [B*H,DVP,Lkpad]).  Every argument is checked before any device work.
 int test_attention(int device, const void* q, const void* k, const void* v, const uint8_t* key_mask, const int32_t* lens, void* out, int B, int H,
                    int Lq, int Lk, int dh, int impl, void* stream) {
   if (!q || !k || !v || !out) return fail(EZB_ERR_ARG, "ezb_test_attention: null pointer");
-  EZB_CUDA(cudaSetDevice(device));
+  const bool simt = impl == 0 || impl == 3;
+  const int variant = impl % 100;
+  if (!simt && (impl < 0 || impl >= 200 || (variant != 1 && variant != 4 && variant != 6 && variant != 7 && variant != 8)))
+    return fail(EZB_ERR_ARG, "ezb_test_attention: impl %d", impl);
+  if (simt && (dh < 4 || dh % 4 || dh > 96)) return fail(EZB_ERR_UNSUPPORTED, "fp32 attention: head dimension %d (multiples of 4 up to 96)", dh);
+  if (!simt && (dh < 8 || dh % 8 || dh > 80)) return fail(EZB_ERR_UNSUPPORTED, "attention: head dimension %d (multiples of 8 up to 80)", dh);
+  if (variant == 8 && dh != 64 && dh != 72) return fail(EZB_ERR_UNSUPPORTED, "attention generation 8: head dimension %d (64 or 72)", dh);
+  if (B < 1 || H < 1 || Lq < 1 || Lk < 1 || (long long)B * H > 65535)
+    return fail(EZB_ERR_SHAPE, "ezb_test_attention: B %d H %d Lq %d Lk %d", B, H, Lq, Lk);
   const float scale = 1.0f / sqrtf((float)dh);
-  if (impl == 0) {
-    if (dh % 4) return fail(EZB_ERR_UNSUPPORTED, "fp32 attention: head dimension %d is not a multiple of 4", dh);
+  if (simt) {
+    EZB_CUDA(cudaSetDevice(device));
     auto kern = lens ? attn_simt_kernel<true> : attn_simt_kernel<false>;
     EZB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     dim3 grid((Lq + SA_WARPS * SA_QW - 1) / (SA_WARPS * SA_QW), B * H);
     ++launch_counter();
     kern<<<grid, SA_WARPS * 32, attn_simt_smem(dh), ST(stream)>>>(reinterpret_cast<const float*>(q), reinterpret_cast<const float*>(k),
                                                                             reinterpret_cast<const float*>(v), key_mask,
-                                                                            reinterpret_cast<__nv_bfloat16*>(out), H, Lq, Lk, dh, scale, 1, lens, nullptr);
+                                                                            reinterpret_cast<__nv_bfloat16*>(out), H, Lq, Lk, dh, scale,
+                                                                            impl == 3 ? 3 : 1, lens, nullptr);
     EZB_CUDA(cudaGetLastError());
     return EZB_OK;
   }
   // impl 1: the variant the options select; 4 / 6 / 7 / 8: that generation forced; +100: q / k rows of 80 elements for dh = 72 (the product's
   // layout) instead of a 64-multiple
-  const int variant = impl % 100, row80 = impl >= 100;
-  if (variant != 1 && variant != 4 && variant != 6 && variant != 7 && variant != 8) return fail(EZB_ERR_ARG, "ezb_test_attention: impl %d", impl);
+  const int row80 = impl >= 100;
+  EZB_CUDA(cudaSetDevice(device));
   const int dhp = (row80 && dh == 72) ? 80 : (dh + 63) / 64 * 64;
   const int dvp = (dh + 15) / 16 * 16, lkpad = (Lk + 7) / 8 * 8;
   device_ctx(device).tmaps.trim();

@@ -433,8 +433,11 @@ typedef struct {
   void* out; float* out32; float* out_v;
 } ezb_test_cond_args;
 int ezb_test_cond(int device, const ezb_test_cond_args* args, void* stream);
-/* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]); 1: the tensor-core kernel variant the options select; 4 / 6 / 7 / 8: that
-   generation forced (8 takes dh 64 or 72 only); +100: q / k rows of 80 elements for dh = 72 (the product's layout) instead of a 64-multiple */
+/* impl 0: fp32 CUDA-core kernel (q, k, v fp32 [B,H,L,dh]; dh a multiple of 4 up to 96) writing out [B, Lq, H dh]; 3: the same kernel writing
+   bf16x3 rows [B, Lq, 3 H dh] = [hi | lo | hi], as the bf16x3 parity mode runs it; 1: the tensor-core kernel variant the options select
+   (dh a multiple of 8 up to 80); 4 / 6 / 7 / 8: that generation forced (8 takes dh 64 or 72 only); +100: q / k rows of 80 elements for
+   dh = 72 (the product's layout) instead of a 64-multiple.  B, H, Lq, Lk >= 1 and B H <= 65535.  Bad arguments are refused before any
+   device work. */
 int ezb_test_attention(int device, const void* q, const void* k, const void* vt, const uint8_t* key_mask, void* out_bf16,
                        int B, int H, int Lq, int Lk, int dh, int impl, void* stream);
 /* Self-attention (Lq = Lk = L, no key mask) of a padded batch, as ezb_test_attention with the same impl codes: lens DEVICE int32 [B],

@@ -19,8 +19,8 @@ def _ref(q, k, v, mask):
     return o.permute(0, 2, 1, 3).reshape(q.shape[0], q.shape[2], -1)
 
 
-# 0 = fp32 CUDA-core kernel (parity mode); 1 = the tensor-core kernel the product uses (generation 6 of attention_mma.cuh unless the options say
-# otherwise); 4 = generation 4 (128 query rows per CTA); +100 = q / k rows of 80 elements for dh = 72 (160-byte pitch) instead of 128
+# 0 = fp32 CUDA-core kernel (parity mode); 1 = the tensor-core kernel the options select (generation 8 of attention_wgmma.cuh for dh 64 / 72
+# by default, generation 6 of attention_mma.cuh for other head dims); 4 = generation 4 (128 query rows per CTA); +100 = q / k rows of 80 elements for dh = 72 (160-byte pitch) instead of 128
 @pytest.mark.parametrize("impl", [0, 1, 4, 101, 104])
 @pytest.mark.parametrize("B,H,Lq,Lk,dh,masked", [(2, 4, 500, 500, 72, False), (2, 3, 256, 256, 64, False), (3, 2, 500, 100, 72, True),
                                                  (2, 2, 40, 12, 72, True), (1, 2, 130, 130, 64, False), (1, 16, 1500, 1500, 72, False),
@@ -77,7 +77,7 @@ def test_attention_kv_resident(B, H, Lq, Lk, dh, masked):
     numbers of query tiles per head, one to eight key blocks, more heads than SMs (two waves of CTAs), masks, growth."""
     from ezaudio_b200 import _lib
     L = _lib.lib()
-    _lib.check(L.ezb_set_option(b"attn6", 0))   # generation-4 kernel (the default is generation 6)
+    _lib.check(L.ezb_set_option(b"attn6", 0))   # generation-4 kernel (the default is generation 8)
     _lib.check(L.ezb_set_option(b"attn_res", 1))
     try:
         test_attention(1, B, H, Lq, Lk, dh, masked)
@@ -97,7 +97,7 @@ def test_attention_mufu_token(B, H, Lq, Lk, dh, masked, res):
     a single query tile, one to twelve key blocks, with and without resident K / V^T."""
     from ezaudio_b200 import _lib
     L = _lib.lib()
-    _lib.check(L.ezb_set_option(b"attn6", 0))   # generation-4 kernel (the default is generation 6)
+    _lib.check(L.ezb_set_option(b"attn6", 0))   # generation-4 kernel (the default is generation 8)
     _lib.check(L.ezb_set_option(b"attn_pp", 1))
     _lib.check(L.ezb_set_option(b"attn_res", res))
     try:

@@ -50,14 +50,14 @@ def _attention(impl, args, lens, B, H, L, dh):
     return out
 
 
-# impl as in ezb_test_attention: 0 fp32 CUDA-core kernel (parity mode); 1 the selected tensor-core variant (generation 6 by default, 4 with
-# attn6 = 0, 4 + RES with attn_res); 4 / 7 forced; +100 the 80-element q / k rows of dh = 72
+# impl as in ezb_test_attention: 0 fp32 CUDA-core kernel (parity mode); 1 the selected tensor-core variant (4 with attn6 = 0, 4 + RES with
+# attn_res); 4 / 6 / 7 forced (generation 8's padded batches are test_attention_wgmma_gpu.py's); +100 the 80-element q / k rows of dh = 72
 @pytest.mark.parametrize("dh", [72, 64])
 @pytest.mark.parametrize("variant", ["simt", "6", "6r80", "4", "4r80", "4res", "7", "7r80"])
 def test_attention_lens_matches_solo_runs(variant, dh):
     from ezaudio_b200 import _lib
     Lib = _lib.lib()
-    impl = {"simt": 0, "6": 1, "6r80": 101, "4": 4, "4r80": 104, "4res": 1, "7": 7, "7r80": 107}[variant]
+    impl = {"simt": 0, "6": 6, "6r80": 106, "4": 4, "4r80": 104, "4res": 1, "7": 7, "7r80": 107}[variant]
     if variant == "4res":
         _lib.check(Lib.ezb_set_option(b"attn6", 0))
         _lib.check(Lib.ezb_set_option(b"attn_res", 1))
