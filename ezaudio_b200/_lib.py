@@ -36,7 +36,12 @@ class DdimSlot(C.Structure):
     _fields_ = [("guidance_scale", C.c_float), ("guidance_rescale", C.c_float), ("coef", C.c_float * 5), ("flags", C.c_int32)]
 
 
-SLOT_ACTIVE, SLOT_CFG = 1, 2   # ezb_ddim_slot.flags
+class DpmSlot(C.Structure):
+    """ezb_dpm_slot: the CFG / DPM-Solver++ constants of one sample of ezb_cfg_dpm_step_slots."""
+    _fields_ = [("guidance_scale", C.c_float), ("guidance_rescale", C.c_float), ("coef", C.c_float * 7), ("flags", C.c_int32)]
+
+
+SLOT_ACTIVE, SLOT_CFG, SLOT_ORDER2 = 1, 2, 4   # ezb_ddim_slot.flags / ezb_dpm_slot.flags
 
 
 class TestEpilogue(C.Structure):
@@ -126,6 +131,8 @@ _SIGS = {
     "ezb_dit_set_context_rows": ([_VP, _VP, _VP, _I, _I, _I, _VP], _I),
     "ezb_dit_forward_tdev": ([_VP, _VP, _VP, _VP, _VP, C.POINTER(_VP), _VP, _I, _I, _VP, _VP], _I),
     "ezb_cfg_ddim_step_slots": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP], _I),
+    "ezb_cfg_dpm_step": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _F, _F, C.POINTER(C.c_float), _I, _VP, _VP], _I),
+    "ezb_cfg_dpm_step_slots": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP], _I),
     "ezb_controlnet_set_condition": ([_VP, _VP, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition_rows": ([_VP, _VP, _I, _I, _I, _VP], _I),
     "ezb_controlnet_forward_tdev": ([_VP, _VP, _VP, _VP, C.POINTER(_VP), _I, _I, _VP], _I),

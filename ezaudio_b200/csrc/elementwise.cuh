@@ -1,5 +1,5 @@
 // Bandwidth-bound kernels of the DiT step: LayerNorm(+AdaLN modulate)+cast, per-head qk-LayerNorm + RoPE + head layout,
-// patch-embed input packing, final 3-tap conv, time-embedding path, weight repacking, CFG + DDIM update.
+// patch-embed input packing, final 3-tap conv, time-embedding path, weight repacking, CFG + DDIM / DPM-Solver++ update.
 // All fp32 math; bf16 only where a tensor feeds a tensor-core operand.
 #pragma once
 #include "common.cuh"
@@ -690,11 +690,16 @@ __device__ __forceinline__ double ld_dsmem_f64(const double* local, uint32_t ran
   asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(mapa_u32(smem_u32(local), rank)));
   return v;
 }
-// The update of one sample by its cluster (after pdl_wait): shared by cfg_ddim_kernel (scalars of the call) and cfg_ddim_slots_kernel
-// (scalars of the sample's slot).  out_uncond null: no guidance; noise null: sigma == 0.
-__device__ __forceinline__ void cfg_ddim_sample(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
-                                                const float* __restrict__ noise, const int32_t* __restrict__ lens, int sample, int C, int L, float gs,
-                                                float gr, float c0, float c1, float c2, float c3, float c4) {
+// The update of one sample by its cluster (after pdl_wait), shared by the DDIM kernels (DPM = false: cfg_ddim_kernel with the scalars of the
+// call, cfg_ddim_slots_kernel with those of the sample's slot) and the DPM-Solver++ kernels (DPM = true, below), which differ only in the
+// per-element update after guidance and rescale.  out_uncond null: no guidance; noise null: its coefficient (c4 / c6) is 0.
+// DDIM: c0..c4 = {sqrt(a), sqrt(1-a), sqrt(a_prev), sqrt(1-a_prev-sigma^2), sigma}.  DPM: c0..c6 = ezb_dpm_slot.coef; history and order2 unused
+// by DDIM.
+template <bool DPM>
+__device__ __forceinline__ void cfg_update_sample(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
+                                                  const float* __restrict__ noise, const int32_t* __restrict__ lens, int sample, int C, int L, float gs,
+                                                  float gr, float c0, float c1, float c2, float c3, float c4, float c5 = 0.f, float c6 = 0.f,
+                                                  float* __restrict__ history = nullptr, bool order2 = false) {
   __shared__ double red[4][32];
   __shared__ double part[4];
   const uint32_t rank = cluster_ctarank();
@@ -747,10 +752,20 @@ __device__ __forceinline__ void cfg_ddim_sample(const float* __restrict__ out_te
       if (gr > 0.f) v = gr * (v * ratio) + (1.f - gr) * v;
     }
     const float xi = x[j];
-    const float x0 = c0 * xi - c1 * v, eps = c0 * v + c1 * xi;
-    float prev = c2 * x0 + c3 * eps;
-    if (z) prev += c4 * z[j];
-    x[j] = prev;
+    if constexpr (DPM) {   // m0 = alpha_s x - sigma_s v;  x <- kx x + k0 m0 [+ k1 (r (m0 - m1))] [+ kz z];  history <- m0
+      float* m = history + base;
+      const float m0 = c0 * xi - c1 * v;
+      float prev = c2 * xi + c3 * m0;
+      if (order2) prev += c4 * (c5 * (m0 - m[j]));
+      if (z) prev += c6 * z[j];
+      m[j] = m0;
+      x[j] = prev;
+    } else {
+      const float x0 = c0 * xi - c1 * v, eps = c0 * v + c1 * xi;
+      float prev = c2 * x0 + c3 * eps;
+      if (z) prev += c4 * z[j];
+      x[j] = prev;
+    }
   }
 }
 __global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
@@ -758,7 +773,7 @@ __global__ void __launch_bounds__(1024) cfg_ddim_kernel(const float* __restrict_
                                                         float c0, float c1, float c2, float c3, float c4) {
   pdl_launch();
   pdl_wait();
-  cfg_ddim_sample(out_text, out_uncond, latents, noise, lens, blockIdx.x / CFG_CLUSTER, C, L, gs, gr, c0, c1, c2, c3, c4);
+  cfg_update_sample<false>(out_text, out_uncond, latents, noise, lens, blockIdx.x / CFG_CLUSTER, C, L, gs, gr, c0, c1, c2, c3, c4);
 }
 // The same update with the constants of each sample read from its slot (ezb_ddim_slot, device memory), so that one captured launch serves
 // samples at different points of different schedules.  out_uncond = the B uncond rows, used by slots with EZB_SLOT_CFG; a slot without
@@ -771,8 +786,36 @@ __global__ void __launch_bounds__(1024) cfg_ddim_slots_kernel(const float* __res
   const int sample = blockIdx.x / CFG_CLUSTER;
   const ezb_ddim_slot s = slots[sample];
   if (!(s.flags & EZB_SLOT_ACTIVE)) return;   // every CTA of the cluster reads the same slot: the cluster leaves whole, before any cluster barrier
-  cfg_ddim_sample(out_text, (s.flags & EZB_SLOT_CFG) ? out_uncond : nullptr, latents, s.coef[4] != 0.f ? noise : nullptr, lens, sample, C, L,
-                  s.guidance_scale, s.guidance_rescale, s.coef[0], s.coef[1], s.coef[2], s.coef[3], s.coef[4]);
+  cfg_update_sample<false>(out_text, (s.flags & EZB_SLOT_CFG) ? out_uncond : nullptr, latents, s.coef[4] != 0.f ? noise : nullptr, lens, sample, C, L,
+                           s.guidance_scale, s.guidance_rescale, s.coef[0], s.coef[1], s.coef[2], s.coef[3], s.coef[4]);
+}
+
+// Classifier-free guidance + rescale fused with the DPM-Solver++ multistep update (diffusers DPMSolverMultistepScheduler, dpmsolver++ and
+// sde-dpmsolver++, midpoint; ezaudio_b200/scheduler.py): cfg_update_sample<true>, the same clusters, slices, element order and rescale
+// reduction as the DDIM update.  Per element, with v the guided model output and c = ezb_dpm_slot.coef = {alpha_s, sigma_s, kx, k0, k1, r, kz}:
+//   m0 = alpha_s x - sigma_s v ;  x <- kx x + k0 m0 [+ k1 (r (m0 - m1))]_order2 [+ kz z]_noise ;  history <- m0
+// m1 (the previous step's m0) is read from history only at order 2; noise null: kz == 0.
+__global__ void __launch_bounds__(1024) cfg_dpm_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond, float* __restrict__ latents,
+                                                       float* __restrict__ history, const float* __restrict__ noise, const int32_t* __restrict__ lens,
+                                                       int C, int L, const ezb_dpm_slot s) {
+  pdl_launch();
+  pdl_wait();
+  cfg_update_sample<true>(out_text, out_uncond, latents, noise, lens, blockIdx.x / CFG_CLUSTER, C, L, s.guidance_scale, s.guidance_rescale, s.coef[0],
+                          s.coef[1], s.coef[2], s.coef[3], s.coef[4], s.coef[5], s.coef[6], history, (s.flags & EZB_SLOT_ORDER2) != 0);
+}
+// Per-sample constants from ezb_dpm_slot (device memory), as cfg_ddim_slots_kernel: a slot without EZB_SLOT_ACTIVE (a free slot, or one that
+// runs DDIM) leaves its latents and history untouched; noise is read only by slots with kz != 0.
+__global__ void __launch_bounds__(1024) cfg_dpm_slots_kernel(const float* __restrict__ out_text, const float* __restrict__ out_uncond,
+                                                             float* __restrict__ latents, float* __restrict__ history, const float* __restrict__ noise,
+                                                             const int32_t* __restrict__ lens, const ezb_dpm_slot* __restrict__ slots, int C, int L) {
+  pdl_launch();
+  pdl_wait();
+  const int sample = blockIdx.x / CFG_CLUSTER;
+  const ezb_dpm_slot s = slots[sample];
+  if (!(s.flags & EZB_SLOT_ACTIVE)) return;   // the cluster leaves whole, before any cluster barrier
+  cfg_update_sample<true>(out_text, (s.flags & EZB_SLOT_CFG) ? out_uncond : nullptr, latents, s.coef[6] != 0.f ? noise : nullptr, lens, sample, C, L,
+                          s.guidance_scale, s.guidance_rescale, s.coef[0], s.coef[1], s.coef[2], s.coef[3], s.coef[4], s.coef[5], s.coef[6], history,
+                          (s.flags & EZB_SLOT_ORDER2) != 0);
 }
 
 // Per-sample modulation rows from DEVICE timestep indices (Dit::select_mod): sample b gets row t_index[b] (clamped to [0, n_t)) of the AdaLN

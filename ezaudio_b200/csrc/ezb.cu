@@ -891,6 +891,28 @@ EZB_API int ezb_cfg_ddim_step_slots(int device, const float* model_out, float* l
   return launch_k(cfg_ddim_slots_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, model_out + (size_t)B * C * L,
                   latents, noise, lens, slots, C, L);
 }
+EZB_API int ezb_cfg_dpm_step(int device, const float* model_out, float* latents, float* history, const float* noise, int B, int C, int L, float gs,
+                             float gr, const float* coef, int order, void* stream, const int32_t* lens) {
+  if (!model_out || !latents || !history || !coef || B < 1 || C < 1 || L < 1 || (order != 1 && order != 2))
+    return fail(EZB_ERR_ARG, "ezb_cfg_dpm_step: bad argument");
+  if (coef[6] != 0.f && !noise) return fail(EZB_ERR_ARG, "ezb_cfg_dpm_step: kz != 0 needs a noise tensor");
+  EZB_CUDA(cudaSetDevice(device));
+  ezb_dpm_slot s;
+  s.guidance_scale = gs;
+  s.guidance_rescale = gr;
+  for (int i = 0; i < 7; ++i) s.coef[i] = coef[i];
+  s.flags = EZB_SLOT_ACTIVE | (gs != 0.f ? EZB_SLOT_CFG : 0) | (order == 2 ? EZB_SLOT_ORDER2 : 0);
+  const float* uncond = gs != 0.f ? model_out + (size_t)B * C * L : nullptr;
+  return launch_k(cfg_dpm_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, uncond, latents, history,
+                  coef[6] != 0.f ? noise : (const float*)nullptr, lens, C, L, s);
+}
+EZB_API int ezb_cfg_dpm_step_slots(int device, const float* model_out, float* latents, float* history, const float* noise, const ezb_dpm_slot* slots,
+                                   int B, int C, int L, void* stream, const int32_t* lens) {
+  if (!model_out || !latents || !history || !slots || B < 1 || C < 1 || L < 1) return fail(EZB_ERR_ARG, "ezb_cfg_dpm_step_slots: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  return launch_k(cfg_dpm_slots_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, model_out + (size_t)B * C * L,
+                  latents, history, noise, lens, slots, C, L);
+}
 EZB_API int ezb_vae_create(ezb_vae** out, const ezb_vae_desc* desc, int device) {
   if (!out || !desc) return fail(EZB_ERR_ARG, "ezb_vae_create: null argument");
   EZB_CUDA(cudaSetDevice(device));

@@ -29,7 +29,13 @@ the ControlNet's condition cache (`DiTControlNet.set_condition_rows`); each step
 scales (`DiTControlNet.forward_step(t_index=, scale=)`) before the DiT.  A ControlNet engine serves no edits (the ControlNet API has no
 editing call).  The FP8 mode is not served.
 
-The host logic (admission, schedules, DDIM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots` (`ControlSlots`),
+Built with `schedulers=` listing "dpmsolver++" and / or "sde-dpmsolver++" besides (or instead of) "ddim", the engine also serves requests with
+`scheduler=` one of those (`scheduler.DPMSolverMultistepScheduler`, second order): each step then launches the fused CFG + DPM-Solver++
+update with per-sample constants (ezb_cfg_dpm_step_slots) after the DDIM one, each kernel skipping the other kind's slots, and every slot
+keeps its previous x0 prediction in a history buffer.  Such a request's audio equals `generate_audio` with that scheduler, one prompt and the
+same seed.  The default engine (DDIM only) captures exactly the step graph it always has.
+
+The host logic (admission, schedules, DDIM / DPM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots` (`ControlSlots`),
 which tests replace with a stub."""
 from __future__ import annotations
 
@@ -46,7 +52,7 @@ import torch
 from . import _lib, post
 from .frontend import ControlRequest, EditRequest, Request
 from .inference import scale_shift_re
-from .scheduler import DDIMScheduler
+from .scheduler import DDIMScheduler, DPMSolverMultistepScheduler
 
 MAX_TABLE = 128   # rows of the denoiser's per-timestep LayerNorm tables (csrc/dit.cuh gc_T / fold_T)
 
@@ -58,10 +64,12 @@ class SlotStep:
     frames: int
     guidance_scale: float     # 0 without guidance
     guidance_rescale: float
-    coef: List[float]         # DDIMScheduler.step_coefficients
+    coef: List[float]         # DDIMScheduler.step_coefficients (DPM: DPMSolverMultistepScheduler.step_coefficients)
     cfg: bool
-    draw_noise: bool          # eta > 0: the slot's generator draws this step's (1, C, frames) noise
+    draw_noise: bool          # eta > 0 (DPM: sde-dpmsolver++): the slot's generator draws this step's (1, C, frames) noise
     conditioning_scale: float = 1.0   # ControlNet requests: the factor of the ControlNet skips
+    dpm: bool = False         # the update is DPM-Solver++ (ezb_cfg_dpm_step_slots) rather than DDIM
+    order: int = 1            # DPM: the solver order of this step
 
 
 @dataclasses.dataclass
@@ -70,7 +78,7 @@ class _Active:
     req: object               # Request, EditRequest or ControlRequest
     frames: int
     timesteps: List[int]
-    sched: DDIMScheduler
+    sched: object             # DDIMScheduler or DPMSolverMultistepScheduler
     step: int = 0
 
 
@@ -82,9 +90,13 @@ class ContinuousEngine:
     slots: requests in flight (the denoiser runs 2 * slots samples; ez must have been built with max_batch >= slots).
     max_length_s: the padded clip length (at most ez.max_length_s); longer requests, and edits whose crop is longer, are rejected.
     ControlNet clips are 10 s.
-    ddim_steps: the step counts requests may ask for; the union of their schedules must fit the timestep table."""
+    ddim_steps: the step counts requests may ask for; the union of their schedules must fit the timestep table.
+    schedulers: the samplers requests may ask for (`Request.scheduler`): "ddim", "dpmsolver++", "sde-dpmsolver++"."""
 
-    def __init__(self, ez, slots: int = 4, max_length_s: float = 10.0, ddim_steps: Sequence[int] = (25, 50, 100), *, backend=None):
+    SCHEDULERS = ("ddim", "dpmsolver++", "sde-dpmsolver++")
+
+    def __init__(self, ez, slots: int = 4, max_length_s: float = 10.0, ddim_steps: Sequence[int] = (25, 50, 100),
+                 schedulers: Sequence[str] = ("ddim",), *, backend=None):
         self.control = bool(getattr(backend, "control", False)) if backend is not None else hasattr(ez, "controlnet")
         self.slots = int(slots)
         if self.slots < 1:
@@ -94,13 +106,19 @@ class ContinuousEngine:
         allowed = sorted({int(n) for n in ddim_steps})
         if not allowed or allowed[0] < 1:
             raise ValueError(f"ddim_steps must list positive step counts, got {list(ddim_steps)}")
+        if isinstance(schedulers, str) or not schedulers or any(k not in self.SCHEDULERS for k in schedulers):
+            raise ValueError(f"schedulers must list some of {list(self.SCHEDULERS)}, got {schedulers!r}")
+        self.schedulers = tuple(k for k in self.SCHEDULERS if k in schedulers)
         make = backend.make_scheduler if backend is not None else (lambda: DDIMScheduler(**ez.params["diff"]))
-        self._scheds = {}
-        for n in allowed:
-            s = make()
-            s.set_timesteps(n)
-            self._scheds[n] = s
-        self._timesteps = {n: [int(t) for t in s.timesteps] for n, s in self._scheds.items()}
+        diff = ez.params["diff"] if ez is not None else {}
+        self._scheds = {}   # (scheduler, steps) -> a scheduler set to that many steps
+        for kind in self.schedulers:
+            for n in allowed:
+                s = make() if kind == "ddim" else DPMSolverMultistepScheduler(**diff, algorithm_type=kind)
+                s.set_timesteps(n)
+                self._scheds[kind, n] = s
+        # DPM-Solver++ uses DDIM's trailing timesteps: the table does not grow
+        self._timesteps = {n: [int(t) for t in s.timesteps] for (_, n), s in self._scheds.items()}
         table = sorted({t for ts in self._timesteps.values() for t in ts})
         max_t = backend.max_timesteps if backend is not None else ez.unet._h.desc.max_timesteps
         if len(table) > min(max_t, MAX_TABLE):
@@ -110,7 +128,8 @@ class ContinuousEngine:
         self.table = table
         self._row = {t: i for i, t in enumerate(table)}
         if backend is None:
-            backend = ControlSlots(ez, self.slots, table) if self.control else CudaSlots(ez, self.slots, max_length_s, table)
+            dpm = any(k != "ddim" for k in self.schedulers)
+            backend = ControlSlots(ez, self.slots, table, dpm=dpm) if self.control else CudaSlots(ez, self.slots, max_length_s, table, dpm=dpm)
         self.backend = backend
         self._queue: collections.deque = collections.deque()
         self._active: List[Optional[_Active]] = [None] * self.slots
@@ -127,8 +146,10 @@ class ContinuousEngine:
         return frames
 
     def _check_common(self, r):
-        if not isinstance(r.ddim_steps, numbers.Integral) or isinstance(r.ddim_steps, bool) or int(r.ddim_steps) not in self._scheds:
+        if not isinstance(r.ddim_steps, numbers.Integral) or isinstance(r.ddim_steps, bool) or int(r.ddim_steps) not in self.ddim_steps:
             raise ValueError(f"ddim_steps {r.ddim_steps} is not one of this engine's step counts {list(self.ddim_steps)}")
+        if r.scheduler not in self.schedulers:
+            raise ValueError(f"scheduler {r.scheduler!r} is not one this engine was built with {list(self.schedulers)}")
         s = r.random_seed
         if s is not None and (not isinstance(s, numbers.Integral) or isinstance(s, bool) or not 0 <= int(s) < 2 ** 63):
             raise ValueError(f"random_seed must be None or an integer in [0, 2**63), got {s!r}")
@@ -223,7 +244,7 @@ class ContinuousEngine:
                 else:
                     self.backend.admit(k, r.prompt, seed, frames)
                 n = int(r.ddim_steps)
-                self._active[k] = _Active(t, r, frames, self._timesteps[n], self._scheds[n])
+                self._active[k] = _Active(t, r, frames, self._timesteps[n], self._scheds[r.scheduler, n])
 
     def step(self) -> List[Tuple[int, int, object]]:
         """Admits queued requests into free slots, runs one denoising step of every request in flight and returns (ticket, sample_rate,
@@ -239,8 +260,12 @@ class ContinuousEngine:
             r, t = a.req, a.timesteps[a.step]
             eta = float(r.eta or 0.0)
             cfg = bool(r.guidance_scale) and r.prompt != ""   # "" switches guidance off (api/ezaudio.py:109-111)
-            plan.append(SlotStep(self._row[t], a.frames, float(r.guidance_scale) if cfg else 0.0, float(r.guidance_rescale or 0.0),
-                                 a.sched.step_coefficients(t, eta), cfg, eta > 0, float(r.conditioning_scale) if self.control else 1.0))
+            gs, gr, cs = float(r.guidance_scale) if cfg else 0.0, float(r.guidance_rescale or 0.0), float(r.conditioning_scale) if self.control else 1.0
+            if r.scheduler == "ddim":
+                plan.append(SlotStep(self._row[t], a.frames, gs, gr, a.sched.step_coefficients(t, eta), cfg, eta > 0, cs))
+            else:   # eta is ignored, as generate_audio ignores it with this scheduler
+                coef, order = a.sched.step_coefficients(a.step)
+                plan.append(SlotStep(self._row[t], a.frames, gs, gr, coef, cfg, a.sched.draws_noise, cs, dpm=True, order=order))
         self.backend.step(plan)
         done = []
         for k, a in enumerate(self._active):
@@ -286,7 +311,7 @@ class CudaSlots:
     Between steps the engine owns the denoiser's context and timestep table: a generate_audio call on the same EzAudio replaces them, and the
     next step restores them (set_context of the whole batch, set_timesteps of the table)."""
 
-    def __init__(self, ez, slots: int, max_length_s: float, table: Sequence[int]):
+    def __init__(self, ez, slots: int, max_length_s: float, table: Sequence[int], dpm: bool = False):
         p = ez.params["autoencoder"]
         self.ez, self.unet, self.S, self.table = ez, ez.unet, int(slots), [int(t) for t in table]
         self.sr, self.latent_sr, self.hop = int(p["sr"]), int(p["latent_sr"]), int(ez.autoencoder.decoder.hop)
@@ -307,15 +332,18 @@ class CudaSlots:
         with torch.cuda.device(self.device):
             d = dict(device=self.device, dtype=torch.float32)
             self.lat, self.noise = torch.zeros(S, C, L, **d), torch.zeros(S, C, L, **d)   # padded frames stay zero
+            self.hist = torch.zeros(S, C, L, **d) if dpm else None   # DPM-Solver++ slots: the previous step's x0 prediction
             self.x_in, self.out = torch.zeros(Be, C, L, **d), torch.zeros(Be, C, L, **d)
             self.gt = torch.zeros(Be, C, L, **d)
             self.gt_mask = torch.ones(Be, L, device=self.device, dtype=torch.uint8)   # 1: the DiT regenerates the frame
             # per-step inputs as one int32 block, staged through pinned memory: t_index [Be] | lens [Be] | ezb_ddim_slot [S] (8 words each)
-            words = 2 * Be + 8 * S
+            # [| ezb_dpm_slot [S] (10 words each) when DPM-Solver++ is served]
+            words = 2 * Be + 8 * S + (10 * S if dpm else 0)
             self._h = torch.zeros(words, dtype=torch.int32, pin_memory=True)
             self._d = torch.zeros(words, dtype=torch.int32, device=self.device)
             self._copied = None
-            self.t_index, self.lens, self.slots_dev = self._d[:Be], self._d[Be:2 * Be], self._d[2 * Be:]
+            self.t_index, self.lens, self.slots_dev = self._d[:Be], self._d[Be:2 * Be], self._d[2 * Be:2 * Be + 8 * S]
+            self.dpm_slots_dev = self._d[2 * Be + 8 * S:] if dpm else None
             uemb, umask = ez.encode_text([""])   # the uncond rows: the "" embedding, once
             self.Lc = int(uemb.shape[1])
             self.ctx = uemb.to(**d).expand(Be, -1, -1).contiguous()
@@ -377,9 +405,17 @@ class CudaSlots:
         self.x_in[:S].copy_(self.lat)
         self.x_in[S:].copy_(self.lat)
         self.unet.forward_step(self.x_in, 0, gt=self.gt, gt_mask_u8=self.gt_mask, out=self.out, lengths=self.lens, t_index=self.t_index)
+        self._launch_update(self.lens[:S])
+
+    def _launch_update(self, lens):
+        """The DDIM slots' update, then (when served) the DPM-Solver++ slots' one; each kernel leaves the other kind's slots alone."""
+        S = self.S
         _lib.check(_lib.lib().ezb_cfg_ddim_step_slots(self.device.index, _lib.ptr(self.out), _lib.ptr(self.lat), _lib.ptr(self.noise),
-                                                      _lib.ptr(self.slots_dev), S, self.C, self.max_frames, _lib.stream_ptr(),
-                                                      _lib.ptr(self.lens[:S])))
+                                                      _lib.ptr(self.slots_dev), S, self.C, self.max_frames, _lib.stream_ptr(), _lib.ptr(lens)))
+        if self.hist is not None:
+            _lib.check(_lib.lib().ezb_cfg_dpm_step_slots(self.device.index, _lib.ptr(self.out), _lib.ptr(self.lat), _lib.ptr(self.hist),
+                                                         _lib.ptr(self.noise), _lib.ptr(self.dpm_slots_dev), S, self.C, self.max_frames,
+                                                         _lib.stream_ptr(), _lib.ptr(lens)))
 
     def step(self, plan: Sequence[Optional[SlotStep]]):
         S, Be = self.S, 2 * self.S
@@ -389,9 +425,12 @@ class CudaSlots:
                 self._copied.synchronize()   # the previous step's copy has read the pinned block
             h = self._h.numpy()
             tix, lens = h[:Be], h[Be:2 * Be]
-            words = h[2 * Be:].reshape(S, 8)
+            words = h[2 * Be:2 * Be + 8 * S].reshape(S, 8)
             fl = words.view(np.float32)
+            dwords = h[2 * Be + 8 * S:].reshape(S, 10) if self.hist is not None else None
             for k, e in enumerate(plan):
+                if dwords is not None:
+                    dwords[k] = 0   # inactive for the DPM kernel unless it is a DPM slot
                 if e is None:   # inactive: one frame, no update
                     tix[k] = tix[S + k] = 0
                     lens[k] = lens[S + k] = 1
@@ -399,9 +438,19 @@ class CudaSlots:
                     continue
                 tix[k] = tix[S + k] = e.t_index
                 lens[k] = lens[S + k] = e.frames
-                fl[k, 0], fl[k, 1] = e.guidance_scale, e.guidance_rescale
-                fl[k, 2:7] = e.coef
-                words[k, 7] = _lib.SLOT_ACTIVE | (_lib.SLOT_CFG if e.cfg else 0)
+                flags = _lib.SLOT_ACTIVE | (_lib.SLOT_CFG if e.cfg else 0)
+                if e.dpm:
+                    if dwords is None:
+                        raise RuntimeError("a DPM-Solver++ step on slots built without DPM-Solver++")
+                    words[k] = 0   # inactive for the DDIM kernel
+                    dfl = dwords.view(np.float32)
+                    dfl[k, 0], dfl[k, 1] = e.guidance_scale, e.guidance_rescale
+                    dfl[k, 2:9] = e.coef
+                    dwords[k, 9] = flags | (_lib.SLOT_ORDER2 if e.order == 2 else 0)
+                else:
+                    fl[k, 0], fl[k, 1] = e.guidance_scale, e.guidance_rescale
+                    fl[k, 2:7] = e.coef
+                    words[k, 7] = flags
                 if e.draw_noise:   # the draw a solo run makes at this step: a contiguous (1, C, frames) tensor from the slot's generator
                     self.noise[k, :, :e.frames] = torch.empty((1, self.C, e.frames), device=self.device).normal_(generator=self.gens[k])[0]
             self._d.copy_(self._h, non_blocking=True)
@@ -456,8 +505,8 @@ class ControlSlots(CudaSlots):
     generate_audio call replaced."""
     control = True
 
-    def __init__(self, ez, slots: int, table: Sequence[int]):
-        super().__init__(ez, slots, 10.0, table)
+    def __init__(self, ez, slots: int, table: Sequence[int], dpm: bool = False):
+        super().__init__(ez, slots, 10.0, table, dpm=dpm)
         self.cn = ez.controlnet
         p = ez.params["autoencoder"]
         self.num_samples = int(10 * self.sr)
@@ -503,8 +552,7 @@ class ControlSlots(CudaSlots):
         self.x_in[S:].copy_(self.lat)
         sk = self.cn.forward_step(self.x_in, t_index=self.t_index, scale=self.scale, outs=self.skips)
         self.unet.forward_step(self.x_in, 0, controlnet_skips=sk, out=self.out, t_index=self.t_index)
-        _lib.check(_lib.lib().ezb_cfg_ddim_step_slots(self.device.index, _lib.ptr(self.out), _lib.ptr(self.lat), _lib.ptr(self.noise),
-                                                      _lib.ptr(self.slots_dev), S, self.C, self.max_frames, _lib.stream_ptr(), None))
+        self._launch_update(None)
 
     def step(self, plan: Sequence[Optional[SlotStep]]):
         with torch.cuda.device(self.device):

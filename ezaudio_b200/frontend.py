@@ -31,6 +31,7 @@ class Request:
     ddim_steps: int = 100
     eta: float = 1
     random_seed: Optional[int] = None
+    scheduler: str = "ddim"   # the continuous engine also serves "dpmsolver++" / "sde-dpmsolver++" when built with them (eta is then ignored)
 
     def group_key(self, length_bucket_s: Optional[float] = None) -> Tuple:
         # "" switches guidance off for the whole call (api/ezaudio.py:109-111): empty prompts only batch with empty prompts
@@ -53,6 +54,11 @@ class ControlRequest:
     eta: float = 1
     conditioning_scale: float = 1
     random_seed: Optional[int] = None
+    # as Request.scheduler; an init-only argument, so that the fields stay one per argument of EzAudio_ControlNet.generate_audio
+    scheduler: dataclasses.InitVar[str] = "ddim"
+
+    def __post_init__(self, scheduler):
+        object.__setattr__(self, "scheduler", scheduler)
 
 
 @dataclasses.dataclass(frozen=True)
@@ -70,6 +76,11 @@ class EditRequest:
     ddim_steps: int = 100
     eta: float = 1
     random_seed: Optional[int] = None
+    # as Request.scheduler; an init-only argument, so that the fields stay one per argument of EzAudio.editing_audio
+    scheduler: dataclasses.InitVar[str] = "ddim"
+
+    def __post_init__(self, scheduler):
+        object.__setattr__(self, "scheduler", scheduler)
 
 
 def length_bucket_bin(length: float, length_bucket_s: float) -> int:
@@ -118,9 +129,16 @@ class BatchingFrontEnd:
         self.length_bucket_s = length_bucket_s
         self._queue: List[Request] = []
 
+    @staticmethod
+    def _check(r: Request) -> Request:
+        if r.scheduler != "ddim":
+            raise ValueError(f"the batching front-end runs DDIM only, got scheduler={r.scheduler!r}; serve DPM-Solver++ requests with "
+                             "engine.ContinuousEngine(schedulers=...) or set EzAudio.noise_scheduler")
+        return r
+
     def submit(self, prompt: str, **kw) -> int:
-        """Queues a request; returns its ticket (index in submission order)."""
-        self._queue.append(Request(prompt, **kw))
+        """Queues a request; returns its ticket (index in submission order).  Requests for another scheduler than DDIM raise ValueError."""
+        self._queue.append(self._check(Request(prompt, **kw)))
         return len(self._queue) - 1
 
     def _run_batch(self, b: Batch):
@@ -143,7 +161,7 @@ class BatchingFrontEnd:
 
     def stream(self, requests: Optional[Iterable[Request]] = None) -> Iterator[Tuple[int, int, object]]:
         """Yields (ticket, sample_rate, waveform) batch by batch, as soon as each batch of THIS rank has finished."""
-        reqs = list(requests) if requests is not None else self._queue
+        reqs = [self._check(r) for r in requests] if requests is not None else self._queue
         if requests is None:
             self._queue = []
         for b in batches_of_rank(plan_batches(reqs, self.max_batch, self.length_bucket_s), self.world, self.rank):

@@ -4,7 +4,8 @@ Differences from the reference loop, all additive:
   * batched prompts (the reference hard-codes batch 1, src/inference.py:67; SURVEY 0.8): prompt i gets its own
     torch.Generator(seed + i), so prompt 0 of a batch reproduces the reference's B=1 run with the same seed;
   * step-invariant work (context embedding, cross-attention K/V, timestep/AdaLN tables) is computed once per clip;
-  * CFG + rescale + DDIM update is one fused kernel (ezb_cfg_ddim_step);
+  * CFG + rescale + DDIM update is one fused kernel (ezb_cfg_ddim_step); so is CFG + rescale + DPM-Solver++ (ezb_cfg_dpm_step) when the
+    scheduler is a `scheduler.DPMSolverMultistepScheduler` -- the swap a diffusers user makes with `noise_scheduler`; eta is then ignored;
   * clips of different lengths in one batch (`lengths=`): the batch is padded to `audio_frames` and every prompt's frames come out as
     that prompt run alone at its own length computes them (same seed, same bits); one length-aware VAE decode turns the padded batch into
     waveforms.  Inpainting joins in with `padded_gt=True`: gt / gt_mask padded like the batch, ignored past each clip's end.
@@ -42,6 +43,12 @@ def _ddim_step(model_out, latents, noise, B, Cc, L, gs, gr, coef, lens=None):
     arr = (C.c_float * 5)(*coef)
     _lib.check(_lib.lib().ezb_cfg_ddim_step(latents.device.index, _lib.ptr(model_out), _lib.ptr(latents), _lib.ptr(noise), B, Cc, L, float(gs or 0.0), float(gr or 0.0),
                                             arr, _lib.stream_ptr(), _lib.ptr(lens)))
+
+
+def _dpm_step(model_out, latents, history, noise, B, Cc, L, gs, gr, coef, order, lens=None):
+    arr = (C.c_float * 7)(*coef)
+    _lib.check(_lib.lib().ezb_cfg_dpm_step(latents.device.index, _lib.ptr(model_out), _lib.ptr(latents), _lib.ptr(history), _lib.ptr(noise), B, Cc, L,
+                                           float(gs or 0.0), float(gr or 0.0), arr, int(order), _lib.stream_ptr(), _lib.ptr(lens)))
 
 
 def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None, padded_gt=False):
@@ -114,6 +121,7 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
     Cc = unet.cfg["out_chans"]
     L = int(audio_frames)
     use_cfg = bool(guidance_scale)
+    dpm = getattr(noise_scheduler, "kind", "ddim") == "dpm"   # DPM-Solver++: multistep, keeps the previous x0 prediction per sample
     noise_scheduler.set_timesteps(ddim_steps)
     timesteps = [int(t) for t in noise_scheduler.timesteps]
 
@@ -171,14 +179,17 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         skips = [torch.empty(Be, L, unet.cfg["embed_dim"], device=device, dtype=torch.float32) for _ in range(controlnet.half)]
 
     # ---- the loop.  Every step is the same launch sequence on static buffers, so the WHOLE schedule (all steps: ~365 kernels each) is captured
-    # once into one CUDA graph per shape / schedule and replayed with a single launch; the per-step Gaussian draws of DDIM (eta > 0) stay in
+    # once into one CUDA graph per shape / schedule and replayed with a single launch; the per-step Gaussian draws of DDIM (eta > 0; and of
+    # sde-dpmsolver++) stay in
     # PyTorch -- same generators, same order, same per-step tensor shapes as the step-by-step loop -- and are simply made up front into one
     # [steps, B, C, L] buffer (one graph per step would interleave 50 launches and 200 RNG kernels).
     # Everything a captured launch sequence bakes in is in the key: shapes (incl. the context length, which fixes the cross-attention K/V layout and
     # tensor maps), the schedule, the guidance constants, which ControlNet handle (its serial, not id(): ids are recycled) and the
     # library's option epoch (ezb_set_option changes kernel selection).
     nsteps = len(timesteps)
-    key = (B, Be, L, lengths is not None, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), float(eta or 0.0),
+    draw = noise_scheduler.draws_noise if dpm else bool(eta and eta > 0)
+    sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
+    key = (B, Be, L, lengths is not None, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
            gt is not None, controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()))
     cache = unet.__dict__.setdefault("_loop_cache", {})
     st = cache.get(key) if use_graphs else None
@@ -186,7 +197,8 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         st = dict(lat=torch.empty(B, Cc, L, device=device, dtype=torch.float32),
                   x_in=torch.empty(Be, Cc, L, device=device, dtype=torch.float32) if use_cfg else None,
                   out=torch.empty(Be, Cc, L, device=device, dtype=torch.float32),
-                  noise=torch.empty(nsteps, B, Cc, L, device=device, dtype=torch.float32) if (eta and eta > 0) else None,
+                  noise=torch.empty(nsteps, B, Cc, L, device=device, dtype=torch.float32) if draw else None,
+                  hist=torch.empty(B, Cc, L, device=device, dtype=torch.float32) if dpm else None,   # the previous step's x0 prediction
                   gt=None if gt_c is None else torch.empty_like(gt_c), m8=None if m8 is None else torch.empty_like(m8),
                   cond=None, skips=None, graph=None, launches=0,
                   lens=torch.empty(Be, device=device, dtype=torch.int32) if lengths is not None else None)   # [lengths | lengths] under CFG
@@ -220,6 +232,9 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
                 for b, g in enumerate(gens):
                     noise_all[i, b, :, :lengths[b]] = torch.empty((1, Cc, lengths[b]), device=device).normal_(generator=g)[0]
 
+    # DPM-Solver++: every step's coefficients and order, computed once, before any capture
+    dpm_coef = [noise_scheduler.step_coefficients(i) for i in range(nsteps)] if dpm else None
+
     def one_step(i, t):
         if use_cfg:
             x_in[:B].copy_(lat)
@@ -231,6 +246,11 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         if controlnet is not None:
             sk = controlnet.forward_step(xi, i, st["cond"], conditioning_scale, gt=st["gt"], gt_mask_u8=st["m8"], outs=st["skips"])
         unet.forward_step(xi, i, gt=st["gt"], gt_mask_u8=st["m8"], controlnet_skips=sk, out=out, lengths=lens)
+        if dpm:
+            coef, order = dpm_coef[i]
+            _dpm_step(out, lat, st["hist"], None if noise_all is None else noise_all[i], B, Cc, L, guidance_scale if use_cfg else 0.0, guidance_rescale,
+                      coef, order, None if lens is None else lens[:B])
+            return
         coef = noise_scheduler.step_coefficients(t, float(eta or 0.0))
         _ddim_step(out, lat, None if noise_all is None else noise_all[i], B, Cc, L, guidance_scale if use_cfg else 0.0, guidance_rescale, coef,
                    None if lens is None else lens[:B])

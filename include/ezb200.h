@@ -9,7 +9,7 @@
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
  * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev,
- * cfg_ddim_step, cfg_ddim_step_slots, decode, encode, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
+ * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, decode, encode, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
  */
@@ -134,6 +134,29 @@ typedef struct {
 enum { EZB_SLOT_ACTIVE = 1, EZB_SLOT_CFG = 2 };
 int ezb_cfg_ddim_step_slots(int device, const float* model_out, float* latents, const float* noise, const ezb_ddim_slot* slots_dev, int B,
                             int C, int L, void* stream, const int32_t* lens);
+
+/* --- fused classifier-free guidance + rescale + DPM-Solver++ multistep update (diffusers DPMSolverMultistepScheduler.step restated for
+ * dpmsolver++ / sde-dpmsolver++, midpoint; ezaudio_b200/scheduler.py).  Guidance, rescale, model_out, lens and `device` as in
+ * ezb_cfg_ddim_step: the same reduction, element order and padded frames left untouched.  coef = {alpha_s, sigma_s, kx, k0, k1, r, kz};
+ * with v the guided output, each element computes m0 = alpha_s x - sigma_s v and x <- kx x + k0 m0 + k1 (r (m0 - m1)) + kz z.
+ * history (B,C,L) fp32 holds m1, the previous step's m0: it is read only at order 2 (order 1 drops the k1 term), and this step's m0 is
+ * written into it.  noise (B,C,L) is read only when kz != 0 and may be NULL otherwise.  latents updated in place. */
+int ezb_cfg_dpm_step(int device, const float* model_out, float* latents, float* history, const float* noise, int B, int C, int L,
+                     float guidance_scale, float guidance_rescale, const float* coef7_host, int order, void* stream, const int32_t* lens);
+/* ezb_cfg_dpm_step with the constants of each sample in a DEVICE array slots_dev[B], read when the kernel runs, as ezb_cfg_ddim_step_slots:
+ * model_out always holds B text rows followed by B uncond rows; a sample with flags & EZB_SLOT_ACTIVE is updated as ezb_cfg_dpm_step on that
+ * sample alone (order 2 when flags & EZB_SLOT_ORDER2) computes it, bit for bit; an inactive sample's latents and history are not touched.
+ * noise is read only by samples whose kz (coef[6]) is non-zero; checking that it is there, and validating lens, is the caller's job.
+ * A batch whose samples run different samplers launches ezb_cfg_ddim_step_slots and this call on the same buffers, each with the other
+ * kind's slots inactive. */
+typedef struct {
+  float guidance_scale, guidance_rescale;
+  float coef[7];   /* as coef7_host of ezb_cfg_dpm_step */
+  int32_t flags;   /* EZB_SLOT_ACTIVE | EZB_SLOT_CFG | EZB_SLOT_ORDER2 */
+} ezb_dpm_slot;
+enum { EZB_SLOT_ORDER2 = 4 };
+int ezb_cfg_dpm_step_slots(int device, const float* model_out, float* latents, float* history, const float* noise, const ezb_dpm_slot* slots_dev,
+                           int B, int C, int L, void* stream, const int32_t* lens);
 
 /* --- VAE decoder: OobleckDecoder.forward (stable_vae/models/autoencoders.py:149-190) behind
  * Autoencoder(embedding=z) (src/modules/autoencoder_wrapper.py:74-77). */
