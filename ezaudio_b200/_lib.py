@@ -145,6 +145,7 @@ _SIGS = {
     "ezb_vae_encode": ([_VP, _VP, _VP, _VP, _I, _I, _VP], _I),
     "ezb_vae_decode_lens": ([_VP, _VP, _VP, _I, _I, _VP, _VP], _I),
     "ezb_vae_encode_lens": ([_VP, _VP, _VP, _VP, _I, _I, _VP, _VP], _I),
+    "ezb_vae_encode_noised": ([_VP, _VP, _VP, _VP, _VP, _F, _F, _VP, _I, _I, _VP, _VP], _I),
     "ezb_t5_create": ([C.POINTER(_VP), C.POINTER(T5Desc), _I], _I),
     "ezb_t5_destroy": ([_VP], _I),
     "ezb_t5_load_weight": ([_VP, C.c_char_p, _VP, C.POINTER(C.c_int64), _I, _VP], _I),

@@ -19,8 +19,8 @@ import torch
 from . import _lib, config, post, weights
 from ._lib import EzbError
 from .dit import DiTControlNet, MaskDiT
-from .inference import inference
-from .scheduler import DDIMScheduler
+from .inference import inference, make_generators
+from .scheduler import DDIMScheduler, start_index
 from .vae import Autoencoder, OobleckDecoder
 
 MAX_SEED = np.iinfo(np.int32).max
@@ -390,6 +390,84 @@ class EzAudio(_Base):
             post.splice_wave(o, w[0], p["s0"], p["n_paste"])
         return sr, [o.cpu().numpy() for o in outs]
 
+    def variation_audio(self, text, init_audio, strength=0.8, guidance_scale=5, guidance_rescale=0.75, ddim_steps=100, eta=1, random_seed=None,
+                        randomize_seed=False, *, pad_length=None):
+        """Audio-to-audio variation (SDEdit; diffusers' img2img, Stable Audio's init_audio): `init_audio` (a WAV path or a float32 mono
+        waveform at the model's rate) is peak-normalised, zero-padded to a whole hop, VAE-encoded and noised to the schedule index
+        `scheduler.start_index(ddim_steps, strength)`; the last int(ddim_steps * strength) steps then denoise it with `text`.  strength 1
+        starts from pure noise (with DDIM the result is then generate_audio's, bit for bit, for the same prompt, seed and frame count);
+        smaller strengths keep more of the clip.  Returns (sr, float32 waveform) of the clip's length in samples.
+        Prompt b's generator (random_seed as in generate_audio) draws its start noise (1, C, frames) first, then the noise of the steps it
+        runs; the VAE bottleneck noise comes from the global RNG in clip order, as in editing_audio.
+        With a list of prompts, `init_audio`, `strength` and `random_seed` list one value per prompt (a scalar applies to all) and the call
+        returns (sr, [waveforms]): one VAE encode, one sampling loop and one decode, the batch padded to the longest clip or to `pad_length`
+        seconds (at most max_length_s).  Each waveform equals the scalar call with its seed, the calls made in list order."""
+        if isinstance(text, (list, tuple)):
+            return self._variation(list(text), True, init_audio, strength, guidance_scale, guidance_rescale, ddim_steps, eta, random_seed,
+                                   randomize_seed, pad_length)
+        if pad_length is not None:
+            raise ValueError("pad_length applies to a list of variations")
+        return self._variation([text], False, [init_audio], [strength], guidance_scale, guidance_rescale, ddim_steps, eta, random_seed,
+                               randomize_seed, None)
+
+    def _variation(self, prompts, batched, init_audio, strength, guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, randomize_seed,
+                   pad_length):
+        sr, latent_sr = self.params["autoencoder"]["sr"], self.params["autoencoder"]["latent_sr"]
+        dec = self.autoencoder.decoder
+        B, hop = len(prompts), dec.hop
+        # ---- everything is checked on the host before any device work
+        if B < 1 or B > dec.max_batch:
+            raise ValueError(f"{B} variations in one call: 1..{dec.max_batch} (max_batch) fit the workspace")
+        num = (int, float, np.integer, np.floating)
+        files = _per_clip("init_audio", init_audio, B, (str, np.ndarray))
+        strengths = _per_clip("strength", strength, B, num)
+        if randomize_seed:
+            seeds = [random.randint(0, MAX_SEED) for _ in range(B)]
+        elif random_seed is None or isinstance(random_seed, num):
+            seeds = random_seed   # an int: prompt b draws from Generator(seed + b), as in generate_audio
+        else:
+            seeds = [int(v) for v in _per_clip("random_seed", random_seed, B, num)]
+        empty = [t == "" for t in prompts]
+        if any(empty) and not all(empty):
+            raise ValueError("empty prompts run without guidance: they cannot share a batch with non-empty ones")
+        if all(empty):
+            guidance_scale = None
+            print("empyt input")
+        starts = [start_index(ddim_steps, v) for v in strengths]
+        raws = [_load_audio(f, sr) if isinstance(f, str) else np.asarray(f, dtype=np.float32) for f in files]
+        if any(r.ndim != 1 or len(r) < 1 or not np.isfinite(r).all() for r in raws):
+            raise ValueError("every init_audio must be a non-empty, finite mono waveform")
+        frames = [-(-len(r) // hop) for r in raws]
+        max_frames = int(round(self.max_length_s * latent_sr))
+        if pad_length is not None and pad_length > self.max_length_s:
+            raise ValueError(f"pad_length {pad_length} s exceeds max_length_s {self.max_length_s} s")
+        L = max(frames) if pad_length is None else int(pad_length * latent_sr)
+        if max(frames) > L or L > max_frames:
+            raise ValueError(f"clips of {frames} latent frames must fit the padded length ({L} frames, at most {max_frames}: "
+                             f"max_length_s {self.max_length_s} s)")
+        sched = self.noise_scheduler
+        sched.set_timesteps(ddim_steps)
+        ab = [sched.add_noise_coefficients(int(sched.timesteps[k])) for k in starts]
+        # ---- per clip: normalise + pad on the device into the padded batch; then the start noise, one fused encode + add_noise
+        clips = torch.zeros(B, 1, L * hop, device=self.device)
+        for b, r in enumerate(raws):
+            clips[b, 0, :frames[b] * hop] = post.prepare_wave(torch.from_numpy(r).to(self.device).unsqueeze(0), frames[b] * hop, normalize=True)[0]
+        gens = make_generators(seeds, B, self.device)
+        C = self.unet.cfg["out_chans"]
+        eps = torch.zeros(B, C, L, device=self.device)
+        for b, g in enumerate(gens):   # generate_audio's initial draw, at the clip's own shape
+            eps[b, :, :frames[b]] = torch.randn((1, C, frames[b]), generator=g, device=self.device)[0]
+        lengths = frames if batched else None
+        p = self.params["autoencoder"]
+        x_t = dec.encode_noised(clips, ab, eps, p["scale"], p["shift"], lengths=lengths)   # bottleneck noise: global RNG, clip order
+        embeds = self._text_embeds(prompts, [""])
+        pred = inference(self.autoencoder, self.unet, None, None, None, None, self.params, sched, prompts, None, L, guidance_scale,
+                         guidance_rescale, ddim_steps, eta, None, self.device, text_embeds=embeds, lengths=lengths, start_index=starts,
+                         init_latents=x_t, generators=gens)
+        if not batched:
+            return sr, pred[0, 0, :len(raws[0])].cpu().numpy()
+        return sr, [w[0, :len(r)].cpu().numpy() for w, r in zip(pred, raws)]
+
 
 def energy_condition(audio: torch.Tensor, hop_size=240, window_size=1920, padding="reflect", min_db=-60, norm=True, quantize_levels=None,
                      **unused):
@@ -408,7 +486,8 @@ def energy_condition(audio: torch.Tensor, hop_size=240, window_size=1920, paddin
 
 
 class EzAudio_ControlNet(_Base):
-    """api/controlnet.py:31.  precision as for EzAudio ("fp8" applies to the DiT and the ControlNet)."""
+    """api/controlnet.py:31.  precision as for EzAudio ("fp8" applies to the DiT and the ControlNet).  It has no audio-to-audio variation
+    call: a variation starts from its own clip, a ControlNet call from the reference clip's energy; use EzAudio.variation_audio."""
 
     def __init__(self, model_name, ckpt_path=None, controlnet_path=None, vae_path=None, device="cuda", *,
                  text_encoder: Optional[Callable] = None, precision: str = "bf16", max_batch: int = 4, config_path=None,

@@ -1019,6 +1019,12 @@ EZB_API int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noi
   if (!h || !audio || !z || !lens) return fail(EZB_ERR_ARG, "ezb_vae_encode_lens: null argument");
   return reinterpret_cast<Vae*>(h)->encode(audio, noise, z, B, T, ST(stream), lens);
 }
+EZB_API int ezb_vae_encode_noised(ezb_vae* h, const float* audio, const float* vae_noise, const float* eps, const float* ab_dev, float scale,
+                                  float shift, float* x_t, int B, int T, const int32_t* lens, void* stream) {
+  if (!h || !audio || !eps || !ab_dev || !x_t) return fail(EZB_ERR_ARG, "ezb_vae_encode_noised: null argument");
+  const VaeNoised nd{eps, ab_dev, scale, shift};
+  return reinterpret_cast<Vae*>(h)->encode(audio, vae_noise, x_t, B, T, ST(stream), lens, &nd);
+}
 }  // extern "C"
 
 namespace {

@@ -10,6 +10,7 @@
 
 #include "elementwise.cuh"
 #include "host.cuh"
+#include "vae_noised.cuh"
 
 namespace ezb {
 
@@ -245,7 +246,6 @@ __global__ void vae_sample_lens_kernel(const float* __restrict__ enc, const floa
                                        const int32_t* __restrict__ lens) {
   vae_sample_body<true>(enc, noise, z, Cz, L, lens);
 }
-
 struct VaeConv {  // one packed conv / conv-transpose
   __nv_bfloat16* w = nullptr;
   const float* bias = nullptr;
@@ -397,6 +397,13 @@ inline int vae_sample(cudaStream_t st, const float* enc, const float* noise, flo
   if (lens != nullptr) vae_sample_lens_kernel<<<g2, 256, 0, st>>>(enc, noise, z, Cz, L, lens);
   else vae_sample_kernel<<<g2, 256, 0, st>>>(enc, noise, z, Cz, L);
   EZB_CUDA(cudaGetLastError());
+  return EZB_OK;
+}
+// enc [B*L, 2*Cz] (mean | scale), eps (B, Cz, L), ab [B][2] -> x_t (B, Cz, L): vae_sample_noised_kernel (vae_noised.cu)
+inline int vae_sample_noised(cudaStream_t st, const float* enc, const float* noise, const VaeNoised& n, float* x_t, int B, int Cz, int L,
+                             const int32_t* lens) {
+  ++launch_counter();
+  EZB_CUDA(vae_sample_noised_launch(st, enc, noise, n, x_t, B, Cz, L, lens));
   return EZB_OK;
 }
 
@@ -615,7 +622,9 @@ struct Vae {
   // audio (B, 1, T) fp32, T = hop * L; noise (B, latent, L) fp32 or null (-> mean); z (B, latent, L) fp32.
   // lens_ (device [B] latent frames, or null): clip b is its first hop * lens_[b] samples; its z frames come out as an encode of the
   // clip alone at that length, the frames past it as zeros, whatever audio and noise hold past the end.
-  int encode(const float* audio, const float* noise, float* z, int B, int T, cudaStream_t st, const int32_t* lens_ = nullptr) {
+  // noised (or null): z receives the start latent of a variation instead (vae_sample_noised_kernel).
+  int encode(const float* audio, const float* noise, float* z, int B, int T, cudaStream_t st, const int32_t* lens_ = nullptr,
+             const VaeNoised* noised = nullptr) {
     if (!finalized || !d.with_encoder) return fail(EZB_ERR_STATE, "VAE encoder weights not loaded");
     int hop = 1;
     for (int j = 0; j < nst; ++j) hop *= e_stride[j];
@@ -641,6 +650,7 @@ struct Vae {
       std::swap(cur, oth);
     }
     EZB_TRY(run_conv(st, e_out, cur, B, Tc, nullptr, resid, nullptr, nullptr));  // (mean | scale), channels-last fp32
+    if (noised != nullptr) return vae_sample_noised(st, resid, noise, *noised, z, B, d.latent_dim, L, lens);
     return vae_sample(st, resid, noise, z, B, d.latent_dim, L, lens);
   }
 

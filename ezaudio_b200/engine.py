@@ -35,6 +35,13 @@ update with per-sample constants (ezb_cfg_dpm_step_slots) after the DDIM one, ea
 keeps its previous x0 prediction in a history buffer.  Such a request's audio equals `generate_audio` with that scheduler, one prompt and the
 same seed.  The default engine (DDIM only) captures exactly the step graph it always has.
 
+The same engine serves audio-to-audio variations (`frontend.VariationRequest`), with the semantics of `EzAudio.variation_audio` for one
+clip.  Admitting one draws its start noise from the slot's generator (the draw a text-to-audio request makes), peak-normalises and pads
+its clip on the device and encodes it alone straight into the noised start latent of slot k's row (`OobleckDecoder.encode_noised`, at the
+request's start timestep; the bottleneck noise comes from the global torch RNG at admission, as for an edit); its schedule then begins at
+`scheduler.start_index(ddim_steps, strength)`, with DPM-Solver++ taking that step at order 1.  Its inpainting rows and mask bytes are a
+text-to-audio slot's, so the step graph does not change.
+
 The host logic (admission, schedules, DDIM / DPM coefficients, tickets) is `ContinuousEngine`; the device work is `CudaSlots` (`ControlSlots`),
 which tests replace with a stub."""
 from __future__ import annotations
@@ -50,9 +57,9 @@ import numpy as np
 import torch
 
 from . import _lib, post
-from .frontend import ControlRequest, EditRequest, Request
+from .frontend import ControlRequest, EditRequest, Request, VariationRequest
 from .inference import scale_shift_re
-from .scheduler import DDIMScheduler, DPMSolverMultistepScheduler
+from .scheduler import DDIMScheduler, DPMSolverMultistepScheduler, start_index
 
 MAX_TABLE = 128   # rows of the denoiser's per-timestep LayerNorm tables (csrc/dit.cuh gc_T / fold_T)
 
@@ -75,11 +82,12 @@ class SlotStep:
 @dataclasses.dataclass
 class _Active:
     ticket: int
-    req: object               # Request, EditRequest or ControlRequest
+    req: object               # Request, EditRequest, VariationRequest or ControlRequest
     frames: int
     timesteps: List[int]
     sched: object             # DDIMScheduler or DPMSolverMultistepScheduler
     step: int = 0
+    begin: int = 0            # the first step of the schedule it runs (a variation's start index)
 
 
 class ContinuousEngine:
@@ -203,12 +211,27 @@ class ContinuousEngine:
             raise ValueError(f"the edit's crop is {plan['frames']} frames; this engine serves 1..{self.backend.max_frames}")
         return plan["frames"], (wave, plan)
 
+    def _variation(self, r: VariationRequest) -> Tuple[int, Tuple[np.ndarray, int]]:
+        """Checks a variation and loads its clip (host only); returns (clip frames, (clip, start index))."""
+        self._check_common(r)
+        v = r.strength
+        if not isinstance(v, numbers.Real) or isinstance(v, bool) or not math.isfinite(v):
+            raise ValueError(f"strength must be a finite number, got {v!r}")
+        k = start_index(int(r.ddim_steps), v)
+        wave = self._read_clip(r.init_audio, "clip to vary")
+        frames = -(-len(wave) // self.backend.hop)
+        if not 1 <= frames <= self.backend.max_frames:
+            raise ValueError(f"the clip is {frames} frames; this engine serves 1..{self.backend.max_frames}")
+        return frames, (wave, k)
+
     def submit(self, prompt: str, **kw) -> int:
-        """Queues a request and returns its ticket: an edit (the keyword arguments of `frontend.EditRequest`) when `gt_file` is given,
-        otherwise a `frontend.Request`, or a `frontend.ControlRequest` for a ControlNet engine.  Invalid requests raise ValueError here,
-        before any device work; a clip given as a path is read here."""
+        """Queues a request and returns its ticket: an edit (the keyword arguments of `frontend.EditRequest`) when `gt_file` is given, a
+        variation (`frontend.VariationRequest`) when `init_audio` is, otherwise a `frontend.Request`, or a `frontend.ControlRequest` for a
+        ControlNet engine.  Invalid requests raise ValueError here, before any device work; a clip given as a path is read here."""
         if "gt_file" in kw:
             return self._enqueue(EditRequest(prompt, **kw))
+        if "init_audio" in kw:
+            return self._enqueue(VariationRequest(prompt, **kw))
         return self._enqueue(ControlRequest(prompt, **kw) if self.control else Request(prompt, **kw))
 
     def _enqueue(self, r) -> int:
@@ -216,6 +239,10 @@ class ContinuousEngine:
             if self.control:
                 raise ValueError("a ControlNet engine serves no edits (EzAudio_ControlNet has no editing call)")
             item = (r,) + self._edit(r)
+        elif isinstance(r, VariationRequest):
+            if self.control:
+                raise ValueError("a ControlNet engine serves no variations (EzAudio_ControlNet has no variation call)")
+            item = (r,) + self._variation(r)
         elif isinstance(r, ControlRequest) and self.control:
             item = (r, self.backend.max_frames, self._control_wave(r))
         elif isinstance(r, Request) and not self.control:
@@ -237,14 +264,19 @@ class ContinuousEngine:
             if self._active[k] is None and self._queue:
                 t, r, frames, extra = self._queue.popleft()
                 seed = None if r.random_seed is None else int(r.random_seed)
+                n, begin = int(r.ddim_steps), 0
+                sched = self._scheds[r.scheduler, n]
                 if self.control:
                     self.backend.admit(k, r.prompt, seed, frames, audio=extra, surpass_noise=float(r.surpass_noise))
                 elif isinstance(r, EditRequest):
                     self.backend.admit(k, r.prompt, seed, frames, edit=extra)
+                elif isinstance(r, VariationRequest):
+                    wave, begin = extra
+                    ab = sched.add_noise_coefficients(self._timesteps[n][begin])
+                    self.backend.admit(k, r.prompt, seed, frames, variation=(wave, ab))
                 else:
                     self.backend.admit(k, r.prompt, seed, frames)
-                n = int(r.ddim_steps)
-                self._active[k] = _Active(t, r, frames, self._timesteps[n], self._scheds[r.scheduler, n])
+                self._active[k] = _Active(t, r, frames, self._timesteps[n], sched, step=begin, begin=begin)
 
     def step(self) -> List[Tuple[int, int, object]]:
         """Admits queued requests into free slots, runs one denoising step of every request in flight and returns (ticket, sample_rate,
@@ -264,7 +296,7 @@ class ContinuousEngine:
             if r.scheduler == "ddim":
                 plan.append(SlotStep(self._row[t], a.frames, gs, gr, a.sched.step_coefficients(t, eta), cfg, eta > 0, cs))
             else:   # eta is ignored, as generate_audio ignores it with this scheduler
-                coef, order = a.sched.step_coefficients(a.step)
+                coef, order = a.sched.step_coefficients(a.step, begin_index=a.begin)
                 plan.append(SlotStep(self._row[t], a.frames, gs, gr, coef, cfg, a.sched.draws_noise, cs, dpm=True, order=order))
         self.backend.step(plan)
         done = []
@@ -279,7 +311,7 @@ class ContinuousEngine:
         return done
 
     def stream(self, requests: Optional[Iterable[object]] = None) -> Iterator[Tuple[int, int, object]]:
-        """Submits `requests` (if given: Request / EditRequest objects, or ControlRequest objects for a ControlNet engine) and yields
+        """Submits `requests` (if given: Request / EditRequest / VariationRequest objects, or ControlRequest objects for a ControlNet engine) and yields
         (ticket, sample_rate, waveform) in completion order until nothing is queued or in flight."""
         if requests is not None:
             for r in requests:
@@ -350,6 +382,7 @@ class CudaSlots:
             self.cmask = umask.to(self.device).bool().expand(Be, -1).contiguous()
         self.gens: List[Optional[torch.Generator]] = [None] * S
         self.edits: List[Optional[Tuple[torch.Tensor, int, int]]] = [None] * S   # an edit's (normalised clip, s0, n_paste)
+        self.trim: List[Optional[int]] = [None] * S   # a variation's clip length in samples
         self.graph, self._key, self._launches = None, None, 0
         self.captures = 0   # step graphs captured so far
         self._ctx_epoch = None
@@ -362,8 +395,10 @@ class CudaSlots:
             self.unet.set_context(self.ctx, self.cmask)
             self._ctx_epoch = h.ctx_epoch
 
-    def admit(self, k: int, prompt: str, seed: Optional[int], frames: int, edit: Optional[Tuple[np.ndarray, dict]] = None):
-        """Starts slot k.  `edit`: (clip, api.edit_plan of the edit) for an edit, whose crop is `frames` latent frames long."""
+    def admit(self, k: int, prompt: str, seed: Optional[int], frames: int, edit: Optional[Tuple[np.ndarray, dict]] = None,
+              variation: Optional[Tuple[np.ndarray, Tuple[float, float]]] = None):
+        """Starts slot k.  `edit`: (clip, api.edit_plan of the edit) for an edit, whose crop is `frames` latent frames long.  `variation`:
+        (clip, (a, s) of add_noise at the start timestep) for a variation of a clip of `frames` latent frames."""
         with torch.cuda.device(self.device):
             if edit is not None:
                 self._admit_edit(k, frames, *edit)
@@ -382,6 +417,17 @@ class CudaSlots:
             self.gens[k] = g
             self.lat[k].zero_()
             self.lat[k, :, :frames] = torch.randn((1, self.C, frames), generator=g, device=self.device)[0]   # the draw of a solo run
+            if variation is not None:
+                self._admit_variation(k, frames, *variation)
+
+    def _admit_variation(self, k: int, frames: int, wave: np.ndarray, ab: Tuple[float, float]):
+        """variation_audio's start of one clip (api.py): normalise and pad the clip on the device, then encode it alone and noise it with
+        the start noise in slot k's latent row, in one pass -- the bottleneck noise comes from the global RNG."""
+        clip = post.prepare_wave(torch.from_numpy(wave).to(self.device).unsqueeze(0), frames * self.hop, normalize=True)
+        p = self.ez.params["autoencoder"]
+        x_t = self.ez.autoencoder.decoder.encode_noised(clip.view(1, 1, -1), [ab], self.lat[k:k + 1, :, :frames], p["scale"], p["shift"])
+        self.lat[k, :, :frames] = x_t[0]
+        self.trim[k] = len(wave)
 
     def _admit_edit(self, k: int, frames: int, wave: np.ndarray, p: dict):
         """editing_audio's preparation of one clip (api.py): normalise and pad the clip on the device, encode the crop alone -- the
@@ -474,8 +520,8 @@ class CudaSlots:
             self.lat.copy_(snap)   # capture does not execute; keep the eager result
 
     def finish(self, k: int, frames: int):
-        """Decodes slot k alone at its own length (as inference() does) and frees it; returns the float32 waveform (hop * frames,), or for
-        an edit the whole edited clip (n_total,), as editing_audio returns it."""
+        """Decodes slot k alone at its own length (as inference() does) and frees it; returns the float32 waveform (hop * frames,), for a
+        variation trimmed to its clip's length, or for an edit the whole edited clip (n_total,), as editing_audio returns it."""
         with torch.cuda.device(self.device):
             p = self.ez.params["autoencoder"]
             pred = scale_shift_re(self.lat[k:k + 1, :, :frames], p["scale"], p["shift"])
@@ -487,7 +533,8 @@ class CudaSlots:
             self.lat[k].zero_()
             self.gens[k] = None
             if edit is None:
-                return wav[0, 0].cpu().numpy()
+                n, self.trim[k] = self.trim[k], None
+                return wav[0, 0, :n].cpu().numpy()
             clip, s0, n = edit
             post.splice_wave(clip, wav[0, 0], s0, n)
             for row in (k, self.S + k):

@@ -83,6 +83,25 @@ class EditRequest:
         object.__setattr__(self, "scheduler", scheduler)
 
 
+@dataclasses.dataclass(frozen=True)
+class VariationRequest:
+    """One audio-to-audio variation: the arguments of `EzAudio.variation_audio` for one clip (defaults included).  `init_audio` is the clip:
+    a path, or a float32 mono waveform at the model's sample rate.  The result has the clip's length in samples."""
+    prompt: str
+    init_audio: object
+    strength: float = 0.8
+    guidance_scale: float = 5
+    guidance_rescale: float = 0.75
+    ddim_steps: int = 100
+    eta: float = 1
+    random_seed: Optional[int] = None
+    # as Request.scheduler; an init-only argument, so that the fields stay one per argument of EzAudio.variation_audio
+    scheduler: dataclasses.InitVar[str] = "ddim"
+
+    def __post_init__(self, scheduler):
+        object.__setattr__(self, "scheduler", scheduler)
+
+
 def length_bucket_bin(length: float, length_bucket_s: float) -> int:
     """Bucket index of a clip length: ceil(length / bucket), so bucket k holds lengths in ((k - 1) * bucket, k * bucket]."""
     return max(1, math.ceil(length / length_bucket_s - 1e-9))
@@ -131,13 +150,19 @@ class BatchingFrontEnd:
 
     @staticmethod
     def _check(r: Request) -> Request:
+        if isinstance(r, (EditRequest, VariationRequest, ControlRequest)):
+            raise ValueError(f"the batching front-end serves text-to-audio requests, got {type(r).__name__}; serve edits, variations and "
+                             "ControlNet requests with engine.ContinuousEngine")
         if r.scheduler != "ddim":
             raise ValueError(f"the batching front-end runs DDIM only, got scheduler={r.scheduler!r}; serve DPM-Solver++ requests with "
                              "engine.ContinuousEngine(schedulers=...) or set EzAudio.noise_scheduler")
         return r
 
     def submit(self, prompt: str, **kw) -> int:
-        """Queues a request; returns its ticket (index in submission order).  Requests for another scheduler than DDIM raise ValueError."""
+        """Queues a request; returns its ticket (index in submission order).  Requests for another scheduler than DDIM, and variations
+        (`init_audio=`), raise ValueError."""
+        if "init_audio" in kw:
+            raise ValueError("the batching front-end serves no variations (init_audio); serve them with engine.ContinuousEngine")
         self._queue.append(self._check(Request(prompt, **kw)))
         return len(self._queue) - 1
 

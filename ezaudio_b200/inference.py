@@ -6,6 +6,8 @@ Differences from the reference loop, all additive:
   * step-invariant work (context embedding, cross-attention K/V, timestep/AdaLN tables) is computed once per clip;
   * CFG + rescale + DDIM update is one fused kernel (ezb_cfg_ddim_step); so is CFG + rescale + DPM-Solver++ (ezb_cfg_dpm_step) when the
     scheduler is a `scheduler.DPMSolverMultistepScheduler` -- the swap a diffusers user makes with `noise_scheduler`; eta is then ignored;
+  * audio-to-audio variations (SDEdit): `start_index=` / `init_latents=` start sample b at its own schedule index from a noised latent
+    (`OobleckDecoder.encode_noised`); the batch runs the steps from the smallest start on, each sample's update switched on from its own;
   * clips of different lengths in one batch (`lengths=`): the batch is padded to `audio_frames` and every prompt's frames come out as
     that prompt run alone at its own length computes them (same seed, same bits); one length-aware VAE decode turns the padded batch into
     waveforms.  Inpainting joins in with `padded_gt=True`: gt / gt_mask padded like the batch, ignored past each clip's end.
@@ -72,11 +74,38 @@ def check_lengths(lengths, B: int, L: int, gt=None, controlnet=None, padded_gt=F
     return lens
 
 
+def make_generators(random_seed, B: int, device):
+    """One torch.Generator per prompt: seed_i of a list, seed + i of an int, a random seed for None."""
+    per_prompt = isinstance(random_seed, (list, tuple))   # one seed per prompt (batching front-end): prompt i ~ Generator(seed_i)
+    if per_prompt and len(random_seed) != B:
+        raise ValueError(f"random_seed lists one seed per prompt: got {len(random_seed)} for {B} prompts")
+    gens = []
+    for i in range(B):
+        g = torch.Generator(device=device)
+        if per_prompt:
+            g.manual_seed(int(random_seed[i]))
+        elif random_seed is not None:
+            g.manual_seed(int(random_seed) + i)
+        else:
+            g.seed()
+        gens.append(g)
+    return gens
+
+
+def _slot_table(struct, rows):
+    """rows [steps][B] of (guidance_scale, guidance_rescale, coef, flags) -> a device int32 block of `struct` (ezb_ddim_slot / ezb_dpm_slot)."""
+    arr = (struct * sum(len(r) for r in rows))()
+    for a, (gs, gr, coef, flags) in zip(arr, (e for r in rows for e in r)):
+        a.guidance_scale, a.guidance_rescale, a.flags = gs, gr, flags
+        a.coef[:] = coef
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.int32)
+
+
 @torch.no_grad()
 def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, gt=None, gt_mask=None,
                    audio_frames=500, guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024,
                    controlnet=None, condition=None, conditioning_scale=1.0, init_noise=None, step_noise=None, device=None,
-                   use_graphs=True, paste_gt=True, lengths=None, padded_gt=False):
+                   use_graphs=True, paste_gt=True, lengths=None, padded_gt=False, *, start_index=None, init_latents=None, generators=None):
     """Denoising loop on cached text embeddings.  text (B,Lc,ctx) / text_mask (B,Lc); uncond_* (1 or B rows) when
     guidance_scale is truthy.  gt / gt_mask (B,C,L) for inpainting.  Returns the final latents (B,C,L) fp32 on device.
     `init_noise` / `step_noise` inject the RNG draws (parity tests); otherwise per-prompt generators are used.
@@ -88,10 +117,22 @@ def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, unc
     accepted).  Frames past a prompt's length are zero.  One captured graph serves every mix of lengths at the same padded length.
     gt / gt_mask go with lengths under `padded_gt=True` (refused without it): both are padded to audio_frames like the batch, the solo run
     is the one with gt[b:b+1, :, :lengths[b]] and the same slice of
-    the mask; what gt and gt_mask hold past a clip's end is ignored."""
+    the mask; what gt and gt_mask hold past a clip's end is ignored.
+    `start_index` (one schedule index per prompt, 0..ddim_steps-1) with `init_latents` (B, C, audio_frames), the noised start of an
+    audio-to-audio variation: the loop runs schedule indices min(start_index) .. ddim_steps-1, the DiT on the whole batch at every step,
+    and sample b is updated from its own start_index[b] on (DPM-Solver++: with begin_index = start_index[b]); before that its latents stay
+    as given.  `generators` (one per prompt, already past the initial draw) make the per-step draws, in step order, for the steps each
+    sample runs; `step_noise[i]` (when injected) is the draw of schedule step i.  Each sample's bits do not depend on the other samples'
+    starts, and a batch of one start equals a run of the truncated schedule."""
+    if start_index is not None:
+        start_index = _check_start(start_index, text.shape[0], int(ddim_steps), int(audio_frames), init_latents, controlnet, gt)
+        if init_noise is not None:
+            raise ValueError("a variation starts from init_latents: init_noise cannot be given with start_index")
+    elif init_latents is not None or generators is not None:
+        raise ValueError("init_latents / generators go with start_index")
     if lengths is not None:
         lengths = check_lengths(lengths, text.shape[0], int(audio_frames), gt, controlnet, padded_gt)
-        if init_noise is not None or step_noise is not None:
+        if init_noise is not None or (step_noise is not None and start_index is None):
             raise ValueError("lengths draws the noise per prompt: init_noise / step_noise cannot be injected")
     dev_index = unet._h.dev_index   # the loop runs where the denoiser's weights live
     if device is not None:
@@ -108,15 +149,27 @@ def sample_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, unc
     with torch.cuda.device(device):
         lat = _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
                                         guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, init_noise,
-                                        step_noise, device, use_graphs, lengths)
+                                        step_noise, device, use_graphs, lengths, start_index, init_latents, generators)
         if gt is not None and paste_gt:
             lat = torch.where(gt_mask.to(device).bool().expand_as(lat), lat, gt.to(device=device, dtype=lat.dtype))
         return lat
 
 
+def _check_start(start_index, B: int, steps: int, L: int, init_latents, controlnet, gt):
+    """Validates a variation's per-prompt start indices and start latents on the host."""
+    if controlnet is not None or gt is not None:
+        raise NotImplementedError("a variation (start_index) runs without a ControlNet and without inpainting")
+    ks = [int(k) for k in start_index]
+    if len(ks) != B or any(k != v for k, v in zip(ks, start_index)) or any(k < 0 or k >= steps for k in ks):
+        raise ValueError(f"start_index lists one schedule index in 0..{steps - 1} per prompt ({B} prompts), got {list(start_index)}")
+    if init_latents is None or init_latents.dim() != 3 or init_latents.shape[0] != B or init_latents.shape[2] != L:
+        raise ValueError(f"start_index needs init_latents of shape ({B}, C, {L})")
+    return ks
+
+
 def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
                               guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, init_noise, step_noise,
-                              device, use_graphs, lengths=None):
+                              device, use_graphs, lengths=None, start=None, init_latents=None, generators=None):
     B = text.shape[0]
     Cc = unet.cfg["out_chans"]
     L = int(audio_frames)
@@ -126,20 +179,11 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
     timesteps = [int(t) for t in noise_scheduler.timesteps]
 
     gens = None
-    if init_noise is None:
-        gens = []
-        per_prompt = isinstance(random_seed, (list, tuple))   # one seed per prompt (batching front-end): prompt i ~ Generator(seed_i)
-        if per_prompt and len(random_seed) != B:
-            raise ValueError(f"random_seed lists one seed per prompt: got {len(random_seed)} for {B} prompts")
-        for i in range(B):
-            g = torch.Generator(device=device)
-            if per_prompt:
-                g.manual_seed(int(random_seed[i]))
-            elif random_seed is not None:
-                g.manual_seed(int(random_seed) + i)
-            else:
-                g.seed()
-            gens.append(g)
+    if start is not None:   # a variation: the start latents are given, the generators are past their initial draw
+        gens = generators
+        latents = init_latents.to(device=device, dtype=torch.float32).clone()
+    elif init_noise is None:
+        gens = make_generators(random_seed, B, device)
         if lengths is None:
             latents = torch.cat([torch.randn((1, Cc, L), generator=g, device=device) for g in gens], 0)
         else:   # each prompt's draw at its own shape, placed into the zeroed padded batch
@@ -186,11 +230,16 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
     # Everything a captured launch sequence bakes in is in the key: shapes (incl. the context length, which fixes the cross-attention K/V layout and
     # tensor maps), the schedule, the guidance constants, which ControlNet handle (its serial, not id(): ids are recycled) and the
     # library's option epoch (ezb_set_option changes kernel selection).
-    nsteps = len(timesteps)
+    k0 = 0 if start is None else min(start)   # the first schedule index the loop runs
+    nsteps = len(timesteps) - k0
     draw = noise_scheduler.draws_noise if dpm else bool(eta and eta > 0)
+    if draw and start is not None and step_noise is None and (gens is None or len(gens) != B):
+        raise ValueError("a variation that draws step noise needs one generator per prompt (generators=) or step_noise")
     sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
     key = (B, Be, L, lengths is not None, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
            gt is not None, controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()))
+    if start is not None:
+        key = key + (("start", k0),)
     cache = unet.__dict__.setdefault("_loop_cache", {})
     st = cache.get(key) if use_graphs else None
     if st is None:
@@ -201,9 +250,10 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
                   hist=torch.empty(B, Cc, L, device=device, dtype=torch.float32) if dpm else None,   # the previous step's x0 prediction
                   gt=None if gt_c is None else torch.empty_like(gt_c), m8=None if m8 is None else torch.empty_like(m8),
                   cond=None, skips=None, graph=None, launches=0,
-                  lens=torch.empty(Be, device=device, dtype=torch.int32) if lengths is not None else None)   # [lengths | lengths] under CFG
-        if st["noise"] is not None and lengths is not None:
-            st["noise"].zero_()   # the padded frames are never read; keep them finite
+                  lens=torch.empty(Be, device=device, dtype=torch.int32) if lengths is not None else None,   # [lengths | lengths] under CFG
+                  slots=None)   # a variation: the per-step slot table [steps, B] of the slots kernels
+        if st["noise"] is not None and (lengths is not None or start is not None):
+            st["noise"].zero_()   # the padded frames, and the draws of samples that have not started, are never read; keep them finite
         if controlnet is not None:
             st["cond"] = torch.empty_like(cond_c)
             st["skips"] = skips
@@ -221,7 +271,17 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
     if lens is not None:   # read by the kernels when they run: a replayed graph follows the new lengths
         lens.copy_(torch.tensor(lengths * (Be // B), dtype=torch.int32))
     lat, x_in, out, noise_all = st["lat"], st["x_in"], st["out"], st["noise"]
-    if noise_all is not None:  # RNG stays in PyTorch, outside the graph: step i, prompt b draws (1, C, L) from prompt b's generator, in step order
+    if noise_all is not None and start is not None:   # a variation: sample b draws at the steps it runs, at its own shape
+        for i in range(nsteps):
+            for b in range(B):
+                if k0 + i < start[b]:
+                    continue
+                n = L if lengths is None else lengths[b]
+                if step_noise is not None:
+                    noise_all[i, b, :, :n] = step_noise[k0 + i][b, :, :n]
+                else:
+                    noise_all[i, b, :, :n] = torch.empty((1, Cc, n), device=device).normal_(generator=gens[b])[0]
+    elif noise_all is not None:  # RNG stays in PyTorch, outside the graph: step i, prompt b draws (1, C, L) from prompt b's generator, in step order
         for i in range(nsteps):
             if step_noise is not None:
                 noise_all[i].copy_(step_noise[i])
@@ -233,7 +293,28 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
                     noise_all[i, b, :, :lengths[b]] = torch.empty((1, Cc, lengths[b]), device=device).normal_(generator=g)[0]
 
     # DPM-Solver++: every step's coefficients and order, computed once, before any capture
-    dpm_coef = [noise_scheduler.step_coefficients(i) for i in range(nsteps)] if dpm else None
+    dpm_coef = [noise_scheduler.step_coefficients(i) for i in range(nsteps)] if dpm and start is None else None
+    if start is not None:   # the slots kernels' constants of every step, in device memory before any capture: sample b is active from start[b]
+        gs_, gr_ = float(guidance_scale) if use_cfg else 0.0, float(guidance_rescale or 0.0)
+        cfg_flag = _lib.SLOT_ACTIVE | (_lib.SLOT_CFG if use_cfg else 0)
+        rows = []
+        for i in range(k0, len(timesteps)):
+            row = []
+            for b in range(B):
+                if i < start[b]:
+                    row.append((0.0, 0.0, (0.0,) * (7 if dpm else 5), 0))
+                elif dpm:
+                    coef, order = noise_scheduler.step_coefficients(i, begin_index=start[b])
+                    row.append((gs_, gr_, coef, cfg_flag | (_lib.SLOT_ORDER2 if order == 2 else 0)))
+                else:
+                    row.append((gs_, gr_, noise_scheduler.step_coefficients(timesteps[i], float(eta or 0.0)), cfg_flag))
+            rows.append(row)
+        table = _slot_table(_lib.DpmSlot if dpm else _lib.DdimSlot, rows).to(device)
+        if st["slots"] is None:
+            st["slots"] = table
+        else:   # read when the kernels run: a replayed graph follows the new starts
+            st["slots"].copy_(table)
+        words = (10 if dpm else 8) * B
 
     def one_step(i, t):
         if use_cfg:
@@ -246,6 +327,18 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         if controlnet is not None:
             sk = controlnet.forward_step(xi, i, st["cond"], conditioning_scale, gt=st["gt"], gt_mask_u8=st["m8"], outs=st["skips"])
         unet.forward_step(xi, i, gt=st["gt"], gt_mask_u8=st["m8"], controlnet_skips=sk, out=out, lengths=lens)
+        if start is not None:
+            j = i - k0
+            sl = st["slots"][j * words:(j + 1) * words]
+            nz = None if noise_all is None else noise_all[j]
+            lb = None if lens is None else lens[:B]
+            if dpm:
+                _lib.check(_lib.lib().ezb_cfg_dpm_step_slots(device.index, _lib.ptr(out), _lib.ptr(lat), _lib.ptr(st["hist"]), _lib.ptr(nz), _lib.ptr(sl),
+                                                             B, Cc, L, _lib.stream_ptr(), _lib.ptr(lb)))
+            else:
+                _lib.check(_lib.lib().ezb_cfg_ddim_step_slots(device.index, _lib.ptr(out), _lib.ptr(lat), _lib.ptr(nz), _lib.ptr(sl), B, Cc, L,
+                                                              _lib.stream_ptr(), _lib.ptr(lb)))
+            return
         if dpm:
             coef, order = dpm_coef[i]
             _dpm_step(out, lat, st["hist"], None if noise_all is None else noise_all[i], B, Cc, L, guidance_scale if use_cfg else 0.0, guidance_rescale,
@@ -260,15 +353,15 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
         st["graph"].replay()
         L_.ezb_launch_count_add(st["launches"])
     else:
-        for i, t in enumerate(timesteps):   # eager pass: warms caches (tensor maps, function attributes) and IS this call's result
-            one_step(i, t)
+        for i in range(k0, len(timesteps)):   # eager pass: warms caches (tensor maps, function attributes) and IS this call's result
+            one_step(i, timesteps[i])
         if use_graphs:
             snap = lat.clone()
             g = torch.cuda.CUDAGraph()
             n0 = L_.ezb_launch_count()
             with torch.cuda.graph(g):
-                for i, t in enumerate(timesteps):
-                    one_step(i, t)
+                for i in range(k0, len(timesteps)):
+                    one_step(i, timesteps[i])
             st["launches"] = int(L_.ezb_launch_count() - n0)
             st["graph"] = g
             lat.copy_(snap)  # capture does not execute; keep the eager result
@@ -278,11 +371,13 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
 @torch.no_grad()
 def inference(autoencoder, unet, gt, gt_mask, tokenizer, text_encoder, params, noise_scheduler, text_raw, neg_text=None,
               audio_frames=500, guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device="cuda",
-              text_embeds=None, controlnet=None, condition=None, conditioning_scale=1.0, lengths=None, padded_gt=False):
+              text_embeds=None, controlnet=None, condition=None, conditioning_scale=1.0, lengths=None, padded_gt=False, *, start_index=None,
+              init_latents=None, generators=None):
     """Signature of src/inference.py:26-37 (+ keyword-only extensions).  Returns the waveform tensor (B,1,480*L).
     With `lengths` (one clip length in frames per prompt, batch padded to audio_frames; see sample_latents) it returns a list of B
     waveforms (1, 480*lengths[b]) from one length-aware VAE decode of the padded batch (each equal to the decode of that clip alone).
-    gt / gt_mask go with lengths under `padded_gt=True`, as in sample_latents: padded to audio_frames, ignored past each clip's end."""
+    gt / gt_mask go with lengths under `padded_gt=True`, as in sample_latents: padded to audio_frames, ignored past each clip's end.
+    start_index / init_latents / generators: an audio-to-audio variation, as in sample_latents."""
     if lengths is not None:
         lengths = check_lengths(lengths, len(text_raw) if text_embeds is None else text_embeds[0].shape[0], int(audio_frames), gt, controlnet,
                                 padded_gt)
@@ -296,7 +391,7 @@ def inference(autoencoder, unet, gt, gt_mask, tokenizer, text_encoder, params, n
         raise ValueError("either tokenizer/text_encoder or text_embeds is required (the denoiser is text-conditioned)")
     latents = sample_latents(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, gt, gt_mask, audio_frames, guidance_scale,
                              guidance_rescale, ddim_steps, eta, random_seed, controlnet, condition, conditioning_scale, device=device, paste_gt=False,
-                             lengths=lengths, padded_gt=padded_gt)
+                             lengths=lengths, padded_gt=padded_gt, start_index=start_index, init_latents=init_latents, generators=generators)
     pred = scale_shift_re(latents, params["autoencoder"]["scale"], params["autoencoder"]["shift"])
     if gt is not None:  # src/inference.py:104-105: pred[~gt_mask] = gt[~gt_mask], with the raw gt, after the rescale
         pred = torch.where(gt_mask.to(pred.device).bool().expand_as(pred), pred, gt.to(device=pred.device, dtype=pred.dtype))

@@ -8,7 +8,7 @@ Only the scalar schedule lives here; the tensor update runs in the fused CUDA ke
 """
 from __future__ import annotations
 
-from typing import List
+from typing import List, Tuple
 
 import numpy as np
 import torch
@@ -35,6 +35,20 @@ def trailing_timesteps(num_train_timesteps: int, num_inference_steps: int) -> to
     return torch.from_numpy(np.round(np.arange(num_train_timesteps, 0, -step_ratio)).astype(np.int64) - 1)
 
 
+def start_index(num_inference_steps: int, strength: float) -> int:
+    """First schedule index of an audio-to-audio variation, in diffusers' img2img convention: the last n_run = min(int(steps * strength),
+    steps) steps run, from index steps - n_run.  strength outside (0, 1], or one that leaves no step to run, raises ValueError."""
+    steps = int(num_inference_steps)
+    if steps < 1 or steps != num_inference_steps:
+        raise ValueError(f"num_inference_steps must be a positive step count, got {num_inference_steps!r}")
+    if isinstance(strength, bool) or not isinstance(strength, (int, float, np.integer, np.floating)) or not 0 < strength <= 1:
+        raise ValueError(f"strength must lie in (0, 1], got {strength!r}")
+    n_run = min(int(steps * strength), steps)
+    if n_run == 0:
+        raise ValueError(f"strength {strength} runs no step of a {steps}-step schedule (int(steps * strength) = 0)")
+    return steps - n_run
+
+
 class DDIMScheduler:
     kind = "ddim"   # what sample_latents and the continuous engine dispatch on
 
@@ -57,6 +71,15 @@ class DDIMScheduler:
 
     def scale_model_input(self, sample, timestep=None):
         return sample
+
+    def add_noise_coefficients(self, timestep: int) -> Tuple[float, float]:
+        """(a, s) of diffusers' add_noise at training timestep t, noisy = a * x0 + s * eps: (sqrt(abar_t), sqrt(1 - abar_t)) in fp32.  Under
+        zero terminal SNR abar_999 is 0, so t = 999 gives exactly (0, 1)."""
+        t = int(timestep)
+        if not 0 <= t < self.num_train_timesteps:
+            raise ValueError(f"timestep {timestep} outside 0..{self.num_train_timesteps - 1}")
+        a = self.alphas_cumprod[t]
+        return float(a ** 0.5), float((1 - a) ** 0.5)
 
     def step_coefficients(self, timestep: int, eta: float) -> List[float]:
         """[sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-sigma^2), sigma] of DDIMScheduler.step (fp32, diffusers op order):
@@ -140,14 +163,29 @@ class DPMSolverMultistepScheduler:
         alpha = 1 / ((sigma ** 2 + 1) ** 0.5)
         return alpha, sigma * alpha
 
-    def step_coefficients(self, step_index: int):
+    def add_noise_coefficients(self, timestep: int) -> Tuple[float, float]:
+        """(a, s) of diffusers' add_noise at timestep t of the schedule, noisy = a * x0 + s * eps: (alpha_t, sigma_t) of its sigma, fp32.
+        At t = 999 the 2**-24 clamp gives a = 2**-12, not 0."""
+        if self.sigmas is None:
+            raise ValueError("call set_timesteps first")
+        hit = (self.timesteps == int(timestep)).nonzero()
+        if len(hit) == 0:
+            raise ValueError(f"timestep {timestep} is not in the {self.num_inference_steps}-step schedule")
+        alpha, sigma = self._alpha_sigma(self.sigmas[int(hit[0, 0])])
+        return float(alpha), float(sigma)
+
+    def step_coefficients(self, step_index: int, begin_index: int = 0):
         """(coef, order) of step `step_index`: coef = [alpha_s, sigma_s, kx, k0, k1, r, kz] of the update in the class docstring
         (k1 = r = 0 at order 1, kz = 0 without noise), fp32 in diffusers' order of operations.  At the last step lambda_t is infinite
-        (sigma_t = 0); exp(-h) is then 0 and every coefficient is finite."""
-        i = int(step_index)
+        (sigma_t = 0); exp(-h) is then 0 and every coefficient is finite.  begin_index: the first step a run takes (an audio-to-audio
+        variation starts part-way, diffusers' set_begin_index); that step has no history and is order 1.  An argument, not state, so that
+        one scheduler serves runs that begin at different steps."""
+        i, k = int(step_index), int(begin_index)
         if self.sigmas is None or not 0 <= i < len(self.orders):
             raise ValueError(f"step index {step_index} outside the schedule; call set_timesteps first")
-        order = self.orders[i]
+        if not 0 <= k <= i:
+            raise ValueError(f"begin index {begin_index} must lie in 0..{i} (the step index)")
+        order = 1 if i == k else self.orders[i]
         alpha_t, sigma_t = self._alpha_sigma(self.sigmas[i + 1])
         alpha_s0, sigma_s0 = self._alpha_sigma(self.sigmas[i])
         lambda_t = torch.log(alpha_t) - torch.log(sigma_t)   # +inf at the last step

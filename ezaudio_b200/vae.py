@@ -109,6 +109,40 @@ class OobleckDecoder:
         samples; frames < lengths[b] of the result equal the encode of that clip alone, bit for bit, and the frames past them are zeros.
         With `noise=None` the bottleneck noise of clip b is drawn as (1, latent, lengths[b]) from the global RNG, in clip order -- the draws
         consecutive solo calls make -- which needs the lengths on the host (a list)."""
+        a, T, L, lens, nz = self._encode_inputs(audio, noise, lengths)
+        z = torch.empty(a.shape[0], self.cfg["latent_dim"], L, device=self.device, dtype=torch.float32)
+
+        def launch(args, lb, b0, nb):
+            if lb is None:
+                return _lib.lib().ezb_vae_encode(*args, _lib.stream_ptr())
+            return _lib.lib().ezb_vae_encode_lens(*args, lb, _lib.stream_ptr())
+        self._run_encode(a, T, nz, z, lens, launch)
+        return z
+
+    def encode_noised(self, audio: torch.Tensor, ab, eps: torch.Tensor, scale: float, shift: float, noise=None, lengths=None) -> torch.Tensor:
+        """The start latent of an audio-to-audio variation in one pass (ezb_vae_encode_noised): with z = encode(audio, noise, lengths),
+        x_t = a_b * ((z + shift) * scale) + s_b * eps_b -- scale_shift, then diffusers' add_noise with clip b's (a_b, s_b) = ab[b]
+        (`DDIMScheduler.add_noise_coefficients`).  ab: (B, 2) fp32 (a cuda tensor is read when the kernel runs), eps (B, latent, L).
+        noise and lengths as in `encode`; with lengths, frames past a clip's end come out as zeros and eps is not read there."""
+        B, L = audio.shape[0], -(-audio.shape[-1] // self.hop)   # checked before _encode_inputs draws the bottleneck noise
+        abt = torch.as_tensor(ab, dtype=torch.float32)
+        if tuple(abt.shape) != (B, 2) or tuple(eps.shape) != (B, self.cfg["latent_dim"], L):
+            raise ValueError(f"ab must be ({B}, 2) and eps ({B}, {self.cfg['latent_dim']}, {L}), got {tuple(abt.shape)} and {tuple(eps.shape)}")
+        a, T, L, lens, nz = self._encode_inputs(audio, noise, lengths)
+        abt = abt.to(self.device).contiguous()
+        e = _as_f32c(eps).to(self.device)
+        x_t = torch.empty(B, self.cfg["latent_dim"], L, device=self.device, dtype=torch.float32)
+        sc, sh = float(scale), float(shift)
+
+        def launch(args, lb, b0, nb):
+            h, au, vn, out, n, t = args
+            return _lib.lib().ezb_vae_encode_noised(h, au, vn, C.c_void_p(e[b0:b0 + nb].data_ptr()), C.c_void_p(abt[b0:b0 + nb].data_ptr()), sc, sh,
+                                                    out, n, t, lb, _lib.stream_ptr())
+        self._run_encode(a, T, nz, x_t, lens, launch)
+        return x_t
+
+    def _encode_inputs(self, audio, noise, lengths):
+        """encode's argument handling: (audio zero-padded to a whole hop, T, L, device lens or None, bottleneck noise or None)."""
         if self.encoder_cfg is None:
             raise _lib.EzbError("this handle was created without encoder_cfg")
         a = _as_f32c(audio).to(self.device)
@@ -133,17 +167,18 @@ class OobleckDecoder:
         elif noise is None:
             noise = torch.randn(B, Cz, L, device=self.device, dtype=torch.float32)
         nz = None if noise is False else _as_f32c(noise).to(self.device)
-        z = torch.empty(B, Cz, L, device=self.device, dtype=torch.float32)
+        return a, T, L, lens, nz
+
+    def _run_encode(self, a, T, nz, out, lens, launch):
+        """Calls launch((handle, audio, noise, out, nb, T), lens or None, b0, nb) on each run of at most max_batch clips."""
+        B = a.shape[0]
         with torch.cuda.device(self.dev_index):
             for b0 in range(0, B, self.max_batch):
                 nb = min(self.max_batch, B - b0)
                 args = (self.h, _lib.ptr(a[b0:b0 + nb]), None if nz is None else C.c_void_p(nz[b0:b0 + nb].data_ptr()),
-                        C.c_void_p(z[b0:b0 + nb].data_ptr()), nb, T)
-                if lens is None:
-                    _lib.check(_lib.lib().ezb_vae_encode(*args, _lib.stream_ptr()))
-                else:
-                    _lib.check(_lib.lib().ezb_vae_encode_lens(*args, _lib.ptr(lens[b0:b0 + nb]), _lib.stream_ptr()))
-        return z
+                        C.c_void_p(out[b0:b0 + nb].data_ptr()), nb, T)
+                lb = None if lens is None else _lib.ptr(lens[b0:b0 + nb])
+                _lib.check(launch(args, lb, b0, nb))
 
 
 class Autoencoder:

@@ -9,7 +9,7 @@
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
  * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev,
- * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, decode, encode, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
+ * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
  */
@@ -191,6 +191,15 @@ int ezb_vae_encode(ezb_vae* h, const float* audio, const float* noise, float* z,
  *   the clip's end. */
 int ezb_vae_decode_lens(ezb_vae* h, const float* z, float* wav, int B, int L, const int32_t* lens, void* stream);
 int ezb_vae_encode_lens(ezb_vae* h, const float* audio, const float* noise, float* z, int B, int T, const int32_t* lens, void* stream);
+/* ezb_vae_encode_noised: the start latent of an audio-to-audio variation (SDEdit) in the encode's last pass.  With z of ezb_vae_encode
+ *   (vae_noise as its noise, NULL -> the mean), x_t = a_b * ((z + shift) * scale) + s_b * eps_b: scale_shift (src/utils/utils.py:20-21,
+ *   the latent the denoiser was trained on, src/train.py:275-284) then diffusers' add_noise, each product and the sum rounded in fp32 as
+ *   PyTorch rounds them.  ab_dev: DEVICE fp32 [B][2], (a_b, s_b) per clip, read when the kernel runs (one captured graph serves any mix);
+ *   eps (B,latent,L) fp32; scale and shift are the autoencoder's.  lens (DEVICE int32 [B], or NULL) as in ezb_vae_encode_lens: frames at or
+ *   past lens[b] are written as zeros, and the encoder rows, vae_noise and eps there are not read.  With a = 1, s = 0, scale = 1 and
+ *   shift = 0, x_t equals z of ezb_vae_encode / ezb_vae_encode_lens bit for bit. */
+int ezb_vae_encode_noised(ezb_vae* h, const float* audio, const float* vae_noise, const float* eps, const float* ab_dev, float scale, float shift,
+                          float* x_t, int B, int T, const int32_t* lens, void* stream);
 
 /* EnergyExtractor.forward (src/models/conditions/energy.py:19-56) as wrapped by Conditioner (condition_wrapper.py:26-42): audio (B,T) fp32
  * -> (B, T/hop) fp32 frame energies in dB, normalised per clip when norm != 0; quantize_levels <= 1 disables quantisation. Only the shipped
