@@ -133,6 +133,8 @@ _SIGS = {
     "ezb_cfg_ddim_step_slots": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP], _I),
     "ezb_cfg_dpm_step": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _F, _F, C.POINTER(C.c_float), _I, _VP, _VP], _I),
     "ezb_cfg_dpm_step_slots": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP], _I),
+    "ezb_window_gather": ([_I, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_window_blend": ([_I, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition": ([_VP, _VP, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition_rows": ([_VP, _VP, _I, _I, _I, _VP], _I),
     "ezb_controlnet_forward_tdev": ([_VP, _VP, _VP, _VP, C.POINTER(_VP), _I, _I, _VP], _I),

@@ -19,7 +19,7 @@ import torch
 from . import _lib, config, post, weights
 from ._lib import EzbError
 from .dit import DiTControlNet, MaskDiT
-from .inference import inference, make_generators
+from .inference import check_long, inference, make_generators, sample_long_latents, scale_shift_re
 from .scheduler import DDIMScheduler, start_index
 from .vae import Autoencoder, OobleckDecoder
 
@@ -389,6 +389,45 @@ class EzAudio(_Base):
         for o, w, p in zip(outs, wavs, plans):
             post.splice_wave(o, w[0], p["s0"], p["n_paste"])
         return sr, [o.cpu().numpy() for o in outs]
+
+    def generate_long_audio(self, text, length, window_length=10, overlap=2, guidance_scale=5, guidance_rescale=0.75, ddim_steps=100, eta=1,
+                            random_seed=None, randomize_seed=False):
+        """Text-to-audio past the denoiser's trained length (`inference.sample_long_latents`): at every step the clip's latent is cut into
+        windows of `window_length` seconds overlapping by `overlap` seconds, all windows are denoised as one batch and their predictions
+        are crossfaded back into one; the long latent is then decoded in tiles (`OobleckDecoder.decode_tiled`).  No DiT call sees more than
+        one window, and no workspace grows with `length`.  `text` is a prompt or a list of prompts, `length` (seconds) one value or one per
+        prompt; seeds as in generate_audio (an int gives prompt b seed + b, a list one seed per prompt).  Returns (sr, waveform) or
+        (sr, [waveforms]) with hop * int(length * latent_sr) samples each.  A clip no longer than the window equals generate_audio's
+        with the same seed and frame count, bit for bit.  The windows (x 2 with guidance) must fit the DiT's 2 * max_batch rows."""
+        batched = not isinstance(text, str)
+        prompts = list(text) if batched else [text]
+        B = len(prompts)
+        latent_sr = self.params["autoencoder"]["latent_sr"]
+        # ---- everything is checked on the host before any device work
+        num = (int, float, np.integer, np.floating)
+        frames = [int(v * latent_sr) for v in _per_clip("length", length, B, num)]
+        if B < 1 or any(f < 1 for f in frames):
+            raise ValueError(f"every length must be positive (at least one latent frame), got {length}")
+        if window_length > self.max_length_s:
+            raise ValueError(f"window_length {window_length} s exceeds max_length_s {self.max_length_s} s")
+        window, hop_over = int(window_length * latent_sr), int(overlap * latent_sr)
+        empty = [t == "" for t in prompts]
+        if any(empty) and not all(empty):
+            raise ValueError("empty prompts run without guidance: they cannot share a batch with non-empty ones")
+        if all(empty):
+            guidance_scale = None
+            print("empyt input")
+        check_long(frames, B, window, hop_over, bool(guidance_scale), int(self.unet._h.desc.max_batch), int(self.unet._h.desc.max_len))
+        if randomize_seed:
+            random_seed = random.randint(0, MAX_SEED)
+        text_emb, mask, uemb, umask = self._text_embeds(prompts, [""])
+        lat = sample_long_latents(self.unet, self.noise_scheduler, text_emb, mask, uemb, umask, frames, window, hop_over, guidance_scale,
+                                  guidance_rescale, ddim_steps, eta, random_seed)
+        p = self.params["autoencoder"]
+        wav = self.autoencoder.decoder.decode_tiled(scale_shift_re(lat, p["scale"], p["shift"]), lengths=frames)
+        hop = self.autoencoder.decoder.hop
+        out = [wav[b, 0, :hop * n].cpu().numpy() for b, n in enumerate(frames)]
+        return (p["sr"], out) if batched else (p["sr"], out[0])
 
     def variation_audio(self, text, init_audio, strength=0.8, guidance_scale=5, guidance_rescale=0.75, ddim_steps=100, eta=1, random_seed=None,
                         randomize_seed=False, *, pad_length=None):

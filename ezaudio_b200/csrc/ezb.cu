@@ -6,6 +6,7 @@
 #include "vae.cuh"
 #include "t5.cuh"
 #include "host.cuh"
+#include "longform.cuh"
 
 using namespace ezb;
 
@@ -912,6 +913,25 @@ EZB_API int ezb_cfg_dpm_step_slots(int device, const float* model_out, float* la
   EZB_CUDA(cudaSetDevice(device));
   return launch_k(cfg_dpm_slots_kernel, dim3(B * CFG_CLUSTER), dim3(1024), 0, ST(stream), CFG_CLUSTER, model_out, model_out + (size_t)B * C * L,
                   latents, history, noise, lens, slots, C, L);
+}
+EZB_API int ezb_window_gather(int device, const float* latents, float* windows, const int32_t* plan_dev, int B, int C, int Nmax, int W, int Lw,
+                              int overlap, int copies, void* stream) {
+  if (!latents || !windows || !plan_dev || B < 1 || C < 1 || Nmax < 1 || W < B || Lw < 2 || overlap < 1 || overlap > Lw / 2 ||
+      (copies != 1 && copies != 2))
+    return fail(EZB_ERR_ARG, "ezb_window_gather: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(window_gather_launch(ST(stream), WindowPlan{plan_dev, B, C, Nmax, W, Lw, overlap}, latents, windows, copies));
+  return EZB_OK;
+}
+EZB_API int ezb_window_blend(int device, const float* windows, float* out, const int32_t* plan_dev, int B, int C, int Nmax, int W, int Lw, int overlap,
+                             void* stream) {
+  if (!windows || !out || !plan_dev || B < 1 || C < 1 || Nmax < 1 || W < B || Lw < 2 || overlap < 1 || overlap > Lw / 2)
+    return fail(EZB_ERR_ARG, "ezb_window_blend: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(window_blend_launch(ST(stream), WindowPlan{plan_dev, B, C, Nmax, W, Lw, overlap}, windows, out));
+  return EZB_OK;
 }
 EZB_API int ezb_vae_create(ezb_vae** out, const ezb_vae_desc* desc, int device) {
   if (!out || !desc) return fail(EZB_ERR_ARG, "ezb_vae_create: null argument");

@@ -1,0 +1,76 @@
+// window_gather_kernel / window_blend_kernel: see longform.cuh for the plan and for why they live in a translation unit of their own.
+#include "longform.cuh"
+
+namespace ezb {
+
+struct ClipWindows { int first, count, n, len; };   // len: frames of each window (Lw, or N when the clip is one short window)
+
+__device__ __forceinline__ ClipWindows clip_windows(const WindowPlan& p, int b) {
+  const int32_t* e = p.plan + 3 * b;
+  const int n = min(max(e[2], 1), p.Nmax);
+  return ClipWindows{e[0], e[1], n, min(n, p.Lw)};
+}
+__device__ __forceinline__ int window_start(const WindowPlan& p, const ClipWindows& cw, int k) {
+  return k == cw.count - 1 ? cw.n - cw.len : k * (p.Lw - p.overlap);
+}
+// min(1, left, right), each ratio an IEEE division, as window_weights (inference.py) states it
+__device__ __forceinline__ float window_weight(const WindowPlan& p, const ClipWindows& cw, int k, int j) {
+  const float o1 = (float)(p.overlap + 1);
+  float w = 1.f;
+  if (k > 0) w = fminf(w, __fdiv_rn((float)(j + 1), o1));
+  if (k < cw.count - 1) w = fminf(w, __fdiv_rn((float)(p.Lw - j), o1));
+  return w;
+}
+
+__global__ void __launch_bounds__(256) window_gather_kernel(const WindowPlan p, const float* __restrict__ latents, float* __restrict__ windows) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.C * p.Lw) return;
+  const int r = blockIdx.y, c = i / p.Lw, j = i - c * p.Lw;
+  float v = 0.f;
+  for (int b = 0; b < p.B; ++b) {
+    const ClipWindows cw = clip_windows(p, b);
+    if (r < cw.first || r >= cw.first + cw.count) continue;
+    if (j < cw.len) v = latents[((size_t)b * p.C + c) * p.Nmax + window_start(p, cw, r - cw.first) + j];
+    break;
+  }
+  windows[(((size_t)blockIdx.z * p.W + r) * p.C + c) * p.Lw + j] = v;
+}
+
+// v(f) = sum_k w_k(f - s_k) v_k(f - s_k) / sum_k w_k(f - s_k) over the windows covering frame f, in increasing k, in fp32.  The first term
+// starts the sums, so one covering window of weight 1 gives its v bit for bit.
+__global__ void __launch_bounds__(256) window_blend_kernel(const WindowPlan p, const float* __restrict__ windows, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.C * p.Nmax) return;
+  const int b = blockIdx.y, c = i / p.Nmax, f = i - c * p.Nmax;
+  const ClipWindows cw = clip_windows(p, b);
+  if (f >= cw.n) return;
+  const int H = p.Lw - p.overlap;
+  // the evenly spaced windows 0 .. count - 2 covering f, then the last one (which starts at N - len) when it covers f
+  const int k_lo = f >= p.Lw ? (f - p.Lw) / H + 1 : 0, k_hi = min(cw.count - 2, f / H);
+  float acc = 0.f, ws = 0.f;
+  bool first = true;
+  auto add = [&](int k, int s) {
+    const int row = cw.first + k;
+    if (row < 0 || row >= p.W) return;
+    const float w = window_weight(p, cw, k, f - s);
+    const float v = windows[((size_t)row * p.C + c) * p.Lw + (f - s)];
+    if (first) { acc = w * v; ws = w; first = false; }
+    else { acc = fmaf(w, v, acc); ws += w; }
+  };
+  for (int k = k_lo; k <= k_hi; ++k) add(k, k * H);
+  const int s_last = cw.n - cw.len;
+  if (f >= s_last) add(cw.count - 1, s_last);
+  out[((size_t)b * p.C + c) * p.Nmax + f] = __fdiv_rn(acc, ws);
+}
+
+cudaError_t window_gather_launch(cudaStream_t st, const WindowPlan& p, const float* latents, float* windows, int copies) {
+  window_gather_kernel<<<dim3((unsigned)((p.C * p.Lw + 255) / 256), p.W, copies), 256, 0, st>>>(p, latents, windows);
+  return cudaGetLastError();
+}
+
+cudaError_t window_blend_launch(cudaStream_t st, const WindowPlan& p, const float* windows, float* out) {
+  window_blend_kernel<<<dim3((unsigned)((p.C * p.Nmax + 255) / 256), p.B), 256, 0, st>>>(p, windows, out);
+  return cudaGetLastError();
+}
+
+}  // namespace ezb

@@ -11,6 +11,8 @@ Differences from the reference loop, all additive:
   * clips of different lengths in one batch (`lengths=`): the batch is padded to `audio_frames` and every prompt's frames come out as
     that prompt run alone at its own length computes them (same seed, same bits); one length-aware VAE decode turns the padded batch into
     waveforms.  Inpainting joins in with `padded_gt=True`: gt / gt_mask padded like the batch, ignored past each clip's end.
+  * clips longer than the denoiser's window (`sample_long_latents`): overlapping windows denoised as one batch, guided per window and
+    crossfaded on the device into one long prediction at every step (MultiDiffusion; ezb_window_gather / ezb_window_blend).
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -19,6 +21,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -366,6 +369,185 @@ def _sample_latents_on_device(unet, noise_scheduler, text, text_mask, uncond_tex
             st["graph"] = g
             lat.copy_(snap)  # capture does not execute; keep the eager result
     return lat.clone()   # the inpainting paste happens after scale_shift_re, in inference() (src/inference.py:102-105)
+
+
+def window_plan(n: int, window: int, overlap: int):
+    """The windows (start, length) of a clip of n frames for windowed denoising (include/ezb200.h, ezb_window_gather): n <= window is one
+    window [0, n); otherwise windows of `window` frames start every window - overlap frames, and the last one ends at the clip's end."""
+    if not 1 <= overlap <= window // 2:
+        raise ValueError(f"overlap must lie in 1..{window // 2} frames (half the window of {window}), got {overlap}")
+    if n <= window:
+        return [(0, n)]
+    hop = window - overlap
+    count = -(-(n - window) // hop) + 1
+    return [(k * hop, window) for k in range(count - 1)] + [(n - window, window)]
+
+
+def window_weights(k: int, count: int, length: int, window: int, overlap: int):
+    """fp32 crossfade weights of window k of count over its `length` frames: min(1, (j + 1) / (overlap + 1) after the first window,
+    (window - j) / (overlap + 1) before the last), as the blend kernel computes them."""
+    j = np.arange(length)
+    w = np.ones(length, dtype=np.float32)
+    o1 = np.float32(overlap + 1)
+    if k > 0:
+        w = np.minimum(w, (j + 1).astype(np.float32) / o1)
+    if k < count - 1:
+        w = np.minimum(w, (window - j).astype(np.float32) / o1)
+    return w
+
+
+def long_plan(lengths, window: int, overlap: int):
+    """Windows of a batch of long clips, laid out clip by clip as consecutive DiT rows: (the plan table [(first row, count, N)] per clip,
+    the windows [(clip, start, length)] in row order)."""
+    table, windows = [], []
+    for b, n in enumerate(lengths):
+        ws = window_plan(n, window, overlap)
+        table.append((len(windows), len(ws), n))
+        windows += [(b, s, ln) for s, ln in ws]
+    return table, windows
+
+
+def check_long(lengths, B: int, window: int, overlap: int, use_cfg: bool, max_rows: int, max_len: int):
+    """Validates a windowed run on the host before any device work; returns (lengths, plan table, windows)."""
+    lens = [int(v) for v in lengths]
+    if len(lens) != B or any(v != w for v, w in zip(lens, lengths)) or any(v < 1 for v in lens):
+        raise ValueError(f"lengths lists one positive whole frame count per prompt ({B} prompts), got {list(lengths)}")
+    if not 2 <= int(window) <= max_len:
+        raise ValueError(f"window must lie in 2..{max_len} frames (the denoiser's max_len), got {window}")
+    table, windows = long_plan(lens, int(window), int(overlap))
+    rows = len(windows) * (2 if use_cfg else 1)
+    if rows > max_rows:
+        raise ValueError(f"{len(windows)} windows{' x 2 (CFG)' if use_cfg else ''} = {rows} DiT rows exceed the row capacity {max_rows} "
+                         f"(2 * max_batch): needs max_batch >= {-(-rows // 2)}")
+    return lens, table, windows
+
+
+@torch.no_grad()
+def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, lengths=(), window=500, overlap=100,
+                        guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device=None, use_graphs=True):
+    """Windowed denoising (MultiDiffusion) of clips longer than the denoiser's window: clip b has lengths[b] frames; at every step its
+    latent is cut into overlapping windows of `window` frames (`overlap` frames of overlap, window_plan), the DiT denoises every window
+    of every clip as one batch, each window's prediction is guided and rescaled on its own (the rescale's std is over one window, as over one
+    trained-length clip), and the blend of the windows' predictions (crossfade weights, window_weights) drives the DDIM or DPM-Solver++
+    update of the long latent.  Returns the latents (B, C, max(lengths)) fp32 on the device, zero past each clip's end.
+    Prompt b's generator (random_seed as in sample_latents) draws the initial noise and each step's noise at (1, C, lengths[b]): the draws
+    a solo sample_latents at that length makes, so a clip that fits one window comes out as that call computes it, bit for bit.
+    The windows (x 2 under CFG) must fit the DiT's row capacity: one forward per step.  The whole schedule is one captured graph."""
+    B = text.shape[0]
+    use_cfg = bool(guidance_scale)
+    desc = unet._h.desc
+    lens, table, windows = check_long(lengths, B, window, overlap, use_cfg, int(desc.max_batch), int(desc.max_len))
+    dev_index = unet._h.dev_index
+    if device is not None:
+        d = torch.device(device)
+        if d.type != "cuda" or (d.index is not None and d.index != dev_index):
+            raise ValueError(f"sample_long_latents(device={d}) but the denoiser lives on cuda:{dev_index}")
+    device = torch.device("cuda", dev_index)
+    with torch.cuda.device(device):
+        return _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, int(window),
+                                      int(overlap), guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs)
+
+
+def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
+    """The guided, rescaled v of every window: ezb_cfg_ddim_step on the window rows with coefficients (1, 0, 0, 1, 0) and no noise writes
+    0 * x0 + 1 * (1 * v + 0 * x) = v into `guided`, exactly the v that kernel computes for its own update (same cluster reduction, same
+    rescale ratio bits).  `guided` (W, C, Lw) plays the latents and must hold finite values (0 * x must be 0)."""
+    _ddim_step(out, guided, None, W, Cc, Lw, gs, gr, (1.0, 0.0, 0.0, 1.0, 0.0), wlens)
+
+
+def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, Lw, O, guidance_scale,
+                           guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs):
+    B, W, N = text.shape[0], len(windows), max(lens)
+    Cc = unet.cfg["out_chans"]
+    use_cfg = bool(guidance_scale)
+    dpm = getattr(noise_scheduler, "kind", "ddim") == "dpm"
+    noise_scheduler.set_timesteps(ddim_steps)
+    timesteps = [int(t) for t in noise_scheduler.timesteps]
+    nsteps = len(timesteps)
+    gens = make_generators(random_seed, B, device)
+    latents = torch.zeros((B, Cc, N), device=device)
+    for b, g in enumerate(gens):
+        latents[b, :, :lens[b]] = torch.randn((1, Cc, lens[b]), generator=g, device=device)[0]
+
+    # the T5 context of every window row: [text of each window | "" of each window]
+    clip_of = torch.tensor([b for b, _, _ in windows], device=device)
+    text = text.to(device=device, dtype=torch.float32)[clip_of]
+    text_mask = text_mask.to(device).bool()[clip_of]
+    if use_cfg:
+        if uncond_text.shape[0] == 1:
+            uncond_text, uncond_mask = uncond_text.expand(B, -1, -1), uncond_mask.expand(B, -1)
+        ctx = torch.cat([text, uncond_text.to(device=device, dtype=torch.float32)[clip_of]], 0).contiguous()
+        cmask = torch.cat([text_mask, uncond_mask.to(device).bool()[clip_of]], 0).contiguous()
+    else:
+        ctx, cmask = text.contiguous(), text_mask.contiguous()
+    Be = ctx.shape[0]
+    unet.set_context(ctx, cmask)
+    unet.set_timesteps(timesteps)
+
+    # Everything the captured launches bake in is in the key: shapes (B, window rows, the longest clip, window, overlap, context length), the
+    # schedule, the guidance constants, the sampler and the library's option epoch.  The plan table and the lengths are read on the device.
+    draw = noise_scheduler.draws_noise if dpm else bool(eta and eta > 0)
+    sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
+    key = (B, W, N, Lw, O, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
+           int(_lib.lib().ezb_option_epoch()))
+    cache = unet.__dict__.setdefault("_long_cache", {})
+    st = cache.get(key) if use_graphs else None
+    if st is None:
+        st = dict(lat=torch.empty(B, Cc, N, device=device), x_in=torch.empty(Be, Cc, Lw, device=device), out=torch.empty(Be, Cc, Lw, device=device),
+                  guided=torch.zeros(W, Cc, Lw, device=device) if use_cfg else None, v=torch.empty(B, Cc, N, device=device),
+                  noise=torch.zeros(nsteps, B, Cc, N, device=device) if draw else None,
+                  hist=torch.empty(B, Cc, N, device=device) if dpm else None,
+                  plan=torch.empty(B * 3, device=device, dtype=torch.int32), wlens=torch.empty(Be, device=device, dtype=torch.int32),
+                  lens=torch.empty(B, device=device, dtype=torch.int32), graph=None, launches=0)
+        if use_graphs:
+            if len(cache) >= 2:
+                cache.clear()
+            cache[key] = st
+    st["lat"].copy_(latents)
+    st["plan"].copy_(torch.tensor([e for row in table for e in row], dtype=torch.int32))
+    st["wlens"].copy_(torch.tensor([ln for _, _, ln in windows] * (Be // W), dtype=torch.int32))
+    st["lens"].copy_(torch.tensor(lens, dtype=torch.int32))
+    lat, x_in, out, v, noise_all, plan = st["lat"], st["x_in"], st["out"], st["v"], st["noise"], st["plan"]
+    if noise_all is not None:   # step i, prompt b: the (1, C, lengths[b]) draw of a solo run, in step order
+        for i in range(nsteps):
+            for b, g in enumerate(gens):
+                noise_all[i, b, :, :lens[b]] = torch.empty((1, Cc, lens[b]), device=device).normal_(generator=g)[0]
+    dpm_coef = [noise_scheduler.step_coefficients(i) for i in range(nsteps)] if dpm else None
+    gs, gr = (float(guidance_scale), float(guidance_rescale or 0.0)) if use_cfg else (0.0, 0.0)
+    L_ = _lib.lib()
+
+    def one_step(i, t):
+        _lib.check(L_.ezb_window_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), B, Cc, N, W, Lw, O, Be // W, _lib.stream_ptr()))
+        unet.forward_step(x_in, i, out=out, lengths=st["wlens"])
+        src = out
+        if use_cfg:
+            _guide_windows(out, st["guided"], W, Cc, Lw, gs, gr, st["wlens"][:W])
+            src = st["guided"]
+        _lib.check(L_.ezb_window_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), B, Cc, N, W, Lw, O, _lib.stream_ptr()))
+        nz = None if noise_all is None else noise_all[i]
+        if dpm:
+            coef, order = dpm_coef[i]
+            _dpm_step(v, lat, st["hist"], nz, B, Cc, N, 0.0, 0.0, coef, order, st["lens"])
+        else:
+            _ddim_step(v, lat, nz, B, Cc, N, 0.0, 0.0, noise_scheduler.step_coefficients(t, float(eta or 0.0)), st["lens"])
+
+    if use_graphs and st["graph"] is not None:
+        st["graph"].replay()
+        L_.ezb_launch_count_add(st["launches"])
+    else:
+        for i, t in enumerate(timesteps):   # eager pass: warms caches and IS this call's result
+            one_step(i, t)
+        if use_graphs:
+            snap = lat.clone()
+            g = torch.cuda.CUDAGraph()
+            n0 = L_.ezb_launch_count()
+            with torch.cuda.graph(g):
+                for i, t in enumerate(timesteps):
+                    one_step(i, t)
+            st["launches"] = int(L_.ezb_launch_count() - n0)
+            st["graph"] = g
+            lat.copy_(snap)
+    return lat.clone()
 
 
 @torch.no_grad()

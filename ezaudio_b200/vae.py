@@ -11,6 +11,22 @@ from . import _lib, weights
 from .dit import PRECISIONS, _as_f32c
 
 
+def decoder_receptive_field(cfg) -> int:
+    """Latent frames on either side of a latent frame that can change the decoder's samples of that frame (the halo decode_tiled gives
+    each chunk): the interval a perturbed frame reaches, propagated through the input conv (k 7), every stage's transposed conv (k 2s,
+    stride s, padding s / 2) and its three residual units (k 7 at dilations 1, 3, 9; the 1x1 convs reach nothing), and the output conv
+    (k 7), in decoder order (the config's strides reversed), then rounded up to whole frames of hop samples."""
+    lo, hi = -3, 3                                        # input conv, in latent frames
+    for s in reversed(list(cfg["strides"])):
+        lo, hi = lo * s - s // 2, hi * s - s // 2 + 2 * s - 1   # outputs input frame i reaches: i*s - s/2 .. i*s - s/2 + 2s - 1
+        lo, hi = lo - 3 * (1 + 3 + 9), hi + 3 * (1 + 3 + 9)
+    lo, hi = lo - 3, hi + 3                               # output conv
+    hop = 1
+    for s in cfg["strides"]:
+        hop *= s
+    return max(-(lo // hop), -(-(hi - (hop - 1)) // hop))
+
+
 class OobleckDecoder:
     """OobleckDecoder (and, when `encoder_cfg` is given, OobleckEncoder + VAE bottleneck) on one ezb_vae handle."""
 
@@ -42,6 +58,7 @@ class OobleckDecoder:
         for s in dec_cfg["strides"]:
             self.hop *= s
         self.max_batch = max_batch
+        self.max_latent_len = max_latent_len
         self.h = C.c_void_p()
         with torch.cuda.device(self.dev_index):
             _lib.check(_lib.lib().ezb_vae_create(C.byref(self.h), C.byref(d), self.dev_index))
@@ -101,6 +118,39 @@ class OobleckDecoder:
         return wav
 
     forward = __call__
+
+    def decode_tiled(self, z: torch.Tensor, lengths=None) -> torch.Tensor:
+        """z (B,latent,L) -> (B,1,hop*L) for L longer than the workspace's max_latent_len, on this handle: each clip is cut into chunks
+        of at most max_latent_len frames whose inner edges carry a halo of decoder_receptive_field frames, up to max_batch chunks go to one
+        length-aware decode, and each chunk's core is pasted into the output.  Every core sample depends only on latent frames inside its
+        chunk, so the result equals a one-shot decode (on a workspace that holds L) bit for bit.  `lengths` (a list of latent frames per
+        clip, or None): z is a padded batch, as in __call__; samples past hop * lengths[b] are zeros."""
+        z = _as_f32c(z).to(self.device)
+        B, Cz, L = z.shape
+        host = [L] * B if lengths is None else self._lens(lengths, B, L)[1]
+        if host is None:
+            raise ValueError("decode_tiled takes the lengths as a list")
+        h, M = decoder_receptive_field(self.cfg), self.max_latent_len
+        core = M - 2 * h
+        if core < 1:
+            raise ValueError(f"max_latent_len {M} leaves no core inside a halo of {h} frames on each side")
+        chunks = []   # (clip, first frame, end frame, core start, core end)
+        for b, n in enumerate(host):
+            for c0 in range(0, n, core if n > M else n):
+                c1 = min(n, c0 + core) if n > M else n
+                chunks.append((b, max(0, c0 - h), min(n, c1 + h), c0, c1))
+        wav = torch.zeros(B, 1, L * self.hop, device=self.device, dtype=torch.float32)
+        hop = self.hop
+        for g0 in range(0, len(chunks), self.max_batch):
+            group = chunks[g0:g0 + self.max_batch]
+            Lc = max(e - s for _, s, e, _, _ in group)
+            zs = torch.zeros(len(group), Cz, Lc, device=self.device, dtype=torch.float32)
+            for k, (b, s, e, _, _) in enumerate(group):
+                zs[k, :, :e - s] = z[b, :, s:e]
+            ws = self(zs, lengths=[e - s for _, s, e, _, _ in group])
+            for k, (b, s, _, c0, c1) in enumerate(group):
+                wav[b, :, c0 * hop:c1 * hop] = ws[k, :, (c0 - s) * hop:(c1 - s) * hop]
+        return wav
 
     def encode(self, audio: torch.Tensor, noise=None, lengths=None) -> torch.Tensor:
         """audio (B,1,T) -> latents (B,latent,T/hop): encoder + z = mean + (softplus(scale)+1e-4) * noise

@@ -9,7 +9,7 @@
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
  * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev,
- * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
+ * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, window_gather, window_blend, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
  */
@@ -157,6 +157,23 @@ typedef struct {
 enum { EZB_SLOT_ORDER2 = 4 };
 int ezb_cfg_dpm_step_slots(int device, const float* model_out, float* latents, float* history, const float* noise, const ezb_dpm_slot* slots_dev,
                            int B, int C, int L, void* stream, const int32_t* lens);
+
+/* Windowed denoising of clips longer than the denoiser's trained window (MultiDiffusion, Bar-Tal et al. 2023).  Clip b of N_b frames is
+ * cut into windows of Lw frames overlapping by `overlap` frames (1 <= overlap <= Lw / 2, hop H = Lw - overlap): N_b <= Lw is one window
+ * [0, N_b); otherwise n_b = ceil((N_b - Lw) / H) + 1 windows start at k * H for k < n_b - 1, and the last at N_b - Lw.  Window k weighs its
+ * local frame j by min(1, left, right): left = (j + 1) / (overlap + 1) when k > 0, else 1; right = (Lw - j) / (overlap + 1) when
+ * k < n_b - 1, else 1.  plan_dev: DEVICE int32 [B][3] = (first window row, n_b, N_b) per clip, the clips' windows laid out clip by clip as
+ * consecutive rows 0 .. W - 1; it is read when the kernels run (a captured graph follows a new plan of the same W) and validating it is
+ * the caller's job (ezaudio_b200.inference.window_plan builds it).  latents / out (B, C, Nmax) fp32, windows (rows, C, Lw) fp32.
+ * ezb_window_gather: window row r gets its frames of the long latents and zeros past its length (N_b when N_b < Lw); copies 2 writes the
+ *   same rows again at row offset W (the uncond half of a CFG batch).
+ * ezb_window_blend: frame f < N_b of clip b gets sum_k w_k v_k / sum_k w_k over the windows covering it, in increasing k, in fp32, the
+ *   division IEEE-rounded; one covering window of weight 1 gives its value bit for bit.  Window frames past a window's length and long
+ *   frames at or past N_b are neither read nor written. */
+int ezb_window_gather(int device, const float* latents, float* windows, const int32_t* plan_dev, int B, int C, int Nmax, int W, int Lw,
+                      int overlap, int copies, void* stream);
+int ezb_window_blend(int device, const float* windows, float* out, const int32_t* plan_dev, int B, int C, int Nmax, int W, int Lw, int overlap,
+                     void* stream);
 
 /* --- VAE decoder: OobleckDecoder.forward (stable_vae/models/autoencoders.py:149-190) behind
  * Autoencoder(embedding=z) (src/modules/autoencoder_wrapper.py:74-77). */
