@@ -138,6 +138,7 @@ _SIGS = {
     "ezb_controlnet_set_condition": ([_VP, _VP, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition_rows": ([_VP, _VP, _I, _I, _I, _VP], _I),
     "ezb_controlnet_forward_tdev": ([_VP, _VP, _VP, _VP, C.POINTER(_VP), _I, _I, _VP], _I),
+    "ezb_controlnet_forward_cached": ([_VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _I, _F, C.POINTER(_VP), _I, _I, _VP], _I),
     "ezb_option_epoch": ([], C.c_ulonglong),
     "ezb_vae_create": ([C.POINTER(_VP), C.POINTER(VaeDesc), _I], _I),
     "ezb_vae_destroy": ([_VP], _I),

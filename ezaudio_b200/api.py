@@ -619,3 +619,75 @@ class EzAudio_ControlNet(_Base):
                          controlnet=self.controlnet, condition=condition, conditioning_scale=conditioning_scale)
         pred = pred.cpu().numpy()
         return sr, [pred[b, 0][:len(r)] for b, r in enumerate(raws)]
+
+    def generate_long_audio(self, text, audio_path, window_length=10, overlap=2, surpass_noise=0, guidance_scale=3.5, guidance_rescale=0,
+                            ddim_steps=50, eta=1, conditioning_scale=1, random_seed=None, randomize_seed=False):
+        """generate_audio for reference clips of any length: the output is as long as the clip (generate_audio cuts it to 10 s).
+        The clip's latent is denoised in windows of `window_length` seconds overlapping by `overlap` seconds, as in
+        EzAudio.generate_long_audio (inference.sample_long_latents), and decoded in tiles.  Clip b of n_b samples gets
+        long_control_frames(n_b, hop, window) latent frames: a clip shorter than the window is padded to it, as generate_audio pads to 10 s.
+        The condition is the energy contour of the whole prepared clip (one peak normalisation and one noise gate per clip, then
+        energy_condition over all of it), so overlapping windows see the same condition values on the frames they share; each window's
+        slice of it goes through the ControlNet's stem once per call.
+        `audio_path`: a path or a float32 waveform, or a list of one per prompt; `surpass_noise` and `random_seed` one value or one per
+        prompt, as in generate_audio; `conditioning_scale` one value for the call.  Returns (sr, waveform) or, for a list of prompts,
+        (sr, [waveforms]), waveform b trimmed to n_b samples.  An empty prompt runs without guidance (as in EzAudio.generate_long_audio) and
+        cannot share a call with non-empty ones.  With window_length=10, a clip of at most 10 s is one window and the result equals
+        generate_audio with the same arguments and seed, bit for bit (for an empty prompt: generate_audio with guidance_scale=0).  The
+        windows (x 2 with guidance) must fit the 2 * max_batch rows of the DiT and the ControlNet: a 60 s clip in 10 s windows with 2 s
+        overlap is 8 windows, which needs max_batch=8 with guidance."""
+        batched = not isinstance(text, str)
+        prompts = list(text) if batched else [text]
+        B = len(prompts)
+        p = self.params["autoencoder"]
+        sr, latent_sr = p["sr"], p["latent_sr"]
+        # ---- everything is checked on the host before any device work
+        if isinstance(audio_path, (list, tuple)):
+            if not batched:
+                raise ValueError("a list of reference clips takes a list of prompts (one clip per prompt)")
+            clips = list(audio_path)
+            if len(clips) != B:
+                raise ValueError(f"audio_path lists one clip per prompt: got {len(clips)} for {B} prompts")
+        else:
+            clips = [audio_path] * B
+        num = (int, float, np.integer, np.floating)
+        gates = [float(g or 0) for g in _per_clip("surpass_noise", surpass_noise, B, num)]
+        if isinstance(random_seed, (list, tuple)) and len(random_seed) != B:
+            raise ValueError(f"random_seed lists one seed per prompt: got {len(random_seed)} for {B} prompts")
+        if B < 1:
+            raise ValueError("no prompt given")
+        if window_length > self.max_length_s:
+            raise ValueError(f"window_length {window_length} s exceeds the ControlNet's {self.max_length_s} s")
+        window, hop_over = int(window_length * latent_sr), int(overlap * latent_sr)
+        empty = [t == "" for t in prompts]
+        if any(empty) and not all(empty):
+            raise ValueError("empty prompts run without guidance: they cannot share a batch with non-empty ones")
+        if all(empty):
+            guidance_scale = None
+        raws = [_load_audio(a, sr) if isinstance(a, str) else np.asarray(a, dtype=np.float32) for a in clips]
+        if any(r.ndim != 1 or len(r) < 1 for r in raws):
+            raise ValueError("every reference clip must be a non-empty mono waveform")
+        hop = int(round(sr / latent_sr))
+        frames = [long_control_frames(len(r), hop, window) for r in raws]
+        rows = min(int(self.unet._h.desc.max_batch), int(self.controlnet._h.desc.max_batch))
+        check_long(frames, B, window, hop_over, bool(guidance_scale), rows, int(self.unet._h.desc.max_len))
+        if randomize_seed:
+            random_seed = random.randint(0, MAX_SEED)
+        cond_kw = {k: v for k, v in self.params["conditioner"].items() if k != "condition_type"}
+        condition = torch.zeros(B, 1, 2 * max(frames), device=self.device)   # clip b's frames past 2 * frames[b] are never read
+        for b, (r, g, n) in enumerate(zip(raws, gates, frames)):
+            wave = post.prepare_wave(torch.from_numpy(r).to(self.device).unsqueeze(0), n * hop, normalize=True, gate=g)
+            condition[b:b + 1, :, :2 * n] = energy_condition(wave, **cond_kw)
+        text_emb, mask, uemb, umask = self._text_embeds(prompts, [""])
+        lat = sample_long_latents(self.unet, self.noise_scheduler, text_emb, mask, uemb, umask, frames, window, hop_over, guidance_scale,
+                                  guidance_rescale, ddim_steps, eta, random_seed, controlnet=self.controlnet, condition=condition,
+                                  conditioning_scale=conditioning_scale)
+        wav = self.autoencoder.decoder.decode_tiled(scale_shift_re(lat, p["scale"], p["shift"]), lengths=frames)
+        out = [wav[b, 0, :len(r)].cpu().numpy() for b, r in enumerate(raws)]
+        return (sr, out) if batched else (sr, out[0])
+
+
+def long_control_frames(n_samples: int, hop: int, window: int) -> int:
+    """Latent frames of EzAudio_ControlNet.generate_long_audio for a reference clip of n_samples samples: enough whole hops to hold the
+    clip, and at least one window (a shorter clip is zero-padded to it, as generate_audio pads to 10 s)."""
+    return max(int(window), -(-int(n_samples) // int(hop)))

@@ -1110,6 +1110,8 @@ struct Dit {
   int controlnet_forward(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, const float* cond, float cscale,
                          float* const* skips_out, int Be, int L, cudaStream_t st);
   int controlnet_forward_tdev(const float* x, const int32_t* tdev, const float* scale_dev, float* const* skips_out, int Be, int L, cudaStream_t st);
+  int controlnet_forward_cached(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, float cscale,
+                                float* const* skips_out, int Be, int L, cudaStream_t st);
   int set_condition(const float* cond, int Be, int L, cudaStream_t st);
   int set_condition_rows(const float* cond, int row0, int n, int L, cudaStream_t st);
   int controlnet_stem(const float* cond, float* out, int Be, int L, cudaStream_t st);
@@ -1187,6 +1189,18 @@ inline int Dit::controlnet_forward_tdev(const float* x, const int32_t* tdev, con
   if (Be != cond_Be || L != cond_L)
     return fail(EZB_ERR_STATE, "controlnet_forward_tdev: Be %d / L %d differ from the condition set by ezb_controlnet_set_condition (%d, %d)", Be, L, cond_Be, cond_L);
   return controlnet_trunk(x, nullptr, nullptr, nullptr, 0, tdev, nullptr, 0.f, scale_dev, skips_out, Be, L, st);
+}
+
+// controlnet_forward on the condition cache: the stem computes each row on its own, so the cached rows hold the bits controlnet_forward
+// writes into cond_emb, and everything after the stem takes the same path (host indices, uniform scale, fold mode).
+inline int Dit::controlnet_forward_cached(const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall, float cscale,
+                                          float* const* skips_out, int Be, int L, cudaStream_t st) {
+  if (!d.is_controlnet) return fail(EZB_ERR_STATE, "ezb_controlnet_forward_cached called on a DiT handle");
+  EZB_TRY(check_call(Be, L));
+  if (Be != cond_Be || L != cond_L)
+    return fail(EZB_ERR_STATE, "controlnet_forward_cached: Be %d / L %d differ from the condition set by ezb_controlnet_set_condition (%d, %d)", Be, L, cond_Be,
+                cond_L);
+  return controlnet_trunk(x, gt, gt_mask, tidx, tall, nullptr, nullptr, cscale, nullptr, skips_out, Be, L, st);
 }
 
 // cond: the raw condition, run through the stem into cond_emb here, or null for the condition cache.  scale_dev (device [Be]) or, when null,

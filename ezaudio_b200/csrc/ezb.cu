@@ -885,6 +885,11 @@ EZB_API int ezb_controlnet_forward_tdev(ezb_dit* h, const float* x, const int32_
   if (!h || !x || !t_index_dev || !scale_dev || !skips_out) return fail(EZB_ERR_ARG, "ezb_controlnet_forward_tdev: null argument");
   return reinterpret_cast<Dit*>(h)->controlnet_forward_tdev(x, t_index_dev, scale_dev, skips_out, Be, L, ST(stream));
 }
+EZB_API int ezb_controlnet_forward_cached(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* tidx, int tall,
+                                          float scale, float* const* skips_out, int Be, int L, void* stream) {
+  if (!h || !x || !skips_out) return fail(EZB_ERR_ARG, "ezb_controlnet_forward_cached: null argument");
+  return reinterpret_cast<Dit*>(h)->controlnet_forward_cached(x, gt, gt_mask, tidx, tall, scale, skips_out, Be, L, ST(stream));
+}
 EZB_API int ezb_cfg_ddim_step_slots(int device, const float* model_out, float* latents, const float* noise, const ezb_ddim_slot* slots, int B, int C,
                                     int L, void* stream, const int32_t* lens) {
   if (!model_out || !latents || !slots || B < 1 || C < 1 || L < 1) return fail(EZB_ERR_ARG, "ezb_cfg_ddim_step_slots: bad argument");

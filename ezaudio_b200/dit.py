@@ -355,12 +355,23 @@ class DiTControlNet:
     def forward_step(self, x, step_index=0, condition=None, conditioning_scale=1.0, gt=None, gt_mask_u8=None, outs=None, t_index=None, scale=None):
         """One ControlNet forward at table row `step_index` on `condition` (Be,1,2L) with one `conditioning_scale`; returns depth/2 skips
         (Be,L,D) fp32 (written into `outs` when given).
+        Without `condition` (and without `t_index` / `scale`) it reads the condition cache of set_condition instead, whose layout (Be, L) x
+        must match (EzbError otherwise): the skips are bit-identical to passing the condition that was cached, and the stem, which does not
+        depend on the step, does not run again (ezb_controlnet_forward_cached).
         With `t_index` and `scale` -- contiguous cuda int32 / fp32 tensors of shape (Be,), read on the device when the kernels run, like
         MaskDiT.forward_step's t_index -- sample b runs at table row t_index[b] on the cached condition of set_condition with its skips times
         scale[b] (0 gives zeros); `condition`, `gt` and `gt_mask_u8` are then not accepted."""
-        if t_index is None and scale is None:
+        if t_index is None and scale is None and condition is not None:
             return self._run(x, gt, gt_mask_u8, None, int(step_index), condition, conditioning_scale, outs)
         Be, Cc, L = x.shape
+        if t_index is None and scale is None:
+            if outs is None:
+                outs = [torch.empty(Be, L, self.cfg["embed_dim"], device=self.device, dtype=torch.float32) for _ in range(self.half)]
+            arr = (C.c_void_p * self.half)(*[o.data_ptr() for o in outs])
+            with torch.cuda.device(self._h.dev_index):
+                _lib.check(_lib.lib().ezb_controlnet_forward_cached(self._h.h, _lib.ptr(x), _lib.ptr(gt), _lib.ptr(gt_mask_u8), None, int(step_index),
+                                                                    float(conditioning_scale), arr, Be, L, _lib.stream_ptr()))
+            return outs
         if t_index is None or scale is None:
             raise ValueError("t_index and scale go together")
         if condition is not None or gt is not None or gt_mask_u8 is not None:

@@ -12,7 +12,8 @@ Differences from the reference loop, all additive:
     that prompt run alone at its own length computes them (same seed, same bits); one length-aware VAE decode turns the padded batch into
     waveforms.  Inpainting joins in with `padded_gt=True`: gt / gt_mask padded like the batch, ignored past each clip's end.
   * clips longer than the denoiser's window (`sample_long_latents`): overlapping windows denoised as one batch, guided per window and
-    crossfaded on the device into one long prediction at every step (MultiDiffusion; ezb_window_gather / ezb_window_blend).
+    crossfaded on the device into one long prediction at every step (MultiDiffusion; ezb_window_gather / ezb_window_blend), with or
+    without a ControlNet whose per-window conditions are cached once per call (ezb_controlnet_forward_cached).
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -424,7 +425,8 @@ def check_long(lengths, B: int, window: int, overlap: int, use_cfg: bool, max_ro
 
 @torch.no_grad()
 def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, lengths=(), window=500, overlap=100,
-                        guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device=None, use_graphs=True):
+                        guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device=None, use_graphs=True, *,
+                        controlnet=None, condition=None, conditioning_scale=1.0):
     """Windowed denoising (MultiDiffusion) of clips longer than the denoiser's window: clip b has lengths[b] frames; at every step its
     latent is cut into overlapping windows of `window` frames (`overlap` frames of overlap, window_plan), the DiT denoises every window
     of every clip as one batch, each window's prediction is guided and rescaled on its own (the rescale's std is over one window, as over one
@@ -432,11 +434,27 @@ def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None
     update of the long latent.  Returns the latents (B, C, max(lengths)) fp32 on the device, zero past each clip's end.
     Prompt b's generator (random_seed as in sample_latents) draws the initial noise and each step's noise at (1, C, lengths[b]): the draws
     a solo sample_latents at that length makes, so a clip that fits one window comes out as that call computes it, bit for bit.
-    The windows (x 2 under CFG) must fit the DiT's row capacity: one forward per step.  The whole schedule is one captured graph."""
+    The windows (x 2 under CFG) must fit the DiT's row capacity: one forward per step.  The whole schedule is one captured graph.
+    `controlnet` (a DiTControlNet with the DiT's rows) with `condition` (B, 1, 2 * max(lengths)) fp32: clip b's condition frames are valid
+    up to 2 * lengths[b], and every clip must be at least one window long, so that every window is full-length.  Window [s, s + window) of
+    clip b is conditioned on condition[b, :, 2s:2s + 2 * window]; those rows go through the ControlNet's stem once per call, into its
+    condition cache (DiTControlNet.set_condition), and every step reads the cache at its timestep with `conditioning_scale`."""
     B = text.shape[0]
     use_cfg = bool(guidance_scale)
     desc = unet._h.desc
-    lens, table, windows = check_long(lengths, B, window, overlap, use_cfg, int(desc.max_batch), int(desc.max_len))
+    max_rows, max_len = int(desc.max_batch), int(desc.max_len)
+    if controlnet is not None or condition is not None:
+        if controlnet is None or condition is None:
+            raise ValueError("controlnet and condition go together")
+        cdesc = controlnet._h.desc
+        max_rows, max_len = min(max_rows, int(cdesc.max_batch)), min(max_len, int(cdesc.max_len))
+    lens, table, windows = check_long(lengths, B, window, overlap, use_cfg, max_rows, max_len)
+    if controlnet is not None:
+        if tuple(condition.shape) != (B, 1, 2 * max(lens)):
+            raise ValueError(f"condition must be (B, 1, 2 * max(lengths)) = {(B, 1, 2 * max(lens))}, got {tuple(condition.shape)}")
+        if min(lens) < int(window):
+            raise ValueError(f"with a ControlNet every clip must be at least one window ({int(window)} frames) long, got {lens}: its stem "
+                             "convolutions cross a shorter window's end")
     dev_index = unet._h.dev_index
     if device is not None:
         d = torch.device(device)
@@ -445,7 +463,8 @@ def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None
     device = torch.device("cuda", dev_index)
     with torch.cuda.device(device):
         return _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, int(window),
-                                      int(overlap), guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs)
+                                      int(overlap), guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs,
+                                      controlnet, condition, conditioning_scale)
 
 
 def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
@@ -456,7 +475,8 @@ def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
 
 
 def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, Lw, O, guidance_scale,
-                           guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs):
+                           guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs, controlnet=None, condition=None,
+                           conditioning_scale=1.0):
     B, W, N = text.shape[0], len(windows), max(lens)
     Cc = unet.cfg["out_chans"]
     use_cfg = bool(guidance_scale)
@@ -483,13 +503,20 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
     Be = ctx.shape[0]
     unet.set_context(ctx, cmask)
     unet.set_timesteps(timesteps)
+    if controlnet is not None:   # every window row's condition, [cond | cond] under CFG, through the stem once into the condition cache
+        cond = condition.to(device=device, dtype=torch.float32)
+        rows = torch.stack([cond[b, :, 2 * s:2 * (s + Lw)] for b, s, _ in windows])
+        controlnet.set_condition(torch.cat([rows] * (Be // W), 0))
+        controlnet.set_context(ctx, cmask)
+        controlnet.set_timesteps(timesteps)
 
     # Everything the captured launches bake in is in the key: shapes (B, window rows, the longest clip, window, overlap, context length), the
-    # schedule, the guidance constants, the sampler and the library's option epoch.  The plan table and the lengths are read on the device.
+    # schedule, the guidance constants, the sampler, the ControlNet handle (its serial) and scale, and the library's option epoch.  The plan
+    # table, the lengths and the ControlNet's condition cache are read on the device.
     draw = noise_scheduler.draws_noise if dpm else bool(eta and eta > 0)
     sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
     key = (B, W, N, Lw, O, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
-           int(_lib.lib().ezb_option_epoch()))
+           controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()))
     cache = unet.__dict__.setdefault("_long_cache", {})
     st = cache.get(key) if use_graphs else None
     if st is None:
@@ -498,7 +525,8 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
                   noise=torch.zeros(nsteps, B, Cc, N, device=device) if draw else None,
                   hist=torch.empty(B, Cc, N, device=device) if dpm else None,
                   plan=torch.empty(B * 3, device=device, dtype=torch.int32), wlens=torch.empty(Be, device=device, dtype=torch.int32),
-                  lens=torch.empty(B, device=device, dtype=torch.int32), graph=None, launches=0)
+                  lens=torch.empty(B, device=device, dtype=torch.int32), graph=None, launches=0,
+                  skips=None if controlnet is None else [torch.empty(Be, Lw, unet.cfg["embed_dim"], device=device) for _ in range(controlnet.half)])
         if use_graphs:
             if len(cache) >= 2:
                 cache.clear()
@@ -518,7 +546,11 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
 
     def one_step(i, t):
         _lib.check(L_.ezb_window_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), B, Cc, N, W, Lw, O, Be // W, _lib.stream_ptr()))
-        unet.forward_step(x_in, i, out=out, lengths=st["wlens"])
+        if controlnet is None:
+            unet.forward_step(x_in, i, out=out, lengths=st["wlens"])
+        else:   # every window is full-length: no lengths, which the DiT does not combine with ControlNet skips
+            sk = controlnet.forward_step(x_in, i, conditioning_scale=conditioning_scale, outs=st["skips"])
+            unet.forward_step(x_in, i, controlnet_skips=sk, out=out)
         src = out
         if use_cfg:
             _guide_windows(out, st["guided"], W, Cc, Lw, gs, gr, st["wlens"][:W])

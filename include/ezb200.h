@@ -8,7 +8,7 @@
  * Conventions: plain pointers and sizes, no torch types.  Every device pointer is owned by the caller (PyTorch) and
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
- * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev,
+ * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev, controlnet_forward_cached,
  * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, window_gather, window_blend, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
@@ -110,6 +110,14 @@ int ezb_controlnet_set_condition(ezb_dit* h, const float* condition, int Be, int
 int ezb_controlnet_set_condition_rows(ezb_dit* h, const float* condition, int row0, int n, int L, void* stream);
 int ezb_controlnet_forward_tdev(ezb_dit* h, const float* x, const int32_t* t_index_dev, const float* scale_dev, float* const* skips_out, int Be,
                                 int L, void* stream);
+/* ezb_controlnet_forward with the stem's output taken from the condition cache instead of a condition argument: for any host indices
+ * (all equal or not) and any conditioning_scale, the skips are bit-identical to ezb_controlnet_forward with the condition that was cached
+ * (the stem computes each row on its own; everything after it takes the same kernels, fold mode included).  conditioning_scale 0 gives zeros
+ * without running the network.  Be must match the context batch and the condition layout, L the layout (EZB_ERR_STATE otherwise).  A
+ * sampling loop that repeats one condition at every step runs the stem once (ezb_controlnet_set_condition) instead of once per step.
+ * Graph-safe, no synchronisation. */
+int ezb_controlnet_forward_cached(ezb_dit* h, const float* x, const float* gt, const uint8_t* gt_mask, const int32_t* t_index_host,
+                                  int t_index_all, float conditioning_scale, float* const* skips_out, int Be, int L, void* stream);
 
 /* --- fused classifier-free guidance + rescale + DDIM update (src/inference.py:12-23,88-100; diffusers DDIMScheduler.step
  * restated, SURVEY Appendix B).  model_out holds B text rows followed by B uncond rows when guidance_scale != 0, else B
