@@ -429,6 +429,86 @@ class EzAudio(_Base):
         out = [wav[b, 0, :hop * n].cpu().numpy() for b, n in enumerate(frames)]
         return (p["sr"], out) if batched else (p["sr"], out[0])
 
+    def editing_long_audio(self, text, boundary, gt_file, mask_start, mask_length, window_length=10, overlap=2, guidance_scale=3.5,
+                           guidance_rescale=0, ddim_steps=100, eta=1, random_seed=None, randomize_seed=False):
+        """editing_audio for crops of any length: inpainting, and continuation past the clip's end (outpainting), over more than the
+        denoiser's window.  The arguments and the crop arithmetic are editing_audio's (edit_plan): the mask [mask_start, mask_start +
+        mask_length) seconds is regenerated with `boundary` seconds of context on either side, and a mask past the clip's end extends it.
+        The crop is encoded in tiles (OobleckDecoder.encode_tiled), denoised in windows of `window_length` seconds overlapping by `overlap`
+        seconds with its gt and mask (inference.sample_long_latents), pasted (pred[~mask] = gt[~mask]), decoded in tiles and spliced back.
+        Only the window has to fit max_length_s; the crop may be any length.  Returns (sr, the whole edited clip), as editing_audio does.
+        A crop that fits one window gives editing_audio's result with the same seed, bit for bit.
+
+        Continuation of a 10-s clip by 30 s with 5 s of context (a 35-s crop: 5 windows, 10 DiT rows with guidance, so
+        EzAudio(..., max_batch=5)):
+
+            ez.editing_long_audio("rain turns into a thunderstorm", boundary=5, gt_file="rain_10s.wav", mask_start=10, mask_length=30)
+
+        With a list of prompts, `gt_file`, `mask_start`, `mask_length`, `boundary` and `random_seed` list one value per prompt (a scalar
+        applies to all; an int seed gives every edit that seed) and the call returns (sr, [clips]): one tiled encode, one windowed loop and
+        one tiled decode.  Each clip equals the scalar call of that edit with its seed, the calls made in list order (the VAE bottleneck
+        noise comes from the global RNG in clip order).  Empty prompts run without guidance and cannot share a call with non-empty ones.
+        The windows of all edits (x 2 with guidance) must fit the DiT's 2 * max_batch rows."""
+        batched = isinstance(text, (list, tuple))
+        prompts = list(text) if batched else [text]
+        sr, latent_sr = self.params["autoencoder"]["sr"], self.params["autoencoder"]["latent_sr"]
+        dec = self.autoencoder.decoder
+        B, hop = len(prompts), dec.hop
+        # ---- everything is checked on the host before any device work
+        if B < 1:
+            raise ValueError("no prompt given")
+        num = (int, float, np.integer, np.floating)
+        scalar = (str, np.ndarray) if batched else (str, np.ndarray, list, tuple)
+        files = _per_clip("gt_file", gt_file, B, scalar)
+        starts, lengths_s = _per_clip("mask_start", mask_start, B, num), _per_clip("mask_length", mask_length, B, num)
+        bounds = _per_clip("boundary", boundary, B, num)
+        if randomize_seed:
+            seeds = [random.randint(0, MAX_SEED) for _ in range(B)]
+        elif random_seed is None:
+            seeds = None
+        else:
+            seeds = [int(v) for v in _per_clip("random_seed", random_seed, B, num)]
+        empty = [t == "" for t in prompts]
+        if any(empty) and not all(empty):
+            raise ValueError("empty prompts run without guidance: they cannot share a batch with non-empty ones")
+        if all(empty):
+            guidance_scale = None
+            print("empyt input")
+        if any(v < 0 for v in starts) or any(v <= 0 for v in lengths_s) or any(v < 0 for v in bounds):
+            raise ValueError("mask_start and boundary must be >= 0 and mask_length > 0 for every edit")
+        if window_length > self.max_length_s:
+            raise ValueError(f"window_length {window_length} s exceeds max_length_s {self.max_length_s} s")
+        window, hop_over = int(window_length * latent_sr), int(overlap * latent_sr)
+        raws = [_load_audio(f, sr) if isinstance(f, str) else np.asarray(f, dtype=np.float32) for f in files]
+        if any(r.ndim != 1 or len(r) < 1 for r in raws):
+            raise ValueError("every gt_file must be a non-empty mono waveform")
+        plans = [edit_plan(len(r), sr, latent_sr, hop, bd, ms, ml) for r, bd, ms, ml in zip(raws, bounds, starts, lengths_s)]
+        frames = [p["frames"] for p in plans]
+        check_long(frames, B, window, hop_over, bool(guidance_scale), int(self.unet._h.desc.max_batch), int(self.unet._h.desc.max_len))
+        # ---- per clip: normalise + pad on the device, crop into the padded batch; one tiled encode (bottleneck noise: global RNG, clip order)
+        N = max(frames)
+        outs, crops = [], torch.zeros(B, 1, N * hop, device=self.device)
+        for b, (r, p) in enumerate(zip(raws, plans)):
+            o = post.prepare_wave(torch.from_numpy(r).to(self.device).unsqueeze(0), p["n_total"], normalize=True)[0]
+            crops[b, 0, :p["s1"] - p["s0"]] = o[p["s0"]:p["s1"]]
+            outs.append(o)
+        gt_latent = dec.encode_tiled(crops, lengths=frames)
+        gt_mask = torch.ones(B, N, dtype=torch.bool)
+        for b, p in enumerate(plans):
+            gt_mask[b, :p["m0"]] = False
+            gt_mask[b, p["m1"]:frames[b]] = False
+        gt_mask = gt_mask.to(self.device)
+        text_emb, mask, uemb, umask = self._text_embeds(prompts, [""])
+        lat = sample_long_latents(self.unet, self.noise_scheduler, text_emb, mask, uemb, umask, frames, window, hop_over, guidance_scale,
+                                  guidance_rescale, ddim_steps, eta, seeds, gt=gt_latent, gt_mask=gt_mask)
+        a = self.params["autoencoder"]
+        pred = torch.where(gt_mask[:, None, :], scale_shift_re(lat, a["scale"], a["shift"]), gt_latent)   # src/inference.py:104-105
+        wav = dec.decode_tiled(pred, lengths=frames)
+        for b, (o, p) in enumerate(zip(outs, plans)):
+            post.splice_wave(o, wav[b, 0], p["s0"], p["n_paste"])
+        res = [o.cpu().numpy() for o in outs]
+        return (sr, res) if batched else (sr, res[0])
+
     def variation_audio(self, text, init_audio, strength=0.8, guidance_scale=5, guidance_rescale=0.75, ddim_steps=100, eta=1, random_seed=None,
                         randomize_seed=False, *, pad_length=None):
         """Audio-to-audio variation (SDEdit; diffusers' img2img, Stable Audio's init_audio): `init_audio` (a WAV path or a float32 mono

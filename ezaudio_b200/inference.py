@@ -13,7 +13,8 @@ Differences from the reference loop, all additive:
     waveforms.  Inpainting joins in with `padded_gt=True`: gt / gt_mask padded like the batch, ignored past each clip's end.
   * clips longer than the denoiser's window (`sample_long_latents`): overlapping windows denoised as one batch, guided per window and
     crossfaded on the device into one long prediction at every step (MultiDiffusion; ezb_window_gather / ezb_window_blend), with or
-    without a ControlNet whose per-window conditions are cached once per call (ezb_controlnet_forward_cached).
+    without a ControlNet whose per-window conditions are cached once per call (ezb_controlnet_forward_cached), or with inpainting
+    operands (gt / gt_mask) whose window rows are cut once per call.
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -426,7 +427,7 @@ def check_long(lengths, B: int, window: int, overlap: int, use_cfg: bool, max_ro
 @torch.no_grad()
 def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, lengths=(), window=500, overlap=100,
                         guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device=None, use_graphs=True, *,
-                        controlnet=None, condition=None, conditioning_scale=1.0):
+                        controlnet=None, condition=None, conditioning_scale=1.0, gt=None, gt_mask=None):
     """Windowed denoising (MultiDiffusion) of clips longer than the denoiser's window: clip b has lengths[b] frames; at every step its
     latent is cut into overlapping windows of `window` frames (`overlap` frames of overlap, window_plan), the DiT denoises every window
     of every clip as one batch, each window's prediction is guided and rescaled on its own (the rescale's std is over one window, as over one
@@ -438,11 +439,21 @@ def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None
     `controlnet` (a DiTControlNet with the DiT's rows) with `condition` (B, 1, 2 * max(lengths)) fp32: clip b's condition frames are valid
     up to 2 * lengths[b], and every clip must be at least one window long, so that every window is full-length.  Window [s, s + window) of
     clip b is conditioned on condition[b, :, 2s:2s + 2 * window]; those rows go through the ControlNet's stem once per call, into its
-    condition cache (DiTControlNet.set_condition), and every step reads the cache at its timestep with `conditioning_scale`."""
+    condition cache (DiTControlNet.set_condition), and every step reads the cache at its timestep with `conditioning_scale`.
+    `gt` (B, C, max(lengths)) fp32 with `gt_mask` (B, max(lengths)) or (B, C, max(lengths)) bool, identical across channels, True =
+    regenerate: inpainting over long clips.  gt is the raw VAE latent of each clip, as sample_latents takes it; neither is read past clip
+    b's lengths[b] frames.  Once per call every window row's slice of gt (ezb_window_gather, zeros past a window's length) and of the mask
+    (ones past a window's length) is cut into static buffers that every step's DiT forward reads, so a replayed graph follows new clips and
+    masks.  The latents are returned without the paste: the caller applies pred[~mask] = gt[~mask] after scale_shift_re, as inference()
+    does.  A clip that fits one window comes out as sample_latents with that gt and mask computes it, bit for bit."""
     B = text.shape[0]
     use_cfg = bool(guidance_scale)
     desc = unet._h.desc
     max_rows, max_len = int(desc.max_batch), int(desc.max_len)
+    if gt is not None and (controlnet is not None or condition is not None):
+        raise NotImplementedError("inpainting (gt) over long clips runs without a ControlNet")
+    if (gt is None) != (gt_mask is None):
+        raise ValueError("gt and gt_mask go together")
     if controlnet is not None or condition is not None:
         if controlnet is None or condition is None:
             raise ValueError("controlnet and condition go together")
@@ -455,6 +466,11 @@ def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None
         if min(lens) < int(window):
             raise ValueError(f"with a ControlNet every clip must be at least one window ({int(window)} frames) long, got {lens}: its stem "
                              "convolutions cross a shorter window's end")
+    if gt is not None:
+        N, Cc = max(lens), unet.cfg["out_chans"]
+        if tuple(gt.shape) != (B, Cc, N) or tuple(gt_mask.shape) not in ((B, N), (B, Cc, N)):
+            raise ValueError(f"gt must be (B, C, max(lengths)) = {(B, Cc, N)} and gt_mask (B, max(lengths)) or (B, C, max(lengths)), got "
+                             f"{tuple(gt.shape)} and {tuple(gt_mask.shape)}")
     dev_index = unet._h.dev_index
     if device is not None:
         d = torch.device(device)
@@ -464,7 +480,7 @@ def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None
     with torch.cuda.device(device):
         return _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, int(window),
                                       int(overlap), guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs,
-                                      controlnet, condition, conditioning_scale)
+                                      controlnet, condition, conditioning_scale, gt, gt_mask)
 
 
 def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
@@ -476,10 +492,12 @@ def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
 
 def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, Lw, O, guidance_scale,
                            guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs, controlnet=None, condition=None,
-                           conditioning_scale=1.0):
+                           conditioning_scale=1.0, gt=None, gt_mask=None):
     B, W, N = text.shape[0], len(windows), max(lens)
     Cc = unet.cfg["out_chans"]
     use_cfg = bool(guidance_scale)
+    if gt is not None:   # the mask as one byte per frame (B, N); checked before any RNG draw
+        m1 = unet._h._mask_u8(gt_mask, B, N, device)
     dpm = getattr(noise_scheduler, "kind", "ddim") == "dpm"
     noise_scheduler.set_timesteps(ddim_steps)
     timesteps = [int(t) for t in noise_scheduler.timesteps]
@@ -516,7 +534,7 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
     draw = noise_scheduler.draws_noise if dpm else bool(eta and eta > 0)
     sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
     key = (B, W, N, Lw, O, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
-           controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()))
+           controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()), gt is not None)
     cache = unet.__dict__.setdefault("_long_cache", {})
     st = cache.get(key) if use_graphs else None
     if st is None:
@@ -526,13 +544,23 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
                   hist=torch.empty(B, Cc, N, device=device) if dpm else None,
                   plan=torch.empty(B * 3, device=device, dtype=torch.int32), wlens=torch.empty(Be, device=device, dtype=torch.int32),
                   lens=torch.empty(B, device=device, dtype=torch.int32), graph=None, launches=0,
-                  skips=None if controlnet is None else [torch.empty(Be, Lw, unet.cfg["embed_dim"], device=device) for _ in range(controlnet.half)])
+                  skips=None if controlnet is None else [torch.empty(Be, Lw, unet.cfg["embed_dim"], device=device) for _ in range(controlnet.half)],
+                  gt=None if gt is None else torch.empty(Be, Cc, Lw, device=device),
+                  m8=None if gt is None else torch.empty(Be, Lw, device=device, dtype=torch.uint8))
         if use_graphs:
             if len(cache) >= 2:
                 cache.clear()
             cache[key] = st
     st["lat"].copy_(latents)
     st["plan"].copy_(torch.tensor([e for row in table for e in row], dtype=torch.int32))
+    if gt is not None:   # constant over the schedule: every window row's gt and mask bytes, cut once per call into the static buffers
+        gsrc = gt.to(device=device, dtype=torch.float32).contiguous()
+        _lib.check(_lib.lib().ezb_window_gather(device.index, _lib.ptr(gsrc), _lib.ptr(st["gt"]), _lib.ptr(st["plan"]), B, Cc, N, W, Lw, O, Be // W,
+                                                _lib.stream_ptr()))
+        j = np.arange(Lw)   # window frame j of row (b, s, ln) is clip frame s + j of b; past ln it reads the trailing 1 (regenerate)
+        idx = np.stack([np.where(j < ln, b * N + s + j, B * N) for b, s, ln in windows])
+        src = torch.cat([m1.reshape(-1), torch.ones(1, device=device, dtype=torch.uint8)])
+        st["m8"].copy_(src[torch.from_numpy(np.tile(idx, (Be // W, 1))).to(device)])
     st["wlens"].copy_(torch.tensor([ln for _, _, ln in windows] * (Be // W), dtype=torch.int32))
     st["lens"].copy_(torch.tensor(lens, dtype=torch.int32))
     lat, x_in, out, v, noise_all, plan = st["lat"], st["x_in"], st["out"], st["v"], st["noise"], st["plan"]
@@ -547,7 +575,7 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
     def one_step(i, t):
         _lib.check(L_.ezb_window_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), B, Cc, N, W, Lw, O, Be // W, _lib.stream_ptr()))
         if controlnet is None:
-            unet.forward_step(x_in, i, out=out, lengths=st["wlens"])
+            unet.forward_step(x_in, i, gt=st["gt"], gt_mask_u8=st["m8"], out=out, lengths=st["wlens"])
         else:   # every window is full-length: no lengths, which the DiT does not combine with ControlNet skips
             sk = controlnet.forward_step(x_in, i, conditioning_scale=conditioning_scale, outs=st["skips"])
             unet.forward_step(x_in, i, controlnet_skips=sk, out=out)

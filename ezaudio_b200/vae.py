@@ -27,6 +27,39 @@ def decoder_receptive_field(cfg) -> int:
     return max(-(lo // hop), -(-(hi - (hop - 1)) // hop))
 
 
+def encoder_receptive_field(cfg) -> int:
+    """Latent frames on either side of a latent frame whose samples can change that frame (the halo encode_tiled gives each chunk): the
+    samples latent frame 0 reads, propagated back through the encoder in encoder order -- the input conv (k 7, pad 3); per stage, three
+    residual units (k 7 at dilations 1, 3, 9; the 1x1 convs reach nothing), then the strided conv (k 2s, stride s, pad ceil(s/2)), which
+    reads inputs o*s - ceil(s/2) .. o*s - ceil(s/2) + 2s - 1 for output o; and the final conv (k 3, pad 1) at the latent rate -- then rounded
+    up to whole frames of hop samples.  Walked from the latent end: [-1, 1] -> per stage (last first) -> [lo, hi] samples."""
+    lo, hi = -1, 1                                        # final conv, in latent frames
+    for s in reversed(list(cfg["strides"])):
+        p = -(-s // 2)
+        lo, hi = lo * s - p, hi * s - p + 2 * s - 1       # the strided conv's inputs
+        lo, hi = lo - 3 * (1 + 3 + 9), hi + 3 * (1 + 3 + 9)
+    lo, hi = lo - 3, hi + 3                               # input conv
+    hop = 1
+    for s in cfg["strides"]:
+        hop *= s
+    return max(-(lo // hop), -(-(hi - (hop - 1)) // hop))
+
+
+def tile_chunks(lengths, max_len: int, halo: int):
+    """The chunks decode_tiled and encode_tiled cut a batch of clips into, in latent frames: [(clip, first frame, end frame, core start,
+    core end)].  A clip of at most max_len frames is one chunk [0, n); a longer one is cut into cores of max_len - 2 * halo frames, each
+    chunk reaching `halo` frames past its core on either side, clipped to the clip's ends."""
+    core = max_len - 2 * halo
+    if core < 1:
+        raise ValueError(f"max_latent_len {max_len} leaves no core inside a halo of {halo} frames on each side")
+    chunks = []
+    for b, n in enumerate(lengths):
+        for c0 in range(0, n, core if n > max_len else n):
+            c1 = min(n, c0 + core) if n > max_len else n
+            chunks.append((b, max(0, c0 - halo), min(n, c1 + halo), c0, c1))
+    return chunks
+
+
 class OobleckDecoder:
     """OobleckDecoder (and, when `encoder_cfg` is given, OobleckEncoder + VAE bottleneck) on one ezb_vae handle."""
 
@@ -130,15 +163,7 @@ class OobleckDecoder:
         host = [L] * B if lengths is None else self._lens(lengths, B, L)[1]
         if host is None:
             raise ValueError("decode_tiled takes the lengths as a list")
-        h, M = decoder_receptive_field(self.cfg), self.max_latent_len
-        core = M - 2 * h
-        if core < 1:
-            raise ValueError(f"max_latent_len {M} leaves no core inside a halo of {h} frames on each side")
-        chunks = []   # (clip, first frame, end frame, core start, core end)
-        for b, n in enumerate(host):
-            for c0 in range(0, n, core if n > M else n):
-                c1 = min(n, c0 + core) if n > M else n
-                chunks.append((b, max(0, c0 - h), min(n, c1 + h), c0, c1))
+        chunks = tile_chunks(host, self.max_latent_len, decoder_receptive_field(self.cfg))
         wav = torch.zeros(B, 1, L * self.hop, device=self.device, dtype=torch.float32)
         hop = self.hop
         for g0 in range(0, len(chunks), self.max_batch):
@@ -167,6 +192,52 @@ class OobleckDecoder:
                 return _lib.lib().ezb_vae_encode(*args, _lib.stream_ptr())
             return _lib.lib().ezb_vae_encode_lens(*args, lb, _lib.stream_ptr())
         self._run_encode(a, T, nz, z, lens, launch)
+        return z
+
+    def encode_tiled(self, audio: torch.Tensor, noise=None, lengths=None) -> torch.Tensor:
+        """encode for clips longer than the workspace's max_latent_len, on this handle: audio (B,1,T) is zero-padded to a whole hop, each
+        clip is cut into chunks of at most max_latent_len frames (tile_chunks) whose inner edges carry a halo of encoder_receptive_field
+        frames, up to max_batch chunks go to one length-aware encode, and each chunk's core frames are pasted into the result.  Every core
+        frame depends only on samples inside its chunk, so the result equals a one-shot encode (on a workspace that holds the whole length)
+        bit for bit.  `lengths` (a list of latent frames per clip, or None for all of them): audio is a padded batch, as in encode; frames
+        past lengths[b] are zeros.  With `noise=None` the bottleneck noise of clip b is drawn from the global RNG as (1, latent, lengths[b]),
+        in clip order -- the draws of encode(lengths=list), and of consecutive solo encodes -- and each chunk reads its slice; a given
+        noise (B, latent, L) is sliced the same way; `noise=False` gives the mean."""
+        if self.encoder_cfg is None:
+            raise _lib.EzbError("this handle was created without encoder_cfg")
+        a = _as_f32c(audio).to(self.device)
+        B, ch, T = a.shape
+        if ch != 1:
+            raise ValueError("mono audio (B,1,T) expected")
+        hop, Cz = self.hop, self.cfg["latent_dim"]
+        L = -(-T // hop)
+        host = [L] * B if lengths is None else self._lens(lengths, B, L)[1]
+        if host is None:
+            raise ValueError("encode_tiled takes the lengths as a list")
+        if noise is not None and noise is not False and tuple(noise.shape) != (B, Cz, L):
+            raise ValueError(f"noise must be ({B}, {Cz}, {L}), got {tuple(noise.shape)}")
+        chunks = tile_chunks(host, self.max_latent_len, encoder_receptive_field(self.encoder_cfg))
+        if T % hop:   # strided convs floor the length; zero-pad to a whole latent frame, as encode does
+            a = torch.nn.functional.pad(a, (0, L * hop - T))
+        if noise is None:
+            noise = torch.zeros(B, Cz, L, device=self.device, dtype=torch.float32)
+            for b, n in enumerate(host):
+                noise[b, :, :n] = torch.randn(1, Cz, n, device=self.device, dtype=torch.float32)[0]
+        elif noise is not False:
+            noise = _as_f32c(noise).to(self.device)
+        z = torch.zeros(B, Cz, L, device=self.device, dtype=torch.float32)
+        for g0 in range(0, len(chunks), self.max_batch):
+            group = chunks[g0:g0 + self.max_batch]
+            Lc = max(e - s for _, s, e, _, _ in group)
+            xs = torch.zeros(len(group), 1, Lc * hop, device=self.device, dtype=torch.float32)
+            ns = False if noise is False else torch.zeros(len(group), Cz, Lc, device=self.device, dtype=torch.float32)
+            for k, (b, s, e, _, _) in enumerate(group):
+                xs[k, :, :(e - s) * hop] = a[b, :, s * hop:e * hop]
+                if ns is not False:
+                    ns[k, :, :e - s] = noise[b, :, s:e]
+            zs = self.encode(xs, noise=ns, lengths=[e - s for _, s, e, _, _ in group])
+            for k, (b, s, _, c0, c1) in enumerate(group):
+                z[b, :, c0:c1] = zs[k, :, c0 - s:c1 - s]
         return z
 
     def encode_noised(self, audio: torch.Tensor, ab, eps: torch.Tensor, scale: float, shift: float, noise=None, lengths=None) -> torch.Tensor:
