@@ -135,6 +135,8 @@ _SIGS = {
     "ezb_cfg_dpm_step_slots": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP], _I),
     "ezb_window_gather": ([_I, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_window_blend": ([_I, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_loop_gather": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_loop_blend": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition": ([_VP, _VP, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition_rows": ([_VP, _VP, _I, _I, _I, _VP], _I),
     "ezb_controlnet_forward_tdev": ([_VP, _VP, _VP, _VP, C.POINTER(_VP), _I, _I, _VP], _I),

@@ -19,7 +19,7 @@ import torch
 from . import _lib, config, post, weights
 from ._lib import EzbError
 from .dit import DiTControlNet, MaskDiT
-from .inference import check_long, inference, make_generators, sample_long_latents, scale_shift_re
+from .inference import check_long, check_loop, inference, make_generators, sample_long_latents, sample_loop_latents, scale_shift_re
 from .scheduler import DDIMScheduler, start_index
 from .vae import Autoencoder, OobleckDecoder
 
@@ -425,6 +425,44 @@ class EzAudio(_Base):
                                   guidance_rescale, ddim_steps, eta, random_seed)
         p = self.params["autoencoder"]
         wav = self.autoencoder.decoder.decode_tiled(scale_shift_re(lat, p["scale"], p["shift"]), lengths=frames)
+        hop = self.autoencoder.decoder.hop
+        out = [wav[b, 0, :hop * n].cpu().numpy() for b, n in enumerate(frames)]
+        return (p["sr"], out) if batched else (p["sr"], out[0])
+
+    def generate_loop_audio(self, text, length, window_length=10, overlap=2, guidance_scale=5, guidance_rescale=0.75, ddim_steps=100, eta=1,
+                            random_seed=None, randomize_seed=False):
+        """Seamless loops: audio whose last sample runs on into its first, for ambience and effect beds played on repeat.  The latent is
+        denoised as a circle (`inference.sample_loop_latents`): windows of `window_length` seconds overlapping by at least `overlap` seconds
+        wrap around the loop's end, and all of them move by a golden-ratio stride at every step, so the seam is denoised in context like
+        any other frame.  The loop is then decoded with halos that wrap around (`OobleckDecoder.decode_loop`).  Prompts, lengths (seconds,
+        one value or one per prompt) and seeds are as in generate_long_audio.  Returns (sr, waveform) or (sr, [waveforms]) with
+        hop * int(length * latent_sr) samples each.  The windows (x 2 with guidance) must fit the DiT's 2 * max_batch rows."""
+        batched = not isinstance(text, str)
+        prompts = list(text) if batched else [text]
+        B = len(prompts)
+        latent_sr = self.params["autoencoder"]["latent_sr"]
+        # ---- everything is checked on the host before any device work
+        num = (int, float, np.integer, np.floating)
+        frames = [int(v * latent_sr) for v in _per_clip("length", length, B, num)]
+        if B < 1 or any(f < 2 for f in frames):
+            raise ValueError(f"every loop must be at least two latent frames ({2 / latent_sr} s) long, got {length}")
+        if window_length > self.max_length_s:
+            raise ValueError(f"window_length {window_length} s exceeds max_length_s {self.max_length_s} s")
+        window, hop_over = int(window_length * latent_sr), int(overlap * latent_sr)
+        empty = [t == "" for t in prompts]
+        if any(empty) and not all(empty):
+            raise ValueError("empty prompts run without guidance: they cannot share a batch with non-empty ones")
+        if all(empty):
+            guidance_scale = None
+            print("empyt input")
+        check_loop(frames, B, window, hop_over, bool(guidance_scale), int(self.unet._h.desc.max_batch), int(self.unet._h.desc.max_len))
+        if randomize_seed:
+            random_seed = random.randint(0, MAX_SEED)
+        text_emb, mask, uemb, umask = self._text_embeds(prompts, [""])
+        lat = sample_loop_latents(self.unet, self.noise_scheduler, text_emb, mask, uemb, umask, frames, window, hop_over, guidance_scale,
+                                  guidance_rescale, ddim_steps, eta, random_seed)
+        p = self.params["autoencoder"]
+        wav = self.autoencoder.decoder.decode_loop(scale_shift_re(lat, p["scale"], p["shift"]), lengths=frames)
         hop = self.autoencoder.decoder.hop
         out = [wav[b, 0, :hop * n].cpu().numpy() for b, n in enumerate(frames)]
         return (p["sr"], out) if batched else (p["sr"], out[0])

@@ -1194,4 +1194,24 @@ EZB_API int ezb_prof_gemm_stats(double min_flops, int* launches, double* flops, 
   return EZB_OK;
 }
 
+EZB_API int ezb_loop_gather(int device, const float* latents, float* windows, const int32_t* plan_dev, const int32_t* offsets_dev, int B, int C,
+                            int Nmax, int W, int Lw, int overlap, int copies, void* stream) {
+  if (!latents || !windows || !plan_dev || !offsets_dev || B < 1 || C < 1 || Nmax < 1 || W < B || Lw < 2 || overlap < 1 || overlap > Lw / 2 ||
+      (copies != 1 && copies != 2))
+    return fail(EZB_ERR_ARG, "ezb_loop_gather: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(loop_gather_launch(ST(stream), LoopPlan{plan_dev, offsets_dev, B, C, Nmax, W, Lw, overlap}, latents, windows, copies));
+  return EZB_OK;
+}
+EZB_API int ezb_loop_blend(int device, const float* windows, float* out, const int32_t* plan_dev, const int32_t* offsets_dev, int B, int C, int Nmax,
+                           int W, int Lw, int overlap, void* stream) {
+  if (!windows || !out || !plan_dev || !offsets_dev || B < 1 || C < 1 || Nmax < 1 || W < B || Lw < 2 || overlap < 1 || overlap > Lw / 2)
+    return fail(EZB_ERR_ARG, "ezb_loop_blend: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(loop_blend_launch(ST(stream), LoopPlan{plan_dev, offsets_dev, B, C, Nmax, W, Lw, overlap}, windows, out));
+  return EZB_OK;
+}
+
 }  // extern "C"

@@ -21,4 +21,19 @@ cudaError_t window_gather_launch(cudaStream_t st, const WindowPlan& p, const flo
 // windows (W, C, Lw) -> out (B, C, Nmax): the weighted mean of the windows covering each frame < N; frames >= N are not written
 cudaError_t window_blend_launch(cudaStream_t st, const WindowPlan& p, const float* windows, float* out);
 
+// Seamless loops: the same gather and blend on a circle, where frame N - 1 of loop b is followed by frame 0.  Loop b (N frames, table row
+// (first, count, N) as above) has windows of Lw_b = min(Lw, N) frames: count == 1 when N <= Lw, else count = ceil(N / (Lw - O)).  At a
+// step with offset r (offsets[b], DEVICE int32, read when the kernels run), window k starts at s_k = ((k * N) / count + r) mod N and reads
+// frames (s_k + j) mod N, j < Lw_b.  Its weight at local frame j is 1 for a one-window loop, else min(1, (j + 1) / (O + 1),
+// (Lw_b - j) / (O + 1)).  ezaudio_b200.inference.loop_plan is the same plan on the host.  These kernels are separate from the linear
+// ones: a wrap there would put a branch in shared code and change their machine code.
+struct LoopPlan { const int32_t* plan; const int32_t* offsets; int B, C, Nmax, W, Lw, overlap; };
+
+// latents (B, C, Nmax) -> windows (copies * W, C, Lw): row r (and row W + r when copies == 2) holds its window's frames, zeros past Lw_b
+cudaError_t loop_gather_launch(cudaStream_t st, const LoopPlan& p, const float* latents, float* windows, int copies);
+// windows (W, C, Lw) -> out (B, C, Nmax): frame f < N gets the weighted mean of the windows covering it, summed in decreasing local index
+// j (so the order depends only on where f sits in each window, and a common shift of every offset shifts the result exactly); frames
+// >= N are not written
+cudaError_t loop_blend_launch(cudaStream_t st, const LoopPlan& p, const float* windows, float* out);
+
 }  // namespace ezb

@@ -14,7 +14,9 @@ Differences from the reference loop, all additive:
   * clips longer than the denoiser's window (`sample_long_latents`): overlapping windows denoised as one batch, guided per window and
     crossfaded on the device into one long prediction at every step (MultiDiffusion; ezb_window_gather / ezb_window_blend), with or
     without a ControlNet whose per-window conditions are cached once per call (ezb_controlnet_forward_cached), or with inpainting
-    operands (gt / gt_mask) whose window rows are cut once per call.
+    operands (gt / gt_mask) whose window rows are cut once per call;
+  * seamless loops (`sample_loop_latents`): the same windowed loop on a circle, the windows wrapping around the loop's end and shifting
+    by a golden-ratio stride at every step (ezb_loop_gather / ezb_loop_blend).
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -424,6 +426,109 @@ def check_long(lengths, B: int, window: int, overlap: int, use_cfg: bool, max_ro
     return lens, table, windows
 
 
+GOLDEN_STRIDE = 0.3819660112501051   # 2 - phi: the per-step shift of a loop's windows, as a fraction of the loop
+
+
+def loop_plan(n: int, window: int, overlap: int):
+    """The windows of a seamless loop of n frames (frame n - 1 followed by frame 0; include/ezb200.h, ezb_loop_gather): (count, length).
+    n <= window is one window of n frames, the whole circle; otherwise ceil(n / (window - overlap)) windows of `window` frames, window k
+    starting at floor(k * n / count) (plus the step's offset, mod n, loop_starts), so neighbours overlap by at least `overlap` frames."""
+    if not 1 <= overlap <= window // 2:
+        raise ValueError(f"overlap must lie in 1..{window // 2} frames (half the window of {window}), got {overlap}")
+    if n < 2:
+        raise ValueError(f"a loop needs at least 2 frames, got {n}")
+    if n <= window:
+        return 1, n
+    return -(-n // (window - overlap)), window
+
+
+def loop_starts(n: int, count: int, offset: int):
+    """Start frames of a loop's windows at a step with offset r: ((k * n) // count + r) mod n."""
+    return [((k * n) // count + offset) % n for k in range(count)]
+
+
+def loop_stride(n: int) -> int:
+    """R = floor(n * (2 - phi) + 0.5): the golden-ratio stride by which a loop's windows move from one step to the next."""
+    return int(np.floor(n * GOLDEN_STRIDE + 0.5))
+
+
+def loop_offsets(lengths, nsteps: int):
+    """The shift schedule [steps][B]: r_{i,b} = (i * R_b) mod N_b.  It moves the seam between windows, and the DiT input edges, to a
+    different place at every step; for a one-window loop it is what denoises the wrap-around in context."""
+    return [[(i * loop_stride(n)) % n for n in lengths] for i in range(nsteps)]
+
+
+def loop_weights(count: int, length: int, overlap: int):
+    """fp32 weights of a loop window over its `length` frames: 1 for a one-window loop, else min(1, (j + 1) / (overlap + 1),
+    (length - j) / (overlap + 1)) -- both ends taper, since on a circle every window has two neighbours -- as the blend kernel computes them."""
+    if count == 1:
+        return np.ones(length, dtype=np.float32)
+    j = np.arange(length)
+    o1 = np.float32(overlap + 1)
+    return np.minimum(np.float32(1), np.minimum((j + 1).astype(np.float32) / o1, (length - j).astype(np.float32) / o1))
+
+
+def check_loop(lengths, B: int, window: int, overlap: int, use_cfg: bool, max_rows: int, max_len: int):
+    """Validates a seamless-loop run on the host before any device work; returns (lengths, plan table [(first row, count, N)] per loop,
+    the windows [(loop, 0, length)] in row order -- their starts move with every step's offset)."""
+    lens = [int(v) for v in lengths]
+    if len(lens) != B or any(v != w for v, w in zip(lens, lengths)) or any(v < 2 for v in lens):
+        raise ValueError(f"lengths lists one whole frame count >= 2 per loop ({B} loops), got {list(lengths)}")
+    if not 2 <= int(window) <= max_len:
+        raise ValueError(f"window must lie in 2..{max_len} frames (the denoiser's max_len), got {window}")
+    table, windows = [], []
+    for b, n in enumerate(lens):
+        count, ln = loop_plan(n, int(window), int(overlap))
+        table.append((len(windows), count, n))
+        windows += [(b, 0, ln)] * count
+    rows = len(windows) * (2 if use_cfg else 1)
+    if rows > max_rows:
+        raise ValueError(f"{len(windows)} windows{' x 2 (CFG)' if use_cfg else ''} = {rows} DiT rows exceed the row capacity {max_rows} "
+                         f"(2 * max_batch): needs max_batch >= {-(-rows // 2)}")
+    return lens, table, windows
+
+
+@torch.no_grad()
+def sample_loop_latents(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lengths, window, overlap, guidance_scale,
+                        guidance_rescale, ddim_steps, eta, random_seed, *, offsets=None, init_noise=None, step_noise=None, device=None,
+                        use_graphs=True):
+    """Seamless loops: windowed denoising (as sample_long_latents) on a circle, where frame lengths[b] - 1 of loop b is followed by its
+    frame 0.  At step i the windows of loop b (loop_plan) start at ((k * N_b) // count + r_{i,b}) mod N_b, with the golden-ratio shift
+    schedule r = loop_offsets(lengths, steps); the gather (ezb_loop_gather) wraps around, the DiT denoises every window of every loop as
+    one batch, each window is guided on its own, and the blend (ezb_loop_blend, weights loop_weights) drives the DDIM or DPM-Solver++ update
+    of the loop latent.  Returns the latents (B, C, max(lengths)) fp32 on the device, zero past each loop's end.  Loop b's generator
+    (random_seed as in sample_latents) draws the initial and per-step noise at (1, C, lengths[b]).  The whole schedule is one captured
+    graph; the plan and every step's offsets are read on the device.
+    `offsets` ([steps][B] ints) replaces the shift schedule; `init_noise` (B, C, max(lengths)) and `step_noise` (one (B, C, max(lengths))
+    per step) replace the generator draws; frames past a loop's end are not read.  With all offsets 0, a loop that fits one window is
+    sample_latents at that length, bit for bit; adding d to every offset with the noise rolled by d rolls the result by d, bit for bit."""
+    B = text.shape[0]
+    use_cfg = bool(guidance_scale)
+    desc = unet._h.desc
+    lens, table, windows = check_loop(lengths, B, window, overlap, use_cfg, int(desc.max_batch), int(desc.max_len))
+    noise_scheduler.set_timesteps(ddim_steps)
+    nsteps, N, Cc = len(noise_scheduler.timesteps), max(lens), unet.cfg["out_chans"]
+    if offsets is None:
+        offsets = loop_offsets(lens, nsteps)
+    offs = [[int(v) for v in row] for row in offsets]
+    if len(offs) != nsteps or any(len(row) != B for row in offs):
+        raise ValueError(f"offsets lists {B} ints per step for {nsteps} steps")
+    if init_noise is not None and tuple(init_noise.shape) != (B, Cc, N):
+        raise ValueError(f"init_noise must be {(B, Cc, N)}, got {tuple(init_noise.shape)}")
+    if step_noise is not None and (len(step_noise) != nsteps or any(tuple(s.shape) != (B, Cc, N) for s in step_noise)):
+        raise ValueError(f"step_noise lists one {(B, Cc, N)} tensor per step ({nsteps} steps)")
+    dev_index = unet._h.dev_index
+    if device is not None:
+        d = torch.device(device)
+        if d.type != "cuda" or (d.index is not None and d.index != dev_index):
+            raise ValueError(f"sample_loop_latents(device={d}) but the denoiser lives on cuda:{dev_index}")
+    device = torch.device("cuda", dev_index)
+    with torch.cuda.device(device):
+        return _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, int(window),
+                                      int(overlap), guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs,
+                                      offsets=offs, init_noise=init_noise, step_noise=step_noise)
+
+
 @torch.no_grad()
 def sample_long_latents(unet, noise_scheduler, text, text_mask, uncond_text=None, uncond_mask=None, lengths=(), window=500, overlap=100,
                         guidance_scale=3, guidance_rescale=0.0, ddim_steps=50, eta=1, random_seed=2024, device=None, use_graphs=True, *,
@@ -492,8 +597,12 @@ def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
 
 def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, Lw, O, guidance_scale,
                            guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs, controlnet=None, condition=None,
-                           conditioning_scale=1.0, gt=None, gt_mask=None):
+                           conditioning_scale=1.0, gt=None, gt_mask=None, offsets=None, init_noise=None, step_noise=None):
+    """The windowed loop of sample_long_latents, and of sample_loop_latents when `offsets` ([steps][B] ints, the loops' shifts) is given:
+    then the circular gather and blend (ezb_loop_gather / ezb_loop_blend) read step i's row of a device offsets table in place of the
+    linear ones, and the schedule is captured into a cache of its own.  init_noise / step_noise (loops only) replace the draws."""
     B, W, N = text.shape[0], len(windows), max(lens)
+    loop = offsets is not None
     Cc = unet.cfg["out_chans"]
     use_cfg = bool(guidance_scale)
     if gt is not None:   # the mask as one byte per frame (B, N); checked before any RNG draw
@@ -505,7 +614,10 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
     gens = make_generators(random_seed, B, device)
     latents = torch.zeros((B, Cc, N), device=device)
     for b, g in enumerate(gens):
-        latents[b, :, :lens[b]] = torch.randn((1, Cc, lens[b]), generator=g, device=device)[0]
+        if init_noise is None:
+            latents[b, :, :lens[b]] = torch.randn((1, Cc, lens[b]), generator=g, device=device)[0]
+        else:
+            latents[b, :, :lens[b]] = init_noise[b, :, :lens[b]].to(device=device, dtype=torch.float32)
 
     # the T5 context of every window row: [text of each window | "" of each window]
     clip_of = torch.tensor([b for b, _, _ in windows], device=device)
@@ -535,7 +647,7 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
     sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
     key = (B, W, N, Lw, O, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
            controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()), gt is not None)
-    cache = unet.__dict__.setdefault("_long_cache", {})
+    cache = unet.__dict__.setdefault("_loop_long_cache" if loop else "_long_cache", {})
     st = cache.get(key) if use_graphs else None
     if st is None:
         st = dict(lat=torch.empty(B, Cc, N, device=device), x_in=torch.empty(Be, Cc, Lw, device=device), out=torch.empty(Be, Cc, Lw, device=device),
@@ -546,7 +658,8 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
                   lens=torch.empty(B, device=device, dtype=torch.int32), graph=None, launches=0,
                   skips=None if controlnet is None else [torch.empty(Be, Lw, unet.cfg["embed_dim"], device=device) for _ in range(controlnet.half)],
                   gt=None if gt is None else torch.empty(Be, Cc, Lw, device=device),
-                  m8=None if gt is None else torch.empty(Be, Lw, device=device, dtype=torch.uint8))
+                  m8=None if gt is None else torch.empty(Be, Lw, device=device, dtype=torch.uint8),
+                  offs=torch.empty(nsteps, B, device=device, dtype=torch.int32) if loop else None)
         if use_graphs:
             if len(cache) >= 2:
                 cache.clear()
@@ -563,17 +676,27 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
         st["m8"].copy_(src[torch.from_numpy(np.tile(idx, (Be // W, 1))).to(device)])
     st["wlens"].copy_(torch.tensor([ln for _, _, ln in windows] * (Be // W), dtype=torch.int32))
     st["lens"].copy_(torch.tensor(lens, dtype=torch.int32))
+    if loop:   # read when the kernels run: a replayed graph follows new offsets
+        st["offs"].copy_(torch.tensor(offsets, dtype=torch.int32))
     lat, x_in, out, v, noise_all, plan = st["lat"], st["x_in"], st["out"], st["v"], st["noise"], st["plan"]
     if noise_all is not None:   # step i, prompt b: the (1, C, lengths[b]) draw of a solo run, in step order
         for i in range(nsteps):
             for b, g in enumerate(gens):
-                noise_all[i, b, :, :lens[b]] = torch.empty((1, Cc, lens[b]), device=device).normal_(generator=g)[0]
+                if step_noise is None:
+                    noise_all[i, b, :, :lens[b]] = torch.empty((1, Cc, lens[b]), device=device).normal_(generator=g)[0]
+                else:
+                    noise_all[i, b, :, :lens[b]] = step_noise[i][b, :, :lens[b]].to(device=device, dtype=torch.float32)
     dpm_coef = [noise_scheduler.step_coefficients(i) for i in range(nsteps)] if dpm else None
     gs, gr = (float(guidance_scale), float(guidance_rescale or 0.0)) if use_cfg else (0.0, 0.0)
     L_ = _lib.lib()
 
     def one_step(i, t):
-        _lib.check(L_.ezb_window_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), B, Cc, N, W, Lw, O, Be // W, _lib.stream_ptr()))
+        if loop:
+            _lib.check(L_.ezb_loop_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), _lib.ptr(st["offs"][i]), B, Cc, N, W, Lw, O,
+                                          Be // W, _lib.stream_ptr()))
+        else:
+            _lib.check(L_.ezb_window_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), B, Cc, N, W, Lw, O, Be // W,
+                                            _lib.stream_ptr()))
         if controlnet is None:
             unet.forward_step(x_in, i, gt=st["gt"], gt_mask_u8=st["m8"], out=out, lengths=st["wlens"])
         else:   # every window is full-length: no lengths, which the DiT does not combine with ControlNet skips
@@ -583,7 +706,11 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
         if use_cfg:
             _guide_windows(out, st["guided"], W, Cc, Lw, gs, gr, st["wlens"][:W])
             src = st["guided"]
-        _lib.check(L_.ezb_window_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), B, Cc, N, W, Lw, O, _lib.stream_ptr()))
+        if loop:
+            _lib.check(L_.ezb_loop_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), _lib.ptr(st["offs"][i]), B, Cc, N, W, Lw, O,
+                                         _lib.stream_ptr()))
+        else:
+            _lib.check(L_.ezb_window_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), B, Cc, N, W, Lw, O, _lib.stream_ptr()))
         nz = None if noise_all is None else noise_all[i]
         if dpm:
             coef, order = dpm_coef[i]

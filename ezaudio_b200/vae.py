@@ -60,6 +60,21 @@ def tile_chunks(lengths, max_len: int, halo: int):
     return chunks
 
 
+def loop_chunks(lengths, max_len: int, halo: int):
+    """The chunks decode_loop cuts a batch of seamless loops into: [(loop, core start, core end, frames)].  A loop of n frames is cut into
+    cores of at most max_len - 2 * halo frames (one core [0, n) when it fits); each chunk is its core with `halo` frames on either side,
+    the frame indices taken mod n, so the halos wrap around the loop's ends (more than once when n < halo)."""
+    core = max_len - 2 * halo
+    if core < 1:
+        raise ValueError(f"max_latent_len {max_len} leaves no core inside a halo of {halo} frames on each side")
+    chunks = []
+    for b, n in enumerate(lengths):
+        for c0 in range(0, n, core):
+            c1 = min(n, c0 + core)
+            chunks.append((b, c0, c1, [f % n for f in range(c0 - halo, c1 + halo)]))
+    return chunks
+
+
 class OobleckDecoder:
     """OobleckDecoder (and, when `encoder_cfg` is given, OobleckEncoder + VAE bottleneck) on one ezb_vae handle."""
 
@@ -175,6 +190,33 @@ class OobleckDecoder:
             ws = self(zs, lengths=[e - s for _, s, e, _, _ in group])
             for k, (b, s, _, c0, c1) in enumerate(group):
                 wav[b, :, c0 * hop:c1 * hop] = ws[k, :, (c0 - s) * hop:(c1 - s) * hop]
+        return wav
+
+    def decode_loop(self, z: torch.Tensor, lengths=None) -> torch.Tensor:
+        """Seamless decode of loops: z (B,latent,L), loop b being its first lengths[b] frames (all L for None), followed by its frame 0
+        after its last -> (B,1,hop*L), samples past hop * lengths[b] zero.  decode_tiled on a circle: each loop is cut into cores of at most
+        max_latent_len - 2h frames (h = decoder_receptive_field) carrying h halo frames on either side taken mod lengths[b] (loop_chunks),
+        the chunks are gathered by one index, up to max_batch go to one length-aware decode, and their cores are pasted.  Every core sample
+        depends only on frames inside its chunk, so loop b's samples equal the middle period of a one-shot decode of the loop repeated,
+        bit for bit: sample hop * lengths[b] - 1 runs on into sample 0."""
+        z = _as_f32c(z).to(self.device)
+        B, Cz, L = z.shape
+        host = [L] * B if lengths is None else self._lens(lengths, B, L)[1]
+        if host is None:
+            raise ValueError("decode_loop takes the lengths as a list")
+        h = decoder_receptive_field(self.cfg)
+        chunks = loop_chunks(host, self.max_latent_len, h)
+        wav = torch.zeros(B, 1, L * self.hop, device=self.device, dtype=torch.float32)
+        hop = self.hop
+        zf = z.transpose(0, 1).reshape(Cz, B * L)
+        for g0 in range(0, len(chunks), self.max_batch):
+            group = chunks[g0:g0 + self.max_batch]
+            Lc = max(len(fr) for *_, fr in group)
+            idx = torch.tensor([[b * L + f for f in fr] + [b * L] * (Lc - len(fr)) for b, _, _, fr in group], dtype=torch.int64)
+            zs = zf[:, idx.to(self.device)].transpose(0, 1).contiguous()   # (chunks, latent, Lc); past a chunk's length never read
+            ws = self(zs, lengths=[len(fr) for *_, fr in group])
+            for k, (b, c0, c1, _) in enumerate(group):
+                wav[b, :, c0 * hop:c1 * hop] = ws[k, :, h * hop:(h + c1 - c0) * hop]
         return wav
 
     def encode(self, audio: torch.Tensor, noise=None, lengths=None) -> torch.Tensor:

@@ -9,7 +9,7 @@
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
  * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev, controlnet_forward_cached,
- * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, window_gather, window_blend, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
+ * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, window_gather, window_blend, loop_gather, loop_blend, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
  */
@@ -182,6 +182,22 @@ int ezb_window_gather(int device, const float* latents, float* windows, const in
                       int overlap, int copies, void* stream);
 int ezb_window_blend(int device, const float* windows, float* out, const int32_t* plan_dev, int B, int C, int Nmax, int W, int Lw, int overlap,
                      void* stream);
+
+/* Seamless loops: windowed denoising on a circle, where frame N_b - 1 of loop b is followed by frame 0.  plan_dev is the table above, with
+ * the windows of loop b: N_b <= Lw is one window of Lw_b = N_b frames, otherwise n_b = ceil(N_b / (Lw - overlap)) windows of Lw_b = Lw
+ * frames.  offsets_dev: DEVICE int32 [B], the step's shift r_b, read when the kernels run (a captured schedule passes each step's row of a
+ * [steps][B] table).  Window k of loop b starts at s_k = (floor(k * N_b / n_b) + r_b) mod N_b and holds frames (s_k + j) mod N_b, j < Lw_b;
+ * its weight at j is 1 when n_b == 1, else min(1, (j + 1) / (overlap + 1), (Lw_b - j) / (overlap + 1)).  ezaudio_b200.inference.loop_plan
+ * builds the table.
+ * ezb_loop_gather: window row r gets its frames and zeros past Lw_b; copies 2 writes the same rows again at row offset W.
+ * ezb_loop_blend: frame f < N_b gets sum w v / sum w over the windows covering it, summed in decreasing local index j (the first term
+ *   starting both sums), in fp32, the division IEEE-rounded.  The order depends only on where f sits in each window, so adding d to every
+ *   offset (with the latents rolled by d) rolls the result by d exactly; one covering window of weight 1 gives its value bit for bit.  Window
+ *   frames past Lw_b and frames at or past N_b are neither read nor written. */
+int ezb_loop_gather(int device, const float* latents, float* windows, const int32_t* plan_dev, const int32_t* offsets_dev, int B, int C, int Nmax,
+                    int W, int Lw, int overlap, int copies, void* stream);
+int ezb_loop_blend(int device, const float* windows, float* out, const int32_t* plan_dev, const int32_t* offsets_dev, int B, int C, int Nmax, int W,
+                   int Lw, int overlap, void* stream);
 
 /* --- VAE decoder: OobleckDecoder.forward (stable_vae/models/autoencoders.py:149-190) behind
  * Autoencoder(embedding=z) (src/modules/autoencoder_wrapper.py:74-77). */
