@@ -137,6 +137,9 @@ _SIGS = {
     "ezb_window_blend": ([_I, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_loop_gather": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_loop_blend": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_timeline_gather": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP], _I),
+    "ezb_timeline_guide": ([_I, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _F, _F, _VP], _I),
+    "ezb_timeline_blend": ([_I, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition": ([_VP, _VP, _I, _I, _VP], _I),
     "ezb_controlnet_set_condition_rows": ([_VP, _VP, _I, _I, _I, _VP], _I),
     "ezb_controlnet_forward_tdev": ([_VP, _VP, _VP, _VP, C.POINTER(_VP), _I, _I, _VP], _I),

@@ -19,7 +19,8 @@ import torch
 from . import _lib, config, post, weights
 from ._lib import EzbError
 from .dit import DiTControlNet, MaskDiT
-from .inference import check_long, check_loop, inference, make_generators, sample_long_latents, sample_loop_latents, scale_shift_re
+from .inference import (check_long, check_loop, check_timeline, inference, make_generators, sample_long_latents, sample_loop_latents,
+                        sample_timeline_latents, scale_shift_re)
 from .scheduler import DDIMScheduler, start_index
 from .vae import Autoencoder, OobleckDecoder
 
@@ -463,6 +464,57 @@ class EzAudio(_Base):
                                   guidance_rescale, ddim_steps, eta, random_seed)
         p = self.params["autoencoder"]
         wav = self.autoencoder.decoder.decode_loop(scale_shift_re(lat, p["scale"], p["shift"]), lengths=frames)
+        hop = self.autoencoder.decoder.hop
+        out = [wav[b, 0, :hop * n].cpu().numpy() for b, n in enumerate(frames)]
+        return (p["sr"], out) if batched else (p["sr"], out[0])
+
+    def generate_timeline_audio(self, timeline, length=None, window_length=10, overlap=2, transition=1, guidance_scale=5, guidance_rescale=0.75,
+                                ddim_steps=100, eta=1, random_seed=None, randomize_seed=False):
+        """Long clips whose prompt changes over time: soundtracks, ambience beds that evolve, sound design for video.  `timeline` is one
+        clip's list of (prompt, start_s, end_s) segments, or a list of such lists for a batch; segments may overlap, and together they must
+        cover the clip.  `length` (seconds, one value or one per clip) defaults to the clip's largest end_s.  The clip is denoised in
+        windows as in generate_long_audio (`inference.sample_timeline_latents`): each window carries one conditioned row per segment within
+        `transition` seconds of it, those rows share one unconditional row, and each row's prediction is weighted by its segment's weight,
+        1 inside the segment and tapering over `transition` seconds on either side (two abutting segments crossfade over 2 * transition
+        seconds; 0 switches hard).  Seeds as in generate_long_audio.  Returns (sr, waveform) or (sr, [waveforms]) with
+        hop * int(length * latent_sr) samples each.  The conditioned rows plus one unconditional row per window must fit the DiT's
+        2 * max_batch rows.  A one-segment timeline equals generate_long_audio with that prompt, bit for bit."""
+        batched = len(timeline) > 0 and not (isinstance(timeline[0], (tuple, list)) and len(timeline[0]) > 0 and isinstance(timeline[0][0], str))
+        clips = [list(c) for c in timeline] if batched else [list(timeline)]
+        B = len(clips)
+        latent_sr = self.params["autoencoder"]["latent_sr"]
+        # ---- everything is checked on the host before any device work
+        num = (int, float, np.integer, np.floating)
+        if B < 1 or any(not c for c in clips):
+            raise ValueError("a timeline lists at least one (prompt, start_s, end_s) segment")
+        for c in clips:
+            for seg in c:
+                if len(seg) != 3 or not isinstance(seg[0], str) or not isinstance(seg[1], num) or not isinstance(seg[2], num):
+                    raise ValueError(f"a timeline segment is (prompt, start_s, end_s), got {seg!r}")
+        if length is None:
+            length = [max(e for _, _, e in c) for c in clips]
+        frames = [int(v * latent_sr) for v in _per_clip("length", length, B, num)]
+        if any(f < 1 for f in frames):
+            raise ValueError(f"every length must be positive (at least one latent frame), got {length}")
+        if window_length > self.max_length_s:
+            raise ValueError(f"window_length {window_length} s exceeds max_length_s {self.max_length_s} s")
+        if transition < 0:
+            raise ValueError(f"transition must be >= 0 seconds, got {transition}")
+        window, hop_over, T = int(window_length * latent_sr), int(overlap * latent_sr), int(transition * latent_sr)
+        segs = [[(round(s * latent_sr), min(round(e * latent_sr), n)) for _, s, e in c] for c, n in zip(clips, frames)]
+        if all(p == "" for c in clips for p, _, _ in c):
+            guidance_scale = None
+        check_timeline(segs, frames, B, window, hop_over, T, bool(guidance_scale), int(self.unet._h.desc.max_batch), int(self.unet._h.desc.max_len))
+        if randomize_seed:
+            random_seed = random.randint(0, MAX_SEED)
+        prompts = list(dict.fromkeys(p for c in clips for p, _, _ in c))   # each distinct prompt is encoded once
+        index = {p: i for i, p in enumerate(prompts)}
+        text_emb, mask, uemb, umask = self._text_embeds(prompts, [""])
+        segments = [[(index[p], s, e) for (p, _, _), (s, e) in zip(c, sg)] for c, sg in zip(clips, segs)]
+        lat = sample_timeline_latents(self.unet, self.noise_scheduler, text_emb, mask, uemb, umask, segments, frames, window, hop_over, T,
+                                      guidance_scale, guidance_rescale, ddim_steps, eta, random_seed)
+        p = self.params["autoencoder"]
+        wav = self.autoencoder.decoder.decode_tiled(scale_shift_re(lat, p["scale"], p["shift"]), lengths=frames)
         hop = self.autoencoder.decoder.hop
         out = [wav[b, 0, :hop * n].cpu().numpy() for b, n in enumerate(frames)]
         return (p["sr"], out) if batched else (p["sr"], out[0])

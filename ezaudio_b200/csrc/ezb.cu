@@ -7,6 +7,7 @@
 #include "t5.cuh"
 #include "host.cuh"
 #include "longform.cuh"
+#include "timeline.cuh"
 
 using namespace ezb;
 
@@ -1211,6 +1212,37 @@ EZB_API int ezb_loop_blend(int device, const float* windows, float* out, const i
   EZB_CUDA(cudaSetDevice(device));
   ++launch_counter();
   EZB_CUDA(loop_blend_launch(ST(stream), LoopPlan{plan_dev, offsets_dev, B, C, Nmax, W, Lw, overlap}, windows, out));
+  return EZB_OK;
+}
+
+EZB_API int ezb_timeline_gather(int device, const float* latents, float* windows, const int32_t* plan_dev, const int32_t* rows_dev, int B, int C,
+                                int Nmax, int W, int R, int Lw, int overlap, int uncond, void* stream) {
+  if (!latents || !windows || !plan_dev || !rows_dev || !aligned16(rows_dev) || B < 1 || C < 1 || Nmax < 1 || W < B || R < W || Lw < 2 ||
+      overlap < 1 || overlap > Lw / 2 || (uncond != 0 && uncond != 1))
+    return fail(EZB_ERR_ARG, "ezb_timeline_gather: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(timeline_gather_launch(ST(stream), TimelinePlan{WindowPlan{plan_dev, B, C, Nmax, W, Lw, overlap}, rows_dev, nullptr, R}, latents, windows,
+                                  uncond));
+  return EZB_OK;
+}
+EZB_API int ezb_timeline_guide(int device, const float* model_out, float* guided, const int32_t* rows_dev, const int32_t* lens_dev, int R, int W, int C,
+                               int Lw, float gs, float gr, void* stream) {
+  if (!model_out || !guided || !rows_dev || !lens_dev || !aligned16(rows_dev) || W < 1 || R < W || C < 1 || Lw < 1)
+    return fail(EZB_ERR_ARG, "ezb_timeline_guide: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(timeline_guide_launch(ST(stream), model_out, guided, rows_dev, lens_dev, R, W, C, Lw, gs, gr));
+  return EZB_OK;
+}
+EZB_API int ezb_timeline_blend(int device, const float* windows, float* out, const int32_t* plan_dev, const int32_t* rows_dev, const int32_t* spans_dev,
+                               int B, int C, int Nmax, int W, int R, int Lw, int overlap, void* stream) {
+  if (!windows || !out || !plan_dev || !rows_dev || !spans_dev || !aligned16(rows_dev) || B < 1 || C < 1 || Nmax < 1 || W < B || R < W ||
+      Lw < 2 || overlap < 1 || overlap > Lw / 2)
+    return fail(EZB_ERR_ARG, "ezb_timeline_blend: bad argument");
+  EZB_CUDA(cudaSetDevice(device));
+  ++launch_counter();
+  EZB_CUDA(timeline_blend_launch(ST(stream), TimelinePlan{WindowPlan{plan_dev, B, C, Nmax, W, Lw, overlap}, rows_dev, spans_dev, R}, windows, out));
   return EZB_OK;
 }
 

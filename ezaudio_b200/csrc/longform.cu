@@ -4,25 +4,6 @@
 
 namespace ezb {
 
-struct ClipWindows { int first, count, n, len; };   // len: frames of each window (Lw, or N when the clip is one short window)
-
-__device__ __forceinline__ ClipWindows clip_windows(const WindowPlan& p, int b) {
-  const int32_t* e = p.plan + 3 * b;
-  const int n = min(max(e[2], 1), p.Nmax);
-  return ClipWindows{e[0], e[1], n, min(n, p.Lw)};
-}
-__device__ __forceinline__ int window_start(const WindowPlan& p, const ClipWindows& cw, int k) {
-  return k == cw.count - 1 ? cw.n - cw.len : k * (p.Lw - p.overlap);
-}
-// min(1, left, right), each ratio an IEEE division, as window_weights (inference.py) states it
-__device__ __forceinline__ float window_weight(const WindowPlan& p, const ClipWindows& cw, int k, int j) {
-  const float o1 = (float)(p.overlap + 1);
-  float w = 1.f;
-  if (k > 0) w = fminf(w, __fdiv_rn((float)(j + 1), o1));
-  if (k < cw.count - 1) w = fminf(w, __fdiv_rn((float)(p.Lw - j), o1));
-  return w;
-}
-
 __global__ void __launch_bounds__(256) window_gather_kernel(const WindowPlan p, const float* __restrict__ latents, float* __restrict__ windows) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.C * p.Lw) return;

@@ -16,6 +16,27 @@ namespace ezb {
 // first .. first + count - 1 of the W window rows.  Windows are (rows, C, Lw), long latents (B, C, Nmax).
 struct WindowPlan { const int32_t* plan; int B, C, Nmax, W, Lw, overlap; };
 
+// clip b's windows as the plan table gives them (n clamped to 1 .. Nmax), window k's start and its weight at local frame j; shared by the
+// linear kernels (longform.cu) and the timeline kernels (timeline.cu)
+struct ClipWindows { int first, count, n, len; };   // len: frames of each window (Lw, or N when the clip is one short window)
+
+__device__ __forceinline__ ClipWindows clip_windows(const WindowPlan& p, int b) {
+  const int32_t* e = p.plan + 3 * b;
+  const int n = min(max(e[2], 1), p.Nmax);
+  return ClipWindows{e[0], e[1], n, min(n, p.Lw)};
+}
+__device__ __forceinline__ int window_start(const WindowPlan& p, const ClipWindows& cw, int k) {
+  return k == cw.count - 1 ? cw.n - cw.len : k * (p.Lw - p.overlap);
+}
+// min(1, left, right), each ratio an IEEE division, as window_weights (inference.py) states it
+__device__ __forceinline__ float window_weight(const WindowPlan& p, const ClipWindows& cw, int k, int j) {
+  const float o1 = (float)(p.overlap + 1);
+  float w = 1.f;
+  if (k > 0) w = fminf(w, __fdiv_rn((float)(j + 1), o1));
+  if (k < cw.count - 1) w = fminf(w, __fdiv_rn((float)(p.Lw - j), o1));
+  return w;
+}
+
 // latents (B, C, Nmax) -> windows (copies * W, C, Lw): row r (and, when copies == 2, row W + r) holds its window's frames, zeros past them
 cudaError_t window_gather_launch(cudaStream_t st, const WindowPlan& p, const float* latents, float* windows, int copies);
 // windows (W, C, Lw) -> out (B, C, Nmax): the weighted mean of the windows covering each frame < N; frames >= N are not written

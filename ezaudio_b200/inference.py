@@ -17,6 +17,8 @@ Differences from the reference loop, all additive:
     operands (gt / gt_mask) whose window rows are cut once per call;
   * seamless loops (`sample_loop_latents`): the same windowed loop on a circle, the windows wrapping around the loop's end and shifting
     by a golden-ratio stride at every step (ezb_loop_gather / ezb_loop_blend).
+  * timelines of prompts (`sample_timeline_latents`): the windowed loop with one row per (window, prompt segment active in it), the rows of a
+    window sharing one unconditional row, each row's prediction weighted by its segment's weight (ezb_timeline_gather / _guide / _blend).
 The call still accepts `tokenizer` / `text_encoder` like the reference; pass `text_embeds=(emb, mask, uncond_emb,
 uncond_mask)` to use cached T5 outputs instead (BASELINE configs use cached embeddings).
 """
@@ -488,6 +490,104 @@ def check_loop(lengths, B: int, window: int, overlap: int, use_cfg: bool, max_ro
     return lens, table, windows
 
 
+def segment_weights(s: int, e: int, n: int, transition: int):
+    """fp32 weights of a timeline segment [s, e) over a clip of n frames with a transition of T frames: min(1, (f - s + T + 1) / (T + 1),
+    (e + T - f) / (T + 1)) on [s - T, e + T), 0 elsewhere, each ratio an IEEE fp32 division, as ezb_timeline_blend computes them.  1 inside
+    the segment, tapering over T frames on either side: abutting segments crossfade over 2T frames centred on their boundary."""
+    f = np.arange(n, dtype=np.int64)
+    t1 = np.float32(transition + 1)
+    a = np.minimum(np.float32(1), np.minimum((f - s + transition + 1).astype(np.float32) / t1, (e + transition - f).astype(np.float32) / t1))
+    a[(f < s - transition) | (f >= e + transition)] = 0
+    return a
+
+
+def timeline_plan(segments, lengths, window: int, overlap: int, transition: int):
+    """Rows of a batch of timelines: segments[b] lists clip b's [(s, e)] frame ranges in timeline order.  The windows are long_plan's; a
+    segment is active in a window when [s - T, e + T) meets it, and each (window, active segment) is one conditioned DiT row, clip by clip,
+    window by window, then in timeline order.  Returns (the plan table and windows of long_plan, the rows [(window, clip, segment index)],
+    the spans [(first row, row count)] per clip)."""
+    table, windows = long_plan(lengths, window, overlap)
+    rows, spans = [], []
+    for b, (first, count, _) in enumerate(table):
+        r0 = len(rows)
+        for k in range(first, first + count):
+            _, ws, ln = windows[k]
+            rows += [(k, b, q) for q, (s, e) in enumerate(segments[b]) if s - transition < ws + ln and e + transition > ws]
+        spans.append((r0, len(rows) - r0))
+    return table, windows, rows, spans
+
+
+def check_timeline(segments, lengths, B: int, window: int, overlap: int, transition: int, use_cfg: bool, max_rows: int, max_len: int):
+    """Validates a timeline run on the host before any device work: every segment non-empty and inside its clip, the segments of a clip
+    covering all of its frames, T >= 0, the window rules of check_long and the row capacity (the conditioned rows, plus one unconditional
+    row per window under CFG).  Returns (lengths, plan table, windows, rows, spans) as timeline_plan gives them."""
+    lens, _, _ = check_long(lengths, B, window, overlap, False, 1 << 62, max_len)   # the window rules; the capacity is checked below
+    if len(segments) != B:
+        raise ValueError(f"segments lists one timeline per clip: got {len(segments)} for {B} clips")
+    T = int(transition)
+    if T != transition or T < 0:
+        raise ValueError(f"transition must be a whole frame count >= 0, got {transition}")
+    segs = []
+    for b, (clip, n) in enumerate(zip(segments, lens)):
+        if len(clip) < 1:
+            raise ValueError(f"timeline {b} has no segment")
+        cover = np.zeros(n + 1, dtype=np.int64)
+        out = []
+        for s, e in clip:
+            if int(s) != s or int(e) != e or not 0 <= s < e <= n:
+                raise ValueError(f"timeline {b}: segment frames [{s}, {e}) must be whole, non-empty and inside the clip's {n} frames")
+            cover[int(s)] += 1
+            cover[int(e)] -= 1
+            out.append((int(s), int(e)))
+        gap = np.flatnonzero(np.cumsum(cover)[:n] == 0)
+        if gap.size:
+            raise ValueError(f"timeline {b}: no segment covers frame {int(gap[0])} (the segments must cover all {n} frames)")
+        segs.append(out)
+    table, windows, rows, spans = timeline_plan(segs, lens, int(window), int(overlap), T)
+    n_rows = len(rows) + (len(windows) if use_cfg else 0)
+    if n_rows > max_rows:
+        uncond = f" + {len(windows)} unconditional rows (CFG)" if use_cfg else ""
+        raise ValueError(f"{len(rows)} timeline rows{uncond} = {n_rows} DiT rows exceed the row capacity {max_rows} (2 * max_batch): "
+                         f"needs max_batch >= {-(-n_rows // 2)}")
+    return lens, table, windows, rows, spans
+
+
+@torch.no_grad()
+def sample_timeline_latents(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, segments, lengths, window, overlap, transition,
+                            guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, *, device=None, use_graphs=True):
+    """Long clips from a timeline of prompts: the windowed loop of sample_long_latents where window k of clip b carries one conditioned row
+    per segment active in it (timeline_plan) and, under guidance, all of them share the window's one unconditional row.  segments[b] lists
+    clip b's [(prompt, s, e)]: `prompt` a row of text (P, Lc, ctx) / text_mask (P, Lc), [s, e) its frames; `transition` (frames) the
+    taper T of segment_weights.  uncond_text / uncond_mask have one row, or one per clip.  At every step ezb_timeline_gather cuts the rows,
+    the DiT runs them as one batch, ezb_timeline_guide guides each conditioned row against its window's uncond row (the rescale's std over
+    one window), and ezb_timeline_blend weighs row r's prediction by its window's crossfade weight times its segment's weight, driving the
+    DDIM or DPM-Solver++ update of the long latent.  Returns the latents (B, C, max(lengths)) fp32 on the device, zero past each clip's end.
+    Seeds as in sample_long_latents.  The whole schedule is one captured graph; its tables are read on the device, so a replay follows new
+    boundaries, prompts and lengths with the same row layout.  A one-segment timeline is sample_long_latents with that prompt, bit for bit."""
+    B = len(segments)
+    use_cfg = bool(guidance_scale)
+    desc = unet._h.desc
+    frames = [[(s, e) for _, s, e in clip] for clip in segments]
+    lens, table, windows, rows, spans = check_timeline(frames, lengths, B, window, overlap, transition, use_cfg, int(desc.max_batch),
+                                                       int(desc.max_len))
+    P = text.shape[0]
+    prompt = [segments[b][q][0] for _, b, q in rows]
+    if any(int(p) != p or not 0 <= p < P for p in prompt):
+        raise ValueError(f"every segment's prompt must be a row index of text (0..{P - 1})")
+    T = int(transition)
+    tl = dict(rows=[(k, *frames[b][q], T) for k, b, q in rows], spans=spans, prompt=[int(p) for p in prompt])
+    dev_index = unet._h.dev_index
+    if device is not None:
+        d = torch.device(device)
+        if d.type != "cuda" or (d.index is not None and d.index != dev_index):
+            raise ValueError(f"sample_timeline_latents(device={d}) but the denoiser lives on cuda:{dev_index}")
+    device = torch.device("cuda", dev_index)
+    with torch.cuda.device(device):
+        return _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, int(window),
+                                      int(overlap), guidance_scale, guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs,
+                                      timeline=tl)
+
+
 @torch.no_grad()
 def sample_loop_latents(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lengths, window, overlap, guidance_scale,
                         guidance_rescale, ddim_steps, eta, random_seed, *, offsets=None, init_noise=None, step_noise=None, device=None,
@@ -597,12 +697,16 @@ def _guide_windows(out, guided, W, Cc, Lw, gs, gr, wlens):
 
 def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, uncond_mask, lens, table, windows, Lw, O, guidance_scale,
                            guidance_rescale, ddim_steps, eta, random_seed, device, use_graphs, controlnet=None, condition=None,
-                           conditioning_scale=1.0, gt=None, gt_mask=None, offsets=None, init_noise=None, step_noise=None):
+                           conditioning_scale=1.0, gt=None, gt_mask=None, offsets=None, init_noise=None, step_noise=None, timeline=None):
     """The windowed loop of sample_long_latents, and of sample_loop_latents when `offsets` ([steps][B] ints, the loops' shifts) is given:
     then the circular gather and blend (ezb_loop_gather / ezb_loop_blend) read step i's row of a device offsets table in place of the
-    linear ones, and the schedule is captured into a cache of its own.  init_noise / step_noise (loops only) replace the draws."""
-    B, W, N = text.shape[0], len(windows), max(lens)
-    loop = offsets is not None
+    linear ones, and the schedule is captured into a cache of its own.  init_noise / step_noise (loops only) replace the draws.
+    `timeline` (sample_timeline_latents: the rows [(window, s, e, T)], the spans [(first row, count)] per clip and the text row of every
+    conditioned row) switches the gather, the guidance and the blend to ezb_timeline_gather / _guide / _blend, with R conditioned rows and
+    one unconditional row per window under CFG, and a cache of its own."""
+    B, W, N = len(lens), len(windows), max(lens)
+    loop, tl = offsets is not None, timeline is not None
+    R = len(timeline["rows"]) if tl else W   # conditioned DiT rows
     Cc = unet.cfg["out_chans"]
     use_cfg = bool(guidance_scale)
     if gt is not None:   # the mask as one byte per frame (B, N); checked before any RNG draw
@@ -619,10 +723,11 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
         else:
             latents[b, :, :lens[b]] = init_noise[b, :, :lens[b]].to(device=device, dtype=torch.float32)
 
-    # the T5 context of every window row: [text of each window | "" of each window]
+    # the T5 context of every window row: [text of each window | "" of each window]; a timeline's rows take their segment's prompt
     clip_of = torch.tensor([b for b, _, _ in windows], device=device)
-    text = text.to(device=device, dtype=torch.float32)[clip_of]
-    text_mask = text_mask.to(device).bool()[clip_of]
+    text_of = torch.tensor(timeline["prompt"], device=device) if tl else clip_of
+    text = text.to(device=device, dtype=torch.float32)[text_of]
+    text_mask = text_mask.to(device).bool()[text_of]
     if use_cfg:
         if uncond_text.shape[0] == 1:
             uncond_text, uncond_mask = uncond_text.expand(B, -1, -1), uncond_mask.expand(B, -1)
@@ -647,11 +752,13 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
     sampler = (noise_scheduler.algorithm_type, noise_scheduler.solver_order) if dpm else ("ddim", float(eta or 0.0))
     key = (B, W, N, Lw, O, int(ctx.shape[1]), tuple(timesteps), use_cfg, float(guidance_scale or 0.0), float(guidance_rescale or 0.0), sampler,
            controlnet._h.serial if controlnet is not None else 0, float(conditioning_scale), int(_lib.lib().ezb_option_epoch()), gt is not None)
-    cache = unet.__dict__.setdefault("_loop_long_cache" if loop else "_long_cache", {})
+    if tl:   # the row layout; the row and span tables are read on the device
+        key = key + (("timeline", R),)
+    cache = unet.__dict__.setdefault("_loop_long_cache" if loop else "_timeline_cache" if tl else "_long_cache", {})
     st = cache.get(key) if use_graphs else None
     if st is None:
         st = dict(lat=torch.empty(B, Cc, N, device=device), x_in=torch.empty(Be, Cc, Lw, device=device), out=torch.empty(Be, Cc, Lw, device=device),
-                  guided=torch.zeros(W, Cc, Lw, device=device) if use_cfg else None, v=torch.empty(B, Cc, N, device=device),
+                  guided=torch.zeros(R, Cc, Lw, device=device) if use_cfg else None, v=torch.empty(B, Cc, N, device=device),
                   noise=torch.zeros(nsteps, B, Cc, N, device=device) if draw else None,
                   hist=torch.empty(B, Cc, N, device=device) if dpm else None,
                   plan=torch.empty(B * 3, device=device, dtype=torch.int32), wlens=torch.empty(Be, device=device, dtype=torch.int32),
@@ -659,7 +766,9 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
                   skips=None if controlnet is None else [torch.empty(Be, Lw, unet.cfg["embed_dim"], device=device) for _ in range(controlnet.half)],
                   gt=None if gt is None else torch.empty(Be, Cc, Lw, device=device),
                   m8=None if gt is None else torch.empty(Be, Lw, device=device, dtype=torch.uint8),
-                  offs=torch.empty(nsteps, B, device=device, dtype=torch.int32) if loop else None)
+                  offs=torch.empty(nsteps, B, device=device, dtype=torch.int32) if loop else None,
+                  rows=torch.empty(R * 4, device=device, dtype=torch.int32) if tl else None,
+                  spans=torch.empty(B * 2, device=device, dtype=torch.int32) if tl else None)
         if use_graphs:
             if len(cache) >= 2:
                 cache.clear()
@@ -674,7 +783,13 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
         idx = np.stack([np.where(j < ln, b * N + s + j, B * N) for b, s, ln in windows])
         src = torch.cat([m1.reshape(-1), torch.ones(1, device=device, dtype=torch.uint8)])
         st["m8"].copy_(src[torch.from_numpy(np.tile(idx, (Be // W, 1))).to(device)])
-    st["wlens"].copy_(torch.tensor([ln for _, _, ln in windows] * (Be // W), dtype=torch.int32))
+    if tl:   # read when the kernels run: a replayed graph follows new boundaries, transitions and prompts with the same rows
+        st["rows"].copy_(torch.tensor([e for row in timeline["rows"] for e in row], dtype=torch.int32))
+        st["spans"].copy_(torch.tensor([e for row in timeline["spans"] for e in row], dtype=torch.int32))
+        st["wlens"].copy_(torch.tensor([windows[row[0]][2] for row in timeline["rows"]] + ([ln for _, _, ln in windows] if use_cfg else []),
+                                       dtype=torch.int32))
+    else:
+        st["wlens"].copy_(torch.tensor([ln for _, _, ln in windows] * (Be // W), dtype=torch.int32))
     st["lens"].copy_(torch.tensor(lens, dtype=torch.int32))
     if loop:   # read when the kernels run: a replayed graph follows new offsets
         st["offs"].copy_(torch.tensor(offsets, dtype=torch.int32))
@@ -694,6 +809,9 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
         if loop:
             _lib.check(L_.ezb_loop_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), _lib.ptr(st["offs"][i]), B, Cc, N, W, Lw, O,
                                           Be // W, _lib.stream_ptr()))
+        elif tl:
+            _lib.check(L_.ezb_timeline_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), _lib.ptr(st["rows"]), B, Cc, N, W, R, Lw, O,
+                                              int(use_cfg), _lib.stream_ptr()))
         else:
             _lib.check(L_.ezb_window_gather(device.index, _lib.ptr(lat), _lib.ptr(x_in), _lib.ptr(plan), B, Cc, N, W, Lw, O, Be // W,
                                             _lib.stream_ptr()))
@@ -703,12 +821,19 @@ def _sample_long_on_device(unet, noise_scheduler, text, text_mask, uncond_text, 
             sk = controlnet.forward_step(x_in, i, conditioning_scale=conditioning_scale, outs=st["skips"])
             unet.forward_step(x_in, i, controlnet_skips=sk, out=out)
         src = out
-        if use_cfg:
+        if use_cfg and tl:
+            _lib.check(L_.ezb_timeline_guide(device.index, _lib.ptr(out), _lib.ptr(st["guided"]), _lib.ptr(st["rows"]), _lib.ptr(st["wlens"]), R, W,
+                                             Cc, Lw, gs, gr, _lib.stream_ptr()))
+            src = st["guided"]
+        elif use_cfg:
             _guide_windows(out, st["guided"], W, Cc, Lw, gs, gr, st["wlens"][:W])
             src = st["guided"]
         if loop:
             _lib.check(L_.ezb_loop_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), _lib.ptr(st["offs"][i]), B, Cc, N, W, Lw, O,
                                          _lib.stream_ptr()))
+        elif tl:
+            _lib.check(L_.ezb_timeline_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), _lib.ptr(st["rows"]), _lib.ptr(st["spans"]),
+                                             B, Cc, N, W, R, Lw, O, _lib.stream_ptr()))
         else:
             _lib.check(L_.ezb_window_blend(device.index, _lib.ptr(src), _lib.ptr(v), _lib.ptr(plan), B, Cc, N, W, Lw, O, _lib.stream_ptr()))
         nz = None if noise_all is None else noise_all[i]

@@ -9,7 +9,8 @@
  * must stay valid until the stream-ordered call has executed.  All work is enqueued on the cudaStream_t passed as
  * `stream` (void*).  The per-step entry points (set_context, set_context_rows, set_timesteps, forward, forward_tdev, controlnet_forward,
  * controlnet_set_condition, controlnet_set_condition_rows, controlnet_forward_tdev, controlnet_forward_cached,
- * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, window_gather, window_blend, loop_gather, loop_blend, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
+ * cfg_ddim_step, cfg_ddim_step_slots, cfg_dpm_step, cfg_dpm_step_slots, window_gather, window_blend, loop_gather, loop_blend,
+ * timeline_gather, timeline_guide, timeline_blend, decode, encode, encode_noised, energy_condition, t5_forward) never synchronise and are safe inside CUDA-graph capture; the load-time ones (create,
  * load_weight, finalize_weights) may synchronise the device.  A handle is not re-entrant.  Returns 0 on success,
  * a negative ezb_status otherwise; ezb_last_error() gives the message of the calling thread's last failure.
  */
@@ -198,6 +199,34 @@ int ezb_loop_gather(int device, const float* latents, float* windows, const int3
                     int W, int Lw, int overlap, int copies, void* stream);
 int ezb_loop_blend(int device, const float* windows, float* out, const int32_t* plan_dev, const int32_t* offsets_dev, int B, int C, int Nmax, int W,
                    int Lw, int overlap, void* stream);
+
+/* Timelines of prompts over long clips (MultiDiffusion's region-based generation on the time axis).  The clips are windowed as for
+ * ezb_window_gather (plan_dev: the same DEVICE int32 [B][3] table, W windows).  Every window carries one conditioned row per segment
+ * active in it, and under guidance all of them share the window's one unconditional row.
+ * rows_dev: DEVICE int32 [R][4], 16-byte aligned, = (window, s, e, T) per conditioned row, laid out clip by clip, window by window, then in
+ *   timeline order.  [s, e) are the segment's frames and T >= 0 its transition in frames.  Segment [s, e) weighs frame f by
+ *   a(f) = min(1, (f - s + T + 1) / (T + 1), (e + T - f) / (T + 1)) on [s - T, e + T) and 0 elsewhere, each ratio an IEEE fp32 division;
+ *   a segment is active in a window when [s - T, e + T) meets it.
+ * spans_dev: DEVICE int32 [B][2] = (first row, row count) per clip.
+ * The tables are read when the kernels run, so a captured graph follows new segment boundaries, transitions and clip lengths with the
+ * same R and W; validating them is the caller's job (ezaudio_b200.inference.timeline_plan builds them).
+ * ezb_timeline_gather: row r < R gets its window's frames of the long latents and zeros past the window's length; with uncond 1, row R + k
+ *   gets window k's the same way (the DiT input is then R + W rows).
+ * ezb_timeline_guide: model_out (R + W, C, Lw) -> guided (R, C, Lw).  Row r is guided against row R + window(r) over lens_dev[r] frames:
+ *   the bits ezb_cfg_ddim_step computes with coefficients (1, 0, 0, 1, 0), no noise and lens {lens_dev[r]} on the pair laid out as
+ *   [row r | row R + window(r)] (the same clusters, slices and double-precision reduction).  guided is that call's "latents" and must hold
+ *   finite values.  A row whose window lies outside 0 .. W - 1 is left untouched.
+ * ezb_timeline_blend: windows (R, C, Lw) -> out (B, C, Nmax).  Frame f < N_b of clip b gets sum w_k(j) a(f) v_r(j) / sum w_k(j) a(f) over
+ *   the rows of its span whose window k covers f (at local frame j, weight w_k as for ezb_window_blend) and whose a(f) > 0, in row order,
+ *   in fp32: the product w_k(j) * a(f) is rounded first, the first term starts both sums, the rest are fused multiply-adds and sums, and
+ *   the division is IEEE-rounded.  One covering row of weight 1 gives its value bit for bit, and a single segment covering the clip gives
+ *   ezb_window_blend's bits.  Row frames past a window's length and frames at or past N_b are neither read nor written. */
+int ezb_timeline_gather(int device, const float* latents, float* windows, const int32_t* plan_dev, const int32_t* rows_dev, int B, int C, int Nmax,
+                        int W, int R, int Lw, int overlap, int uncond, void* stream);
+int ezb_timeline_guide(int device, const float* model_out, float* guided, const int32_t* rows_dev, const int32_t* lens_dev, int R, int W, int C, int Lw,
+                       float gs, float gr, void* stream);
+int ezb_timeline_blend(int device, const float* windows, float* out, const int32_t* plan_dev, const int32_t* rows_dev, const int32_t* spans_dev,
+                       int B, int C, int Nmax, int W, int R, int Lw, int overlap, void* stream);
 
 /* --- VAE decoder: OobleckDecoder.forward (stable_vae/models/autoencoders.py:149-190) behind
  * Autoencoder(embedding=z) (src/modules/autoencoder_wrapper.py:74-77). */
